@@ -1,14 +1,13 @@
 #!/usr/bin/env python
-"""bench.py -- the driver's measurement contract for the libFM SGD hot path.
+"""bench.py -- throughput measurement of the libFM SGD hot path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1], the configuration `metric` is quoted on):
 SGD, k=8, MovieLens-1M-shaped CSR (6040 users x 3706 items, 1,000,209 rows,
 2 nnz/row, value 1), regression, lr 0.01, init_stdev 0.1.  A "step" is one pass
-of the hot path over the whole data set = one SGD epoch = one launch of
-fm_sgd_hogwild_kernel (plus, for N > 1, the per-epoch NCCL all-reduce of w0|w|V
-and the 1/N scale).  Weak scaling: every rank owns a full C2-sized row shard.
+of the hot path over the whole data set = one SGD epoch = one fmb200_sgd_epoch
+(plus, for N > 1, the per-epoch exchange of w0|w|V).  Weak scaling: every rank owns a full C2-sized row shard.
 
 value  : examples/s with inputs resident in HBM, CUDA events on the library's own
          stream, L2 flushed (256 MiB write) before every timed step, max over ranks.
@@ -20,6 +19,10 @@ parity : RMSE trajectory of the timed mode against the sequential oracle on a pl
          C2-shaped set from the same initial model (N == 1).
 tolerance_mode : the same workload in FMB200_MODE_ORDERED (sequentially consistent, fp64, inside
          the 1e-5 RMSE gate): examples/s device-timed and end to end, and its parity numbers.
+dump   : --dump-outputs DIR writes the model the timed path left after its last timed step, as a caller of
+         fmb200_get_params receives it: DIR/w0.npy, DIR/w.npy, DIR/v.npy (float64, v factor-major [k][n]).
+         Data and initial model are seeded and the C2 epoch is reproducible, so runs with the same arguments
+         write the same values.
 extra  : BASELINE configs C3 (k=64, 39 nnz/row, 1M features, 10M rows), C2 with Zipf(1) ids and C4 (the MCMC
          e-term pass, k=16, ML-10M shape), each with its own roofline object (N == 1; --no-extras skips them).
 """
@@ -228,25 +231,7 @@ def timed_epochs(lrn, data, steps, warmup, flush, stream, torch):
 
 
 def hbm_peak():
-    peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(peaks_path):
-        return float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def static_traffic(key, rows):
-    """ncu dram__bytes_read+write per launch from the committed capture (NOT a per-run measurement;
-    scaled by the row count when the captured launch covered fewer rows)."""
-    tp = os.path.join(ROOT, "profiles", "epoch_dram_bytes.json")
-    try:
-        ent = json.load(open(tp))[key]
-        scale = rows / ent["rows_per_launch"]
-        src = "static: " + ent["source"]
-        if abs(scale - 1.0) > 1e-9:
-            src += "; scaled x%.3g to this launch's rows" % scale
-        return ent["dram_bytes_per_launch"] * scale, src
-    except Exception:
-        return None, None
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 def kernel_name(cfg, mode):
@@ -263,7 +248,7 @@ def kernel_name(cfg, mode):
         cfg["lanes_per_row"], cfg["slots"], cfg["damp"], cfg["grid"], cfg["block"])
 
 
-def extra_config(name, data, k, task, device, steps, warmup, flush, stream, torch, traffic_key):
+def extra_config(name, data, k, task, device, steps, warmup, flush, stream, torch):
     """One more BASELINE config, device-timed, with its own roofline object."""
     from libfm_b200 import FmLearnSgdElement, FmModel, MODE_HOGWILD
     fm = FmModel(data.num_feature, k)
@@ -284,11 +269,10 @@ def extra_config(name, data, k, task, device, steps, warmup, flush, stream, torc
     z = data.num_values / data.num_cases
     bpe = 2 * k * z * 4
     achieved = data.num_cases * bpe / (ms * 1e-3) / 1e9
-    traffic, tsrc = static_traffic(traffic_key, data.num_cases)
     return {"workload": name, "rows": data.num_cases, "k": k, "nnz_per_row": z, "value": data.num_cases / (ms * 1e-3),
             "unit": UNIT, "ms_per_step": ms, "steps": steps, "gpu_launches": int(launches),
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "traffic_source": tsrc, "peak_source": peak_src,
+                         "traffic": None, "peak_source": peak_src,
                          "algorithmic_bytes_per_example": bpe, "kernel": kernel_name(cfg, "hogwild")},
             "kernel_geometry": cfg}
 
@@ -438,6 +422,23 @@ def extra_c5(world, rank, local_rank, dist, torch, flush, rows_total, steps=3):
             "kernel_geometry": cfg}
 
 
+def dump_model(lrn, out_dir):
+    """The parameters after the last timed step, as fmb200_get_params hands them to a caller."""
+    import ctypes as C
+    import numpy as np
+    n, k = lrn.fm.num_attribute, lrn.fm.num_factor
+    w0 = C.c_double()
+    w = np.empty(n, dtype=np.float64)
+    v = np.empty((k, n), dtype=np.float64)
+    P = lambda a: a.ctypes.data_as(C.POINTER(C.c_double))  # noqa: E731
+    if lrn.lib.fmb200_get_params(lrn._ctx, C.byref(w0), P(w), P(v)) != 0:
+        raise RuntimeError(lrn.lib.fmb200_last_error().decode())
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "w0.npy"), np.array([w0.value], dtype=np.float64))
+    np.save(os.path.join(out_dir, "w.npy"), w)
+    np.save(os.path.join(out_dir, "v.npy"), v)
+
+
 # --------------------------------------------------------------------------
 # the GPU arm
 # --------------------------------------------------------------------------
@@ -565,6 +566,8 @@ def run_gpu_arm(args):
         wall = time.perf_counter() - wall0
         barrier()
     launches = lrn.kernel_launches() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_model(lrn, args.dump_outputs)
     step_ms = [a.elapsed_time(b) for a, b in ev]
     total_ms = torch.tensor([sum(step_ms)], dtype=torch.float64, device="cuda")
     if world > 1:
@@ -712,11 +715,10 @@ def run_gpu_arm(args):
     # ---- roofline of the dominant kernel (the epoch kernel of the timed mode) ----------------
     peak, peak_src = hbm_peak()
     bytes_per_example = 2 * K_FACTORS * 2 * 4  # 2*k*nnz*4 (SURVEY.md section 8d)
-    kernel_ms = ms_per_step  # N == 1: the step is exactly one launch; N > 1: + the peer exchange kernel
+    kernel_ms = ms_per_step  # the epoch's launches; N > 1: + the peer exchange kernel
     achieved = rows * bytes_per_example / (kernel_ms * 1e-3) / 1e9
-    traffic, traffic_src = static_traffic("c2", rows)
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_src,
+                "frac": achieved / peak, "traffic": None,
                 "peak_source": peak_src, "algorithmic_bytes_per_example": bytes_per_example,
                 "kernel": kernel_name(cfg, "hogwild")}
 
@@ -731,13 +733,13 @@ def run_gpu_arm(args):
             try:
                 dz = synth.movielens_1m_shaped(seed=7, zipf=1.0)
                 extra["c2_zipf"] = extra_config("C2 with Zipf(1) user/item ids (hot-feature stress)", dz, K_FACTORS, 0,
-                                                local_rank, 10, 3, flush, stream, torch, "c2_zipf")
+                                                local_rank, 10, 3, flush, stream, torch)
                 del dz
                 d3 = synth.multi_field(args.c3_rows, 39, 1_000_000, 11)
                 d3.binarize_targets()
                 extra["c3"] = extra_config("C3: SGD k=64, Criteo-shaped CSR (1M features, 39 nnz/row, %d rows), "
                                            "-task c, Hogwild" % args.c3_rows, d3, 64, 1, local_rank, 5, 3, flush,
-                                           stream, torch, "c3")
+                                           stream, torch)
                 del d3
                 extra["c4"] = extra_c4(local_rank, args.c4_rows)
             except Exception as exc:  # an extra must never cost the headline line
@@ -795,7 +797,13 @@ def main():
     ap.add_argument("--c5-rows", type=int, default=100_000_000, help="total rows of C5 over all ranks")
     ap.add_argument("--collective", default="auto", choices=["auto", "p2p", "nccl"])
     ap.add_argument("--exchange", default="meanfield", choices=["meanfield", "mean"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the model after the last timed step as DIR/{w0,w,v}.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes what the GPU arm computed; the reference arm has nothing to dump")
     if args.impl == "reference":
         return run_reference_arm(args)
     return run_gpu_arm(args)

@@ -1,4 +1,4 @@
-/* fmb200.h -- C ABI of the B200-native libFM SGD hot path.
+/* fmb200.h -- C ABI of the H100-native libFM SGD hot path.
  *
  * The reference (srendle/libfm) has no plugin/FFI interface; its de-facto seam is
  * the fm_learn vtable (src/libfm/src/fm_learn.h:31-60) and the per-row calls
@@ -17,7 +17,7 @@
  *    whose fm_model carries mutable scratch, fm_model.h:65); distinct contexts
  *    may be driven from distinct threads/processes.
  *  - the library is CUDA-only: there is no CPU fallback.  fmb200_create fails
- *    loudly when no sm_100 device is usable.
+ *    loudly when no sm_90 device is usable.
  */
 #ifndef FMB200_H_
 #define FMB200_H_
@@ -36,8 +36,9 @@ typedef struct fmb200_ctx fmb200_ctx;
 /* execution modes of fmb200_sgd_epoch */
 #define FMB200_MODE_INORDER 0 /* sequential-equivalent: rows strictly in file order, fp64
                                  state; bit-compatible with fm_learn_sgd_element::learn */
-#define FMB200_MODE_HOGWILD 1 /* throughput: rows in parallel, fp32 state, red.global.add
-                                 write-back, damped per-tile bias step */
+#define FMB200_MODE_HOGWILD 1 /* throughput: rows in parallel, fp32 state, damped per-tile bias
+                                 step; rows of at most 4 entries with k <= 8 give the same
+                                 result on every run */
 
 #define FMB200_MODE_ORDERED 2 /* sequentially consistent: every example reads all parameters as
                                  the examples before it left them (the reference's order), fp64

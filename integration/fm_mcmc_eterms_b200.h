@@ -50,9 +50,9 @@ inline void b200_predict_data_and_write_to_eterms(fm_model* fm, DVector<Data*>& 
   std::vector<double> e;
   for (uint ds = 0; ds < main_data.dim; ds++) {
     Data* d = main_data(ds);
-    if (d->relation.dim != 0) throw "the B200 e-term pass does not handle relations";
+    if (d->relation.dim != 0) throw "the GPU e-term pass does not handle relations";
     LargeSparseMatrixMemory<DATA_FLOAT>* mem = dynamic_cast<LargeSparseMatrixMemory<DATA_FLOAT>*>(d->data);
-    if (mem == NULL) throw "the B200 e-term pass needs the row-major data in memory (text input)";
+    if (mem == NULL) throw "the GPU e-term pass needs the row-major data in memory (text input)";
     int slot = -1;
     for (size_t i = 0; i < slots.size(); i++)
       if (slots[i] == d) slot = (int)i;

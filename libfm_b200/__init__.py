@@ -1,4 +1,4 @@
-"""libfm_b200 -- the libFM SGD training hot path, rebuilt for B200 (sm_100a).
+"""libfm_b200 -- the libFM SGD training hot path, rebuilt for H100 (sm_90a).
 
 Scope: the per-example loop of srendle/libfm (`fm_model::predict` + `fm_SGD`
 driven by `fm_learn_sgd_element::learn`) as hand-written CUDA behind the C ABI

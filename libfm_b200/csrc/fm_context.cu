@@ -284,8 +284,8 @@ int fmb200_create(fmb200_ctx** out, int device, uint32_t n_attr, int num_factor,
   if (device < 0 || device >= count) return fail("device %d out of range (count %d)", device, count);
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10)
-    return fail("device %d is sm_%d%d; this library contains sm_100a code only", device, prop.major,
+  if (prop.major != 9 || prop.minor != 0)
+    return fail("device %d is sm_%d%d; this library contains sm_90a code only", device, prop.major,
                 prop.minor);
   fmb200_ctx* c = new (std::nothrow) fmb200_ctx();
   if (!c) return fail("out of host memory");
@@ -305,6 +305,7 @@ void fmb200_destroy(fmb200_ctx* c) {
   for (int q = 0; q < FMB200_MAX_PEERS; q++)
     if (c->peer_ipc[q] && c->peer_base[q]) cudaIpcCloseMemHandle(c->peer_base[q]);
   if (c->comm_base) cudaFree(c->comm_base);
+  if (c->d_acc) cudaFree(c->d_acc);
   if (c->p64.base) cudaFree(c->p64.base);
   if (c->sgda_grad_w) cudaFree(c->sgda_grad_w);
   if (c->sgda_grad_v) cudaFree(c->sgda_grad_v);
@@ -535,6 +536,8 @@ int fmb200_set_params(fmb200_ctx* c, double w0, const double* w, const double* v
       for (uint32_t i = 0; i < n; i++) hv32[(size_t)i * kp + f] = (float)v[(size_t)f * n + i];
     CK(cudaMemcpyAsync(c->p64.base, h64.data(), h64.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
     CK(cudaMemcpyAsync(c->p32.base, h32.data(), h32.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    // a fresh state: clear the divergence flag of the fixed-point accumulator (fm_rowlane.cu)
+    if (c->d_acc) CK(cudaMemsetAsync(c->d_acc + c->p32.n_floats, 0, sizeof(unsigned long long), c->stream));
     CK(cudaStreamSynchronize(c->stream));
     c->peer_base_valid = false;
     c->hogwild_fresh = true;

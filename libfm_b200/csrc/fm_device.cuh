@@ -1,4 +1,4 @@
-// fm_device.cuh -- sm_100a device-side primitives shared by the FM kernels:
+// fm_device.cuh -- sm_90a device-side primitives shared by the FM kernels:
 // mbarrier + 1-D TMA bulk copies (cp.async.bulk, SASS UBLKCP), L2-coherent
 // loads, vector reductions (red.global.add.v4.f32, SASS REDG.E.ADD.F32x4).
 #pragma once

@@ -1,4 +1,4 @@
-// fm_hogwild.cu -- the throughput SGD epoch (FMB200_MODE_HOGWILD), sm_100a.
+// fm_hogwild.cu -- the throughput SGD epoch (FMB200_MODE_HOGWILD), sm_90a.
 //
 // Replaces the row loop of fm_learn_sgd_element::learn (reference
 // src/libfm/src/fm_learn_sgd_element.h:56-67 = fm_model::predict, fm_model.h:105-127,
@@ -380,7 +380,7 @@ static HogwildArgs make_args(fmb200_ctx* c, const DataSlot& d, uint64_t n_tiles,
   a.feat_cnt = d.feat_cnt;
   a.conc_scale = 1.f;
   a.w0_conc = 1.f;
-  a.hot_thr = 3.0e38f;
+  a.acc_w0 = a.acc_w = a.acc_v = a.acc_bad = nullptr;
   a.sched = c->d_sched;
   a.global_entries = 0;
   return a;
@@ -412,8 +412,7 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, const DataSlot& d, bool* handle
                           : pick_rowlane_kernel(gp, (int)d.max_row_nnz, damp, combine);
   if (fn == nullptr) return cudaSuccess;
   const int hdr = ws ? 512 : HW_HDR_BYTES;
-  // COMBINE (non-WS): two 128-slot hot-feature tables of 64-byte entries behind the ring
-  const int smem_ws = hdr + HW_NSTAGE * (int)sbytes + ((combine && !ws) ? 2 * 128 * 64 : 0);
+  const int smem_ws = hdr + HW_NSTAGE * (int)sbytes;
   const int launch_threads = ws ? threads + 32 : threads;
   cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_ws);
   if (e != cudaSuccess) return e;
@@ -428,8 +427,6 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, const DataSlot& d, bool* handle
   a.conc_scale = (float)(std::min<double>((double)d.n_rows, (double)grid * TR) / (double)d.n_rows);
   // the warp-specialised kernel reads the bias when a stage is filled: HW_NSTAGE tiles ahead
   a.w0_conc = (float)std::min<double>((double)d.n_rows, (double)grid * TR * (ws ? HW_NSTAGE : 1));
-  // park a feature in the CTA's hot table when it is expected at least twice per tile
-  a.hot_thr = (float)std::max(4.0, 2.0 * (double)d.n_rows / (double)TR);
   // First epoch after the state was (re)set: the bias starts far from its equilibrium (w0 = 0 against a
   // target mean of ~3.5 on ratings) and a window of grid*TR rows would all be scored with that bias -- the
   // sequential loop corrects it within its first few hundred rows (fm_sgd.h:34-37: 1 - lr per row).  So
@@ -437,23 +434,63 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, const DataSlot& d, bool* handle
   // loop), the rest on the full grid.  Costs ~40 us once; the epoch-0 RMSE gap to the oracle drops by an
   // order of magnitude (DESIGN.md section 3.3).
   constexpr uint64_t kRampTiles = 4;
-  if (c->hogwild_fresh && c->k0 && c->tune_damp >= 0 && n_tiles > 8 * kRampTiles) {
-    HogwildArgs r = a;
-    r.n_rows = kRampTiles * (uint64_t)TR;
-    r.n_tiles = (uint32_t)kRampTiles;
-    r.conc_scale = (float)((double)TR / (double)d.n_rows);
-    r.w0_conc = (float)TR;
-    fn<<<1, launch_threads, smem_ws, c->stream>>>(r);
-    c->launches++;
-    const uint64_t skip = kRampTiles * (uint64_t)TR;  // a multiple of 32: TMA source alignment holds
-    a.row_ptr += skip;
-    a.target += skip;
-    a.n_rows -= skip;
-    a.n_tiles = (uint32_t)(n_tiles - kRampTiles);
-  }
+  const bool ramp = c->hogwild_fresh && c->k0 && c->tune_damp >= 0 && n_tiles > 8 * kRampTiles;
   c->hogwild_fresh = false;
-  fn<<<grid, launch_threads, smem_ws, c->stream>>>(a);
-  c->launches++;
+  if (ws) {
+    if (ramp) {
+      HogwildArgs r = a;
+      r.n_rows = kRampTiles * (uint64_t)TR;
+      r.n_tiles = (uint32_t)kRampTiles;
+      r.conc_scale = (float)((double)TR / (double)d.n_rows);
+      r.w0_conc = (float)TR;
+      fn<<<1, launch_threads, smem_ws, c->stream>>>(r);
+      c->launches++;
+      const uint64_t skip = kRampTiles * (uint64_t)TR;  // a multiple of 32: TMA source alignment holds
+      a.row_ptr += skip;
+      a.target += skip;
+      a.n_rows -= skip;
+      a.n_tiles = (uint32_t)(n_tiles - kRampTiles);
+    }
+    fn<<<grid, launch_threads, smem_ws, c->stream>>>(a);
+    c->launches++;
+  } else {
+    // The epoch as a sequence of launches of at most grid tiles each (the window of rows the
+    // free-running kernel has in flight); each launch reads the state the previous one left and
+    // its steps are folded in after it: the same result on every run.  A ramp launch is one tile.
+    const uint64_t n_acc = c->p32.n_floats;
+    if (c->d_acc == nullptr) {  // + the flag word of acc_add
+      e = cudaMalloc(&c->d_acc, (n_acc + 1) * sizeof(unsigned long long));
+      if (e != cudaSuccess) return e;
+      e = cudaMemsetAsync(c->d_acc, 0, (n_acc + 1) * sizeof(unsigned long long), c->stream);
+      if (e != cudaSuccess) return e;
+    }
+    float* base = c->p32.base;
+    a.acc_w0 = c->d_acc + (a.w0 - base);
+    a.acc_w = c->d_acc + (a.w - base);
+    a.acc_v = c->d_acc + (a.v - base);
+    a.acc_bad = c->d_acc + n_acc;
+    const int fold_grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((n_acc + 255) / 256, (uint64_t)c->sm_count * 4));
+    uint64_t t0 = 0;
+    while (t0 < n_tiles) {
+      const bool ramp_tile = ramp && t0 < kRampTiles;
+      const uint64_t nt = ramp_tile ? 1 : std::min<uint64_t>((uint64_t)grid, n_tiles - t0);
+      HogwildArgs w = a;
+      const uint64_t skip = t0 * (uint64_t)TR;  // a multiple of 32: TMA source alignment holds
+      w.row_ptr += skip;
+      w.target += skip;
+      w.n_rows = std::min<uint64_t>(nt * (uint64_t)TR, d.n_rows - skip);
+      w.n_tiles = (uint32_t)nt;
+      if (ramp_tile) {
+        w.conc_scale = (float)((double)TR / (double)d.n_rows);
+        w.w0_conc = (float)TR;
+      }
+      fn<<<(int)nt, launch_threads, smem_ws, c->stream>>>(w);
+      e = fold_acc(base, c->d_acc, n_acc, fold_grid, c->stream);
+      if (e != cudaSuccess) return e;
+      c->launches += 2;
+      t0 += nt;
+    }
+  }
   c->last_cfg = EpochConfig{1, (int)std::max<uint32_t>(1, d.max_row_nnz), TR, grid, launch_threads, smem_ws, damp ? 1 : 0};
   *handled = true;
   return cudaGetLastError();

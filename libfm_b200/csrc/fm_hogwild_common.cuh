@@ -32,11 +32,28 @@ struct HogwildArgs {
   const float* feat_cnt;  // occurrences of each feature in this data set (DAMP)
   float conc_scale;       // rows processed concurrently / n_rows: count -> concurrency
   float w0_conc;          // rows in flight w.r.t. the bias (tile granularity)
-  float hot_thr;          // COMBINE: occurrence count from which a feature is parked in the CTA's hot table
   unsigned int* sched;    // [0] next unclaimed tile, [1] CTAs that ran dry (both 0 between launches)
   int global_entries;     // rows too long for the staging ring: ids / values are read from global
                           // memory, only row offsets and targets are staged (tile_cap == 0)
+  // fm_sgd_rowlane_kernel: the steps of a launch accumulate here as fixed point (acc_add), element i
+  // beside element i of the packed state, and fold_acc adds them to the state after the launch
+  unsigned long long *acc_w0, *acc_w, *acc_v;
+  unsigned long long* acc_bad;  // set when a step was not finite or too large for the fixed point
 };
+
+// Fixed point of the accumulated steps: integer sums do not depend on the order in which the
+// reductions arrive, so an epoch built from such launches computes the same state on every run.
+// Resolution 2^-32; the int64 range holds sums up to 2^31.  A step that is not finite or not below
+// kAccStepMax (a diverging run) is not added but raises *bad, and fold_acc then turns the whole state
+// into NaN, as the free-running fp32 reductions would have spread it: with at most 2^20 rows per
+// launch the sums stay below 2^31.
+constexpr float kAccScale = 0x1p32f;
+constexpr float kAccStepMax = 0x1p11f;
+
+__device__ __forceinline__ void acc_add(unsigned long long* p, float d, unsigned long long* bad) {
+  if (fabsf(d) < kAccStepMax) atomicAdd(p, (unsigned long long)__float2ll_rn(d * kAccScale));
+  else atomicOr(bad, 1ull);  // also NaN: the comparison is false
+}
 
 __device__ __forceinline__ unsigned char* stage_base(unsigned char* smem, const HogwildArgs& a,
                                                      int stage) {
@@ -152,5 +169,8 @@ using HogwildKernelFn = void (*)(const HogwildArgs);
 HogwildKernelFn pick_rowlane_kernel(int gp, int max_row_nnz, bool damp, bool combine);
 // warp-specialised variant: blockDim = rows_per_tile + 32, smem header 512 B
 HogwildKernelFn pick_rowlane_ws_kernel(int gp, int max_row_nnz, bool damp, bool combine);
+// state[i] += acc[i] (fixed point), acc[i] = 0 for i < n: the end of one fm_sgd_rowlane_kernel launch.
+// acc[n] is the flag of acc_add: while it is set every state element becomes NaN.
+cudaError_t fold_acc(float* state, unsigned long long* acc, uint64_t n, int grid, cudaStream_t s);
 
 }  // namespace fmb

@@ -304,9 +304,8 @@ __device__ __forceinline__ void ord_store(double* p, const double (&v)[KF], int 
 // (fm_learn_sgd_element.h:58-62, fm_sgd.h:34-37) is affine in w0 once the example's clamp state (inside / at
 // min / at max) is fixed: w0' = a_t w0 + b_t.  Every example's own thread GUESSES its state from the bias at
 // the start of the run and publishes (a_t, b_t); warp 0 then walks  w <- fma(a_t, w, b_t)  -- one dependent
-// DFMA per example (8 cycles on B200), cut into segments that are composed in parallel (ord_bias_chain); the
-// Kogge-Stone scan over shuffles this replaces spent 270 dependent instructions, ~2 700 cycles, per run
-// (profiles/r02_ordered_v5_ncu_summary.md).  The examples' threads then check their guess against the bias they
+// DFMA per example, cut into segments that are composed in parallel (ord_bias_chain); the
+// Kogge-Stone scan over shuffles this replaces spent 270 dependent instructions per run.  The examples' threads then check their guess against the bias they
 // actually read, in parallel; the first contradicted one corrects its pair and the chain is walked again from
 // there (a consistent assignment IS the sequential answer, by induction over t; every pass finalises at least
 // one more example).
@@ -436,7 +435,7 @@ __device__ __forceinline__ void ord_tile_runs(const OrderedArgs& a, unsigned cha
   // entries a, b the score is  w_a + w_b + sum_f v_af v_bf  (1/2 ((a+b)^2 - a^2 - b^2) = ab) and the
   // gradient of v_af is mult v_bf  (sum_f - v_af = v_bf)  -- 10 fp64 operations per example instead of 64 for
   // the score, 52 instead of ~100 for the update; fp64 instruction issue is what phase A of a run spends its
-  // time on (profiles/r02_ordered_v6_ncu_summary.md)
+  // time on
   const bool oh = (ZF == 2) && onehot;
   const int gl = tid % GL;   // lane inside the example's group
   const int grp = tid / GL;  // example slot inside a run
@@ -957,8 +956,8 @@ __device__ __forceinline__ void ordered_epoch_body(const OrderedArgs& a, unsigne
 
 // ---- driver 2: warp-specialised.  The first `ncompute` threads walk the runs of tile T; the remaining
 // (helper) threads meanwhile write tile T-1's final records back to global memory and then fetch tile T+1's
-// records.  The v5 capture (profiles/r02_ordered_v5_ncu_summary.md) had the write-back loop at 19% and the
-// fetch issue at ~5% of all stall samples with every thread doing everything in sequence; both are LSU work a
+// records.  With every thread doing everything in sequence, the write-back loop and the fetch issue take a
+// share of the stall samples; both are LSU work a
 // single SM issues at about one 16-byte request per cycle, and neither is on the dependency chain.
 //
 // Order of the global traffic is the single-role driver's: the fetch of tile T+1 is issued behind tile T-1's

@@ -7,9 +7,8 @@
 // A warp therefore processes 32/E examples at once (k=64, 39 nnz/row: G=16, S=2,
 // one example per warp, two factor rows = four 128-byte lines per LDG.128).
 //
-// Two access patterns live side by side because the SM pays a ~25-cycle floor per
-// memory instruction no matter how few sectors it touches
-// (profiles/r01_red_microbench.txt):
+// Two access patterns live side by side because the SM pays a floor per memory
+// instruction no matter how few sectors it touches:
 //   * factor rows V[id,:]  -- chunk-parallel: lane (s,c) owns chunk c of the entries
 //     s, s+S, ...; the first R chunks stay in registers for the write-back.
 //   * linear weights w[id] -- ENTRY-parallel: lane l of the group owns the entries

@@ -5,8 +5,8 @@
 // "MovieLens" shape (BASELINE config C2: k=8, 2 nnz/row).  The sub-warp row-group
 // kernel spends ~30 warp instructions per example there (segmented shuffles,
 // per-lane address arithmetic replicated over 4 lanes per row); the measured
-// bound of the shape is the SM's L1TEX/LSU rate for scattered 32-byte sectors
-// (profiles/r01_red_microbench.txt), so everything else has to get out of the way.
+// bound of the shape is the SM's L1TEX/LSU rate for scattered 32-byte sectors,
+// so everything else has to get out of the way.
 //
 // Mapping
 //  * lane t of a CTA owns row t of the staged tile (rows_per_tile == blockDim.x);
@@ -17,9 +17,9 @@
 //    instruction; instead lane PAIRS (2j, 2j+1) co-operate: instruction A fetches
 //    the row of lane 2j (even lane low half, odd lane high half), instruction B the
 //    row of lane 2j+1, and one 4-float __shfl_xor swaps the halves into place.
-//    The write-back mirrors it (swap, then two red.global.add.v4.f32 whose lane
-//    pairs cover one full sector each).  Sector requests per (row, entry): 1 gather
-//    + 1 reduction for V, 1 + 1 for w -- the minimum for this layout.
+//    The write-back mirrors it: after the swap each lane owns half a sector of one
+//    row.  fm_sgd_rowlane_kernel adds it to the fixed-point accumulator (acc_add);
+//    the warp-specialised variant issues red.global.add.v4.f32 into the state.
 //  * GP == 1 (k <= 4): a factor row is a single float4; every lane fetches its own.
 #include <algorithm>
 
@@ -32,57 +32,15 @@ struct FactorRow {
   float v[4 * GP];
 };
 
-// CTA-level write combining for the hottest features of skewed data (COMBINE kernels).
-// Same-address L2 reductions serialise: a feature that appears in 11% of the rows costs
-// the whole chip ~4 ns per reduction.  After the in-warp merge, steps for features with
-// at least `hot_thr` occurrences are parked in a small direct-mapped shared-memory table
-// (tag = feature id) and leave the CTA as ONE reduction per feature and tile.  A slot that
-// is taken by another feature simply sends the step to L2 as before.
-constexpr int HOT_SLOTS = 128;
-struct HotEntry {
-  uint32_t tag;   // feature id, HOT_EMPTY when free
-  float dw;
-  float dv[8];
-  uint32_t pad[6];  // 64 bytes: one entry per pair of banks rows, no false sharing of tags
-};
-constexpr uint32_t HOT_EMPTY = 0xffffffffu;
-
-// returns true when the step was parked in the table
-template <int K>
-__device__ __forceinline__ bool hot_park(HotEntry* tab, uint32_t id, const float (&d)[K], float dw) {
-  HotEntry* e = tab + (id & (HOT_SLOTS - 1));
-  const uint32_t prev = atomicCAS(&e->tag, HOT_EMPTY, id);
-  if (prev != HOT_EMPTY && prev != id) return false;
-#pragma unroll
-  for (int f = 0; f < K; ++f) atomicAdd(&e->dv[f], d[f]);
-  atomicAdd(&e->dw, dw);
-  return true;
-}
-
-// flush one table: thread t handles slot t (call with t < HOT_SLOTS after a barrier)
-template <int GP>
-__device__ __forceinline__ void hot_flush(const HogwildArgs& a, HotEntry* tab, int t) {
-  HotEntry* e = tab + t;
-  const uint32_t id = e->tag;
-  if (id == HOT_EMPTY) return;
-  red_add_f4(a.v + (size_t)id * GP * 4, e->dv[0], e->dv[1], e->dv[2], e->dv[3]);
-  if (GP == 2) red_add_f4(a.v + (size_t)id * GP * 4 + 4, e->dv[4], e->dv[5], e->dv[6], e->dv[7]);
-  if (a.use_w) red_add_f(a.w + (size_t)id * a.ws, e->dw);
-  e->tag = HOT_EMPTY;
-  e->dw = 0.f;
-#pragma unroll
-  for (int f = 0; f < 8; ++f) e->dv[f] = 0.f;
-}
-
 // One tile, one lane per row: gather, score, multiplier, write-back.  `get_w0` is called
 // once the gathers are in flight and returns the tile's bias.  Returns this lane's loss
 // multiplier and joint curvature (zero for lanes without a row) for the bias step.
-template <int GP, int Z, bool DAMP, bool COMBINE, typename W0F>
+// ACC: the steps go to the fixed-point accumulator (a.acc_*) instead of the state.
+template <int GP, int Z, bool DAMP, bool COMBINE, bool ACC, typename W0F>
 __device__ __forceinline__ void rowlane_tile(const HogwildArgs& a, const uint64_t* rp,
                                              const float* ys, const uint32_t* ids,
                                              const float* xs, int rows_here, int tid, W0F get_w0,
-                                             float& mult_out, float& hjoint_out,
-                                             HotEntry* hot_tab = nullptr) {
+                                             float& mult_out, float& hjoint_out) {
   constexpr int K = 4 * GP;
   const int lane = tid & 31;
   const int odd = lane & 1;
@@ -231,10 +189,6 @@ __device__ __forceinline__ void rowlane_tile(const HogwildArgs& a, const uint64_
         }
         on_c = on && (lane == first);
       }
-      // hot features leave the CTA once per tile
-      if (hot_tab != nullptr && on_c && __ldg(a.feat_cnt + id[e]) >= a.hot_thr) {
-        if (hot_park<K>(hot_tab, id[e], d, dw)) on_c = false;
-      }
     }
     if (GP == 2) {
       // swap halves inside the lane pair so that each reduction covers a full sector
@@ -261,18 +215,38 @@ __device__ __forceinline__ void rowlane_tile(const HogwildArgs& a, const uint64_
       const float4 va = odd ? recv : keep;
       // row B (odd lane's): even writes the received low half, odd writes its high half
       const float4 vb = odd ? keep : recv;
-      if (onA) red_add_f4(a.v + ((size_t)idA * 2 + odd) * 4, va.x, va.y, va.z, va.w);
-      if (onB) red_add_f4(a.v + ((size_t)idB * 2 + odd) * 4, vb.x, vb.y, vb.z, vb.w);
-    } else {
-      if (on_c) red_add_f4(a.v + (size_t)id[e] * 4, d[0], d[1], d[2], d[3]);
+      if (ACC) {
+        unsigned long long* pa = a.acc_v + ((size_t)idA * 2 + odd) * 4;
+        unsigned long long* pb = a.acc_v + ((size_t)idB * 2 + odd) * 4;
+        if (onA) { acc_add(pa, va.x, a.acc_bad); acc_add(pa + 1, va.y, a.acc_bad); acc_add(pa + 2, va.z, a.acc_bad); acc_add(pa + 3, va.w, a.acc_bad); }
+        if (onB) { acc_add(pb, vb.x, a.acc_bad); acc_add(pb + 1, vb.y, a.acc_bad); acc_add(pb + 2, vb.z, a.acc_bad); acc_add(pb + 3, vb.w, a.acc_bad); }
+      } else {
+        if (onA) red_add_f4(a.v + ((size_t)idA * 2 + odd) * 4, va.x, va.y, va.z, va.w);
+        if (onB) red_add_f4(a.v + ((size_t)idB * 2 + odd) * 4, vb.x, vb.y, vb.z, vb.w);
+      }
+    } else if (on_c) {
+      if (ACC) {
+        unsigned long long* pv = a.acc_v + (size_t)id[e] * 4;
+#pragma unroll
+        for (int f = 0; f < 4; ++f) acc_add(pv + f, d[f], a.acc_bad);
+      } else {
+        red_add_f4(a.v + (size_t)id[e] * 4, d[0], d[1], d[2], d[3]);
+      }
     }
-    if (on_c && use_w) red_add_f(a.w + (size_t)id[e] * a.ws, dw);
+    if (on_c && use_w) {
+      if (ACC) acc_add(a.acc_w + (size_t)id[e] * a.ws, dw, a.acc_bad);
+      else red_add_f(a.w + (size_t)id[e] * a.ws, dw);
+    }
   }
 
   mult_out = mult;
   hjoint_out = valid ? hjoint : 0.f;
 }
 
+// Reads the state and accumulates its steps in a.acc_* (fold_acc applies them after the launch):
+// every row of a launch sees the state as the previous launch left it, whichever CTA runs it and
+// whenever, so the launch computes the same steps on every run.  The launcher sizes a launch to the
+// rows the free-running kernel would have in flight.
 template <int GP, int Z, bool DAMP, bool COMBINE>
 __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const HogwildArgs a) {
   constexpr int K = 4 * GP;
@@ -291,16 +265,6 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const
     fence_mbar_init();
   }
   if (tid == (int)blockDim.x - 32) policy = policy_evict_first();
-  // COMBINE: two hot-feature tables (ping-pong by tile parity) behind the staging ring
-  HotEntry* hot = reinterpret_cast<HotEntry*>(smem + HW_HDR_BYTES + (size_t)HW_NSTAGE * a.stage_bytes);
-  if (COMBINE) {
-    for (int i = tid; i < 2 * HOT_SLOTS; i += blockDim.x) {
-      hot[i].tag = HOT_EMPTY;
-      hot[i].dw = 0.f;
-#pragma unroll
-      for (int f = 0; f < 8; ++f) hot[i].dv[f] = 0.f;
-    }
-  }
   __syncthreads();
   uint32_t* s_tile = reinterpret_cast<uint32_t*>(smem + 208);  // [HW_NSTAGE] tile staged per stage
   TileSched sched{a.sched, a.n_tiles, false};
@@ -359,10 +323,9 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const
     const uint64_t ab = rp[0] & ~3ull;
 
     float mult, hj, w0 = 0.f;
-    rowlane_tile<GP, Z, DAMP, COMBINE>(
+    rowlane_tile<GP, Z, DAMP, COMBINE, true>(
         a, rp, ys, ids, xs, rows_here, tid,
-        [&]() { return w0 = bias.get(use_w0, tid, it, (int)blockDim.x); }, mult, hj,
-        COMBINE ? hot + (it & 1) * HOT_SLOTS : nullptr);
+        [&]() { return w0 = bias.get(use_w0, tid, it, (int)blockDim.x); }, mult, hj);
     // ---- bias: one damped reduction into the global w0 per tile ----
     float2* s_part = reinterpret_cast<float2*>(s_acc) + (it & 1) * 8;  // [2 slots][8 warps]
     if (use_w0) {
@@ -371,11 +334,6 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const
       if (lane == 0) s_part[tid >> 5] = make_float2(msum, hsum);
     }
     __syncthreads();
-    // this tile's hot table is complete: one reduction per parked feature, while the next
-    // tile already accumulates into the other table
-    if (COMBINE) {
-      for (int i = tid; i < HOT_SLOTS; i += blockDim.x) hot_flush<GP>(a, hot + (it & 1) * HOT_SLOTS, i);
-    }
     if (tid == ptid) {
       s_tile[stage] = nt;
       if (nt != HW_NO_TILE) issue_tile(a, smem, bars, nt, stage, policy, nt_nb, nt_ne);
@@ -388,11 +346,26 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const
         const float T = (float)rows_here;
         M += T * a.reg0 * w0;
         const float gsc = gamma_scale(fmaxf(a.w0_conc, 1.f), lr * (H / T + a.reg0));
-        red_add_f(a.w0, -lr * gsc * M);
+        acc_add(a.acc_w0, -lr * gsc * M, a.acc_bad);
       }
     }
   }
   if (tid == ptid) sched.finish(gridDim.x, claim_raw);
+}
+
+__global__ void fm_fold_acc_kernel(float* state, unsigned long long* acc, uint64_t n) {
+  const bool bad = acc[n] != 0ull;
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const long long q = (long long)acc[i];
+    if (bad) state[i] = __int_as_float(0x7fffffff);
+    else if (q != 0) state[i] += (float)((double)q * (1.0 / (double)kAccScale));
+    if (q != 0) acc[i] = 0ull;
+  }
+}
+
+cudaError_t fold_acc(float* state, unsigned long long* acc, uint64_t n, int grid, cudaStream_t s) {
+  fm_fold_acc_kernel<<<grid, 256, 0, s>>>(state, acc, n);
+  return cudaGetLastError();
 }
 
 // ---------------------------------------------------------------------------
@@ -504,7 +477,7 @@ __global__ void __launch_bounds__(HW_MAX_THREADS + 32, 3) fm_sgd_rowlane_ws_kern
     const int rows_here = (int)min((uint64_t)TR, a.n_rows - row0);
     const float w0 = s_w0[stage];
     float mult, hj;
-    rowlane_tile<GP, Z, DAMP, COMBINE>(a, rp, ys, ids, xs, rows_here, tid, [&]() { return w0; }, mult, hj);
+    rowlane_tile<GP, Z, DAMP, COMBINE, false>(a, rp, ys, ids, xs, rows_here, tid, [&]() { return w0; }, mult, hj);
     if (use_w0) {
       const float msum = warp_sum(mult);
       const float hsum = warp_sum(hj);

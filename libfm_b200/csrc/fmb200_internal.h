@@ -42,8 +42,7 @@ struct DataSlot {
 
 // Packed fp32 state: [w0, 0, 0, 0 | w[n*ws] padded to a multiple of 4 | V[n][kp]].
 // ws = stride of the linear weights in floats: 8 (one w per 32-byte sector) for small
-// tables, whose few lines otherwise serialise at L2 under load+reduction traffic
-// (profiles/r01_red_microbench.txt: 260 vs 128 cycles per load+RED pair at n=9746), else 1.
+// tables, whose few lines otherwise serialise at L2 under load+reduction traffic, else 1.
 struct Params32 {
   float* base = nullptr;
   uint64_t n_floats = 0;
@@ -104,6 +103,7 @@ struct fmb200_ctx {
   double* d_pred = nullptr;  // predict output staging
   uint64_t pred_cap = 0;
   unsigned int* d_sched = nullptr;   // hogwild tile scheduler: [next tile, CTAs run dry]
+  unsigned long long* d_acc = nullptr;  // fixed-point steps of one row-lane launch, beside p32 (zero between launches)
   unsigned int* d_flag = nullptr;    // 16 device words: upload-time inspection results
   unsigned int* h_flag = nullptr;    // pinned host mirror of d_flag
   void* h_stage = nullptr;           // pinned staging for set/get_params (small models)

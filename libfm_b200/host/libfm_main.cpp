@@ -1,4 +1,4 @@
-// libfm_main.cpp -- the drop-in `libFM` command line for the SGD path on B200.
+// libfm_main.cpp -- the drop-in `libFM` command line for the SGD path on H100.
 //
 // Keeps the reference's flags, defaults, stdout lines and file formats
 // (reference src/libfm/libfm.cpp:62-441) and swaps the learner for one whose
@@ -34,7 +34,7 @@ int main(int argc, char** argv) {
     CmdLine cmd(argc, argv);
     const char* bar = "----------------------------------------------------------------------------";
     std::cout << bar << std::endl;
-    std::cout << "libFM (libfm_b200: B200-native SGD path)" << std::endl;
+    std::cout << "libFM (libfm_b200: H100-native SGD path)" << std::endl;
     std::cout << "  CLI-compatible with libFM 1.4.4 for -method sgd; see INTEGRATION.md" << std::endl;
     std::cout << bar << std::endl;
 

@@ -195,7 +195,7 @@ class FmModel:
 
 
 class FmLearnSgdElement:
-    """fm_learn_sgd_element on a B200: one libfmb200 context (one GPU)."""
+    """fm_learn_sgd_element on an H100: one libfmb200 context (one GPU)."""
 
     def __init__(self, fm: FmModel, device: int = 0, mode: int = MODE_HOGWILD):
         self.lib = _capi.load()

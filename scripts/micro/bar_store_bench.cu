@@ -3,7 +3,7 @@
 // hundred cycles) showed half of its stall samples on barriers; this isolates the cause.
 //   one CTA of `threads`; per iteration: `nst` 16-byte global stores per thread to scattered rows, then a
 //   barrier; cycles per iteration by clock64.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o bar_store_bench bar_store_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o bar_store_bench bar_store_bench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <stdint.h>

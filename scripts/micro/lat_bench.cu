@@ -1,6 +1,6 @@
 // Latency microbenchmark for the ordered (sequentially-consistent) epoch kernel design:
 // dependent-chain latencies of the operations its per-run critical path is made of.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o lat_bench lat_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o lat_bench lat_bench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,9 +1,20 @@
-// Microbenchmark: cost model of fire-and-forget fp32 reductions (REDG) on B200.
+// Microbenchmark: cost model of fire-and-forget fp32 reductions (REDG).
 // Each warp issues NITER reduction instructions to pseudo-random rows of a table.
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+// the device's SM count and maximum SM clock, read in main(): the per-SM cycle figures are
+// wall time x clock x SMs / instructions
+static int g_sms = 0;
+static double g_hz = 0;
+static void read_device() {
+  int khz = 0;
+  cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, 0);
+  cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);
+  g_hz = khz * 1e3;
+}
 __device__ __forceinline__ void red4(float* p, float a) {
   asm volatile("red.relaxed.gpu.global.add.v4.f32 [%0], {%1,%1,%1,%1};" ::"l"(p), "f"(a) : "memory");
 }
@@ -55,16 +66,17 @@ void run(const char* name, float* tab, uint32_t rows32, int grid, int block, int
   cudaEventRecord(b); cudaEventSynchronize(b);
   float ms; cudaEventElapsedTime(&ms, a, b);
   double instr = (double)grid * (block / 32) * niter;
-  int sms = grid < 148 ? grid : 148;
-  printf("%-44s rows=%8u grid=%4d: %8.1f us  %7.2f G instr/s  %6.1f cyc/instr/SM(@1.9GHz)\n", name, rows32, grid, ms * 1e3,
-         instr / ms / 1e6, ms * 1e-3 * 1.9e9 * sms / instr);
+  int sms = grid < g_sms ? grid : g_sms;
+  printf("%-44s rows=%8u grid=%4d: %8.1f us  %7.2f G instr/s  %6.1f cyc/instr/SM\n", name, rows32, grid, ms * 1e3,
+         instr / ms / 1e6, ms * 1e-3 * g_hz * sms / instr);
 }
 int main() {
+  read_device();
   float *tab, *sink; size_t bytes = 512ull << 20;
   cudaMalloc(&tab, bytes); cudaMemset(tab, 0, bytes); cudaMalloc(&sink, 4);
   const int niter = 256, block = 256;
   for (uint32_t rows32 : {9746u, 82248u}) {
-    int grid = 148 * 4;
+    int grid = g_sms * 4;
     run<2>("scalar RED 32 lanes, 32B stride", tab, rows32, grid, block, niter, sink);
     run<8>("scalar RED 32 lanes, contiguous 4B", tab, rows32, grid, block, niter, sink);
     run<9>("scalar LD  32 lanes, contiguous 4B", tab, rows32, grid, block, niter, sink);

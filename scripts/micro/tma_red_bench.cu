@@ -7,11 +7,22 @@
 //   E  ld.global.cg.v4 lane pairs                                  (today's V gather)
 //   F  E and B interleaved (LSU gathers + TMA reductions: do they overlap?)
 //   G  E and A interleaved (today's mix)
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tma_red_bench tma_red_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tma_red_bench tma_red_bench.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+// the device's SM count and maximum SM clock, read in main(): the per-SM cycle figures are
+// wall time x clock x SMs / instructions
+static int g_sms = 0;
+static double g_hz = 0;
+static void read_device() {
+  int khz = 0;
+  cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, 0);
+  cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);
+  g_hz = khz * 1e3;
+}
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ uint32_t hash(uint32_t x) {
@@ -92,7 +103,7 @@ __global__ void __launch_bounds__(256) k(float* tab, uint32_t rows, int niter, f
 
 template <int MODE>
 void run(const char* name, float* tab, uint32_t rows, int rows_per_instr) {
-  const int grid = 148 * 4, block = 256, niter = 256;
+  const int grid = g_sms * 4, block = 256, niter = 256;
   cudaEvent_t a, b;
   cudaEventCreate(&a);
   cudaEventCreate(&b);
@@ -108,12 +119,13 @@ void run(const char* name, float* tab, uint32_t rows, int rows_per_instr) {
   const cudaError_t e = cudaGetLastError();
   const double instr = (double)grid * (block / 32) * niter;
   printf("%-58s %8.1f us  %6.1f cyc/warp-instr/SM  %5.2f cyc/row/SM  %s\n", name, ms * 1e3,
-         ms * 1e-3 * 1.9e9 * 148 / instr, ms * 1e-3 * 1.9e9 * 148 / instr / rows_per_instr,
+         ms * 1e-3 * g_hz * g_sms / instr, ms * 1e-3 * g_hz * g_sms / instr / rows_per_instr,
          e == cudaSuccess ? "" : cudaGetErrorString(e));
   cudaFree(sink);
 }
 
 int main() {
+  read_device();
   float* tab;
   const size_t bytes = 64ull << 20;
   cudaMalloc(&tab, bytes);

@@ -1,3 +1,4 @@
+import hashlib
 import os
 import sys
 
@@ -13,7 +14,7 @@ GOLDEN_CASES = sorted(f[:-4] for f in os.listdir(GOLDEN) if f.endswith(".npz"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); select with -m gpu")
 
 
 def load_golden(name):
@@ -23,6 +24,18 @@ def load_golden(name):
     tr = Data(z["tr_row_ptr"], z["tr_col"], z["tr_val"], z["tr_target"], n)
     te = Data(z["te_row_ptr"], z["te_col"], z["te_val"], z["te_target"], n)
     return z, tr, te
+
+
+def digest(a):
+    """SHA-256 of an array's bytes: how tests/golden/reference/outputs.npz stores large results."""
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+
+
+@pytest.fixture(scope="session")
+def ref_golden():
+    """What the reference computed for the inputs of the tests that compare against it
+    (scripts/make_ref_golden.py)."""
+    return np.load(os.path.join(GOLDEN, "reference", "outputs.npz"))
 
 
 @pytest.fixture(scope="session")

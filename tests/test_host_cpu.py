@@ -6,11 +6,9 @@ import sys
 import numpy as np
 import pytest
 
-from conftest import ROOT
+from conftest import ROOT, digest
 from libfm_b200 import Data, FmError, FmModel, synth
 from libfm_b200 import dist as fdist
-from oracle import Ref, have_ref
-from oracle.binding import REF_CLI
 
 TRICKY = """# a comment line
 5 0:1 7:0.5
@@ -29,13 +27,12 @@ def tricky_file(tmp_path):
     return str(p)
 
 
-@pytest.mark.skipif(not have_ref(), reason="oracle/_ref not built")
-def test_python_loader_matches_reference_loader(tricky_file):
-    rp, col, val, tgt, nf, mn, mx = Ref.load_data(tricky_file)
+def test_python_loader_matches_reference_loader(tricky_file, ref_golden):
+    g = ref_golden
     d = Data.load(tricky_file)
-    assert np.array_equal(d.row_ptr, rp) and np.array_equal(d.col, col)
-    assert np.array_equal(d.val, val) and np.array_equal(d.target, tgt)
-    assert d.num_feature == nf and d.min_target == mn and d.max_target == mx
+    assert np.array_equal(d.row_ptr, g["tricky_row_ptr"]) and np.array_equal(d.col, g["tricky_col"])
+    assert np.array_equal(d.val, g["tricky_val"]) and np.array_equal(d.target, g["tricky_target"])
+    assert [d.num_feature, d.min_target, d.max_target] == g["tricky_meta"].tolist()
 
 
 def test_python_loader_rejects_garbage(tmp_path):
@@ -47,46 +44,51 @@ def test_python_loader_rejects_garbage(tmp_path):
         Data.load(str(tmp_path / "missing"))
 
 
-@pytest.mark.skipif(not have_ref(), reason="oracle/_ref not built")
-def test_model_init_draw_order_bit_exact():
+def test_model_init_draw_order_bit_exact(ref_golden):
     fm = FmModel(37, 5)
     fm.init_stdev = 0.1
     fm.init(seed=42)
-    ref = Ref(37, 5, seed=42, init_stdev=0.1)
-    w0, w, v = ref.get_params()
-    assert fm.w0 == w0 and np.array_equal(fm.w, w) and np.array_equal(fm.v, v)
+    g = ref_golden
+    assert fm.w0 == g["init37_w0"] and np.array_equal(fm.w, g["init37_w"]) and np.array_equal(fm.v, g["init37_v"])
 
 
-@pytest.mark.skipif(not have_ref(), reason="oracle/_ref not built")
-def test_model_text_checkpoint_readable_by_reference(tmp_path):
+def checkpoint_model():
     fm = FmModel(12, 3)
     fm.init_stdev = 0.1
     fm.init(seed=3)
     fm.w0, fm.w[:] = 0.125, np.linspace(-1, 1, 12)
+    return fm
+
+
+def test_model_text_checkpoint_readable_by_reference(tmp_path, ref_golden):
+    """The reference's fm_model::loadModel of this checkpoint, and its saveModel afterwards (stored)."""
+    fm = checkpoint_model()
     path = str(tmp_path / "m.txt")
     fm.saveModel(path)
-    ref = Ref(12, 3, seed=1)
-    assert ref.load_model(path) == 1
-    w0, w, v = ref.get_params()
+    g = ref_golden
     g6 = lambda a: np.array([float("%g" % x) for x in np.ravel(a)]).reshape(np.shape(a))  # noqa: E731
-    assert w0 == 0.125 and np.array_equal(w, g6(fm.w)) and np.array_equal(v, g6(fm.v))
-    ref_path = str(tmp_path / "ref.txt")
-    ref.save_model(ref_path)
-    assert open(ref_path).read() == open(path).read()  # idempotent text form
+    assert g["ckpt_w0"] == 0.125 and np.array_equal(g["ckpt_w"], g6(fm.w)) and np.array_equal(g["ckpt_v"], g6(fm.v))
+    assert str(g["ckpt_text"]) == open(path).read()  # idempotent text form
 
 
-def test_cli_loader_lines_match_reference(tricky_file, tmp_path):
+def cli_loader_args(path):
+    return ["-task", "r", "-train", path, "-test", path, "-method", "sgd", "-iter", "0", "-learn_rate", "0.01",
+            "-seed", "1"]
+
+
+def loader_lines(stdout):
+    return [l for l in stdout.splitlines() if l.startswith("num_rows=") or l.startswith("has x")]
+
+
+def test_cli_loader_lines_match_reference(tricky_file, tmp_path, ref_golden):
     """bin/libFM parses its inputs before it needs a GPU: its loader summary lines must
     equal the reference CLI's, byte for byte."""
     cli = os.path.join(ROOT, "bin", "libFM")
-    if not (os.path.exists(cli) and os.path.exists(REF_CLI)):
+    if not os.path.exists(cli):
         pytest.skip("CLI binaries not built")
-    args = ["-task", "r", "-train", tricky_file, "-test", tricky_file, "-method", "sgd",
-            "-iter", "0", "-learn_rate", "0.01", "-seed", "1"]
-    ours = subprocess.run([cli] + args, capture_output=True, text=True)
-    ref = subprocess.run([REF_CLI] + args, capture_output=True, text=True)
-    pick = lambda s: [l for l in s.splitlines() if l.startswith("num_rows=") or l.startswith("has x")]  # noqa: E731
-    assert pick(ours.stdout) == pick(ref.stdout) and len(pick(ref.stdout)) == 6
+    ours = subprocess.run([cli] + cli_loader_args(tricky_file), capture_output=True, text=True)
+    want = ref_golden["cli_loader_lines"].tolist()
+    assert loader_lines(ours.stdout) == want and len(want) == 6
     import torch
     if not torch.cuda.is_available():
         assert ours.returncode != 0 and "no CPU path" in ours.stderr
@@ -250,13 +252,16 @@ def _read_dump(path):
     return rp, col, val, tgt, nf, float(mn), float(mx)
 
 
-@pytest.mark.skipif(not have_ref(), reason="oracle/_ref not built")
-def test_cli_loader_threaded_text_equals_reference(loader_dump, tmp_path):
-    """A > 1 MB text file takes the multi-threaded path of host/sparse_data.h (cut at
-    line boundaries, parsed by all cores, concatenated in file order): the CSR must be
-    bit-identical to what the reference's two-pass sscanf loader builds."""
+def _file_digest(path):
+    return digest(np.frombuffer(open(path, "rb").read(), np.uint8))
+
+
+def _csr_digest(csr):
+    return "".join(digest(a) for a in csr[:4])
+
+
+def write_threaded_input(path):
     r = np.random.default_rng(5)
-    path = str(tmp_path / "big.libfm")
     with open(path, "w") as f:
         f.write("# header comment\n\n")
         for i in range(60_000):
@@ -269,14 +274,21 @@ def test_cli_loader_threaded_text_equals_reference(loader_dump, tmp_path):
             if i % 1000 == 0:
                 f.write("\n# interleaved comment\n")
         f.write("4 7:1")  # last line without a newline
+
+
+def test_cli_loader_threaded_text_equals_reference(loader_dump, tmp_path, ref_golden):
+    """A > 1 MB text file takes the multi-threaded path of host/sparse_data.h (cut at
+    line boundaries, parsed by all cores, concatenated in file order): the CSR must be
+    bit-identical to what the reference's two-pass sscanf loader builds."""
+    path = str(tmp_path / "big.libfm")
+    write_threaded_input(path)
     assert os.path.getsize(path) > (1 << 20)
+    assert _file_digest(path) == ref_golden["threaded_input_sha"]  # the input the reference read
     out = str(tmp_path / "dump.bin")
     subprocess.run([loader_dump, path, out], check=True)
     got = _read_dump(out)
-    want = Ref.load_data(path)
-    for a, b in zip(got[:4], want[:4]):
-        assert np.array_equal(a, b)
-    assert got[4:] == (want[4], want[5], want[6])
+    assert _csr_digest(got) == ref_golden["threaded_csr_sha"]
+    assert list(got[4:]) == ref_golden["threaded_meta"].tolist()
 
 
 def test_cli_loader_reports_first_error_in_file_order(loader_dump, tmp_path):
@@ -288,30 +300,30 @@ def test_cli_loader_reports_first_error_in_file_order(loader_dump, tmp_path):
     assert r.returncode == 1 and 'cannot parse line "1 3:1 oops70000" at character o' in r.stderr
 
 
-def test_convert_tool_output_is_byte_identical_to_reference(tricky_file, tmp_path):
+def write_convert_input(path):
+    synth.to_libfm_text(synth.ragged(80_000, 3000, 6, seed=4), path)
+
+
+def test_convert_tool_output_is_byte_identical_to_reference(tricky_file, tmp_path, ref_golden):
     """bin/convert (host/convert_main.cpp) vs the reference's convert tool: same flags,
     byte-identical .x / .y files -- also on a file large enough for the threaded parser."""
-    from oracle.binding import REF_CONVERT
     ours = os.path.join(ROOT, "bin", "convert")
-    if not (os.path.exists(ours) and os.path.exists(REF_CONVERT)):
+    if not os.path.exists(ours):
         pytest.skip("convert binaries not built")
     big = str(tmp_path / "big.libfm")
-    synth.to_libfm_text(synth.ragged(80_000, 3000, 6, seed=4), big)
+    write_convert_input(big)
     assert os.path.getsize(big) > (1 << 20)
-    for src in (tricky_file, big):
-        for tool, tag in ((ours, "a"), (REF_CONVERT, "b")):
-            r = subprocess.run([tool, "--ifile", src, "--ofilex", str(tmp_path / (tag + ".x")),
-                                "--ofiley", str(tmp_path / (tag + ".y"))], capture_output=True, text=True)
-            assert os.path.exists(tmp_path / (tag + ".x")), r.stderr
-        assert open(tmp_path / "a.x", "rb").read() == open(tmp_path / "b.x", "rb").read()
-        assert open(tmp_path / "a.y", "rb").read() == open(tmp_path / "b.y", "rb").read()
+    assert _file_digest(big) == ref_golden["convert_big_input_sha"]
+    for tag, src in (("tricky", tricky_file), ("big", big)):
+        x, y = str(tmp_path / "a.x"), str(tmp_path / "a.y")
+        r = subprocess.run([ours, "--ifile", src, "--ofilex", x, "--ofiley", y], capture_output=True, text=True)
+        assert os.path.exists(x), r.stderr
+        assert _file_digest(x) + _file_digest(y) == ref_golden["convert_%s_sha" % tag]
 
 
-@pytest.mark.skipif(not have_ref(), reason="oracle/_ref not built")
-def test_cli_loader_fuzz_against_reference(loader_dump, tmp_path):
-    """Randomised libfm text (odd spacing, signs, exponents, comments, blank lines, empty
-    rows, garbage) through host/sparse_data.h and through the reference's Data::load:
-    identical CSR, or the same `cannot parse line` error."""
+def fuzz_inputs():
+    """40 randomised libfm texts (odd spacing, signs, exponents, comments, blank lines, empty rows,
+    every fourth with a garbage line)."""
     r = np.random.default_rng(2024)
 
     def num(x):
@@ -332,19 +344,26 @@ def test_cli_loader_fuzz_against_reference(loader_dump, tmp_path):
         lines = [line() for _ in range(int(r.integers(1, 60)))]
         if trial % 4 == 3:
             lines.insert(int(r.integers(0, len(lines) + 1)), str(r.choice(bad_tails)))
+        yield "\n".join(lines) + ("\n" if r.random() < 0.7 else "")
+
+
+def test_cli_loader_fuzz_against_reference(loader_dump, tmp_path, ref_golden):
+    """Randomised libfm text through host/sparse_data.h, against what the reference's Data::load
+    made of the same texts: identical CSR, or the same `cannot parse line` error."""
+    g = ref_golden
+    for trial, text in enumerate(fuzz_inputs()):
         path = str(tmp_path / ("f%d.libfm" % trial))
         with open(path, "w") as f:
-            f.write("\n".join(lines) + ("\n" if r.random() < 0.7 else ""))
+            f.write(text)
+        assert _file_digest(path) == g["fuzz_input_sha"][trial], trial  # the text the reference read
         out = str(tmp_path / "d.bin")
         ours = subprocess.run([loader_dump, path, out], capture_output=True, text=True)
-        try:
-            want = Ref.load_data(path)
-        except RuntimeError as e:
-            assert ours.returncode == 1, (trial, lines, str(e))
-            assert str(e).strip() in ours.stderr, (str(e), ours.stderr)
+        err = str(g["fuzz_error"][trial])
+        if err:
+            assert ours.returncode == 1, (trial, text, err)
+            assert err in ours.stderr, (err, ours.stderr)
             continue
-        assert ours.returncode == 0, (trial, ours.stderr, lines)
+        assert ours.returncode == 0, (trial, ours.stderr, text)
         got = _read_dump(out)
-        for a, b in zip(got[:4], want[:4]):
-            assert np.array_equal(a, b), (trial, lines)
-        assert got[4:] == (want[4], want[5], want[6]), (trial, got[4:], want[4:])
+        assert _csr_digest(got) == g["fuzz_csr_sha"][trial], (trial, text)
+        assert list(got[4:]) == g["fuzz_meta"][trial].tolist(), (trial, got[4:])

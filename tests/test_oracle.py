@@ -1,14 +1,14 @@
-"""CPU: pin the plain-C restatement (oracle/fm_oracle.c) against (a) the golden
-vectors the REFERENCE produced (tests/golden, scripts/make_golden.py) and
-(b) the reference itself when its shim is available (oracle/_ref)."""
+"""CPU: pin the plain-C restatement (oracle/fm_oracle.c) against what the REFERENCE
+produced: the golden vectors of tests/golden/*.npz (scripts/make_golden.py) and the
+reference's results stored in tests/golden/reference/outputs.npz (scripts/make_ref_golden.py)."""
 import ctypes as C
 
 import numpy as np
 import pytest
 
-from conftest import GOLDEN_CASES, load_golden
+from conftest import GOLDEN_CASES, digest, load_golden
 from libfm_b200 import synth
-from oracle import Port, Ref, have_ref
+from oracle import Port
 
 
 def _port_from_golden(z):
@@ -43,46 +43,37 @@ def test_port_epochs_bit_exact_vs_golden(name):
     assert np.array_equal(p.predict(te, task, mn, mx, True), z["pred_test"])
 
 
-@pytest.mark.skipif(not have_ref(), reason="oracle/_ref not built (no /root/reference)")
-def test_port_vs_live_reference_c1_shape():
+def test_port_vs_live_reference_c1_shape(ref_golden):
     tr = synth.plumbing_10k()
     te = synth.plumbing_10k(seed=99, n_rows=2000)
     n, k = max(tr.num_feature, te.num_feature), 8
-    ref = Ref(n, k, seed=42, init_stdev=0.1)
     port = Port(n, k)
     port.init(42, 0.0, 0.1)
-    ref.learn(tr, te, 0, 0.01, 2, tr.min_target, tr.max_target)
     for _ in range(2):
         port.sgd_epoch(tr, 0, 0.01, tr.min_target, tr.max_target)
-    w0, w, v = ref.get_params()
-    assert w0 == port.w0.value and np.array_equal(w, port.w) and np.array_equal(v, port.v)
-    assert ref.evaluate(te, 0, tr.min_target, tr.max_target) == port.metric(te, 0, tr.min_target, tr.max_target)
+    assert port.w0.value == ref_golden["c1_w0"]
+    assert digest(port.w) + digest(port.v) == ref_golden["c1_wv_sha"]
+    assert port.metric(te, 0, tr.min_target, tr.max_target) == ref_golden["c1_test_metric"]
 
 
-@pytest.mark.skipif(not have_ref(), reason="oracle/_ref not built (no /root/reference)")
-def test_port_rng_matches_reference():
-    L = Ref.lib()
+def test_port_rng_matches_reference(ref_golden):
     p = Port(1, 1)
-    L.ref_srand(C.c_long(123))
-    a = [L.ref_ran_gaussian() for _ in range(1000)]
     p.lib.fmo_srand(C.c_long(123))
     b = [p.lib.fmo_ran_gaussian() for _ in range(1000)]
-    assert a == b
+    assert b == ref_golden["rng_gauss_123"].tolist()
 
 
-@pytest.mark.skipif(not have_ref(), reason="oracle/_ref not built (no /root/reference)")
-def test_port_predict_row_edge_cases():
+PREDICT_ROW_CASES = [([], []), ([3], [2.5]), ([3, 3], [1.0, -2.0]), ([0, 19, 7], [0.5, 1.5, -1.0])]
+
+
+def test_port_predict_row_edge_cases(ref_golden):
     n, k = 20, 3
-    ref = Ref(n, k, seed=5)
-    w0, w, v = ref.get_params()
-    w = np.linspace(-1, 1, n)
-    ref.set_params(0.25, w, v)
     port = Port(n, k)
-    port.set_params(0.25, w, v)
-    for col, val in [([], []), ([3], [2.5]), ([3, 3], [1.0, -2.0]), ([0, 19, 7], [0.5, 1.5, -1.0])]:
-        pr, sr, ssr = ref.predict_row(col, val)
+    port.set_params(0.25, np.linspace(-1, 1, n), ref_golden["row_v"])
+    for i, (col, val) in enumerate(PREDICT_ROW_CASES):
         pp, sp, ssp = port.predict_row(col, val)
-        assert pr == pp and np.array_equal(sr, sp) and np.array_equal(ssr, ssp)
+        assert pp == ref_golden["row_p"][i]
+        assert np.array_equal(sp, ref_golden["row_s"][i]) and np.array_equal(ssp, ref_golden["row_ss"][i])
 
 
 def _ragged_short_rows(n_rows, n_feat, seed, dup_every=0):
@@ -156,13 +147,11 @@ def test_wavefront_schedule_refuses_ineligible_shapes():
     assert q.sgd_epoch_wavefront(synth.two_field(100, 50, 50, seed=1), 0, 0.01, 1.0, 5.0) == 0
 
 
-@pytest.mark.parametrize("case", ["ragged_unsorted_dups", "two_field", "no_linear", "k0_only"])
-def test_mcmc_eterm_port_is_bit_identical_to_reference(case):
-    """oracle/fm_oracle.c::fmo_mcmc_eterms against the reference's own e-term pass
-    (fm_learn_mcmc::predict_data_and_write_to_eterms, run through its transposed copy of the data)."""
-    from oracle import Ref, have_ref
-    if not have_ref():
-        pytest.skip("oracle/_ref not built")
+MCMC_CASES = ["ragged_unsorted_dups", "two_field", "no_linear", "k0_only"]
+
+
+def mcmc_case(case):
+    """data, n, k, k0, k1, w0, w of one e-term case"""
     k, k0, k1 = 6, 1, 1
     if case == "ragged_unsorted_dups":
         d = synth.ragged(4000, 300, 11, seed=31)   # unsorted ids, repeated ids inside rows, empty rows
@@ -176,26 +165,26 @@ def test_mcmc_eterm_port_is_bit_identical_to_reference(case):
         d = synth.ragged(2000, 200, 6, seed=34)
         k = 0
     n = d.num_feature
-    ref = Ref(n, k, k0, k1, seed=42, init_stdev=0.1)
-    _, _, v = ref.get_params()
     r = np.random.default_rng(5)
-    w0, w = 0.25, r.standard_normal(n) * 0.1
-    ref.set_params(w0, w, v)
+    return d, n, k, k0, k1, 0.25, r.standard_normal(n) * 0.1
+
+
+@pytest.mark.parametrize("case", MCMC_CASES)
+def test_mcmc_eterm_port_is_bit_identical_to_reference(case, ref_golden):
+    """oracle/fm_oracle.c::fmo_mcmc_eterms against the reference's own e-term pass
+    (fm_learn_mcmc::predict_data_and_write_to_eterms, run through its transposed copy of the data)."""
+    d, n, k, k0, k1, w0, w = mcmc_case(case)
     p = Port(n, k, k0, k1)
-    p.set_params(w0, w, v)
-    got, want = p.mcmc_eterms(d), ref.mcmc_eterms(d)
-    assert np.array_equal(got, want)
+    p.init(42, 0.0, 0.1)  # the reference's draw of V for seed 42
+    p.set_params(w0, w, p.v)
+    got = p.mcmc_eterms(d)
+    assert digest(got) == ref_golden["mcmc_%s_sha" % case]
     # same quantity as fm_model::predict, different association: equal to rounding only
     assert np.max(np.abs(got - p.predict(d, 0, 0, 0, transform=False))) < 1e-12
 
 
-@pytest.mark.parametrize("task", [0, 1])
-def test_sgda_port_is_bit_identical_to_reference(task):
-    """oracle/fm_oracle_sgda.c against the reference's own fm_learn_sgd_element_adapt_reg::learn
-    (4 epochs: the first without lambda-steps, validation cursor wrapping, two attribute groups)."""
-    from oracle import Ref, have_ref
-    if not have_ref():
-        pytest.skip("oracle/_ref not built")
+def sgda_case(task):
+    """train, validation, test, attribute groups, n, k, min/max target of one SGDA case"""
     full = synth.two_field(9000, 300, 200, seed=4, planted_k=3)
     tr, rest = synth.split_rows(full, 6000)
     va, te = synth.split_rows(rest, 2000)
@@ -204,16 +193,21 @@ def test_sgda_port_is_bit_identical_to_reference(task):
             d.target[:] = np.where(d.target > 3, 1.0, -1.0)
     n, k = full.num_feature, 5
     group = (np.arange(n) >= 300).astype(np.uint32)
-    mn, mx = float(tr.target.min()), float(tr.target.max())
-    ref = Ref(n, k, seed=42, init_stdev=0.1)
-    w0, w, v = ref.get_params()
+    return tr, va, te, group, n, k, float(tr.target.min()), float(tr.target.max())
+
+
+@pytest.mark.parametrize("task", [0, 1])
+def test_sgda_port_is_bit_identical_to_reference(task, ref_golden):
+    """oracle/fm_oracle_sgda.c against the reference's own fm_learn_sgd_element_adapt_reg::learn
+    (4 epochs: the first without lambda-steps, validation cursor wrapping, two attribute groups)."""
+    tr, va, te, group, n, k, mn, mx = sgda_case(task)
     p = Port(n, k)
-    p.set_params(w0, w, v)
+    p.init(42, 0.0, 0.1)  # the reference's initial model for seed 42
     p.sgda_begin(group)
-    reg_w, reg_v = ref.sgda_learn(tr, va, te, group, task, 0.02, 4, mn, mx)
     for e in range(4):
         p.sgda_epoch(tr, va, task, 0.02, mn, mx, e > 0)
-    a0, aw, av = ref.get_params()
-    assert a0 == p.w0.value and np.array_equal(aw, p.w) and np.array_equal(av, p.v)
+    assert p.w0.value == ref_golden["sgda%d_w0" % task]
+    assert digest(p.w) + digest(p.v) == ref_golden["sgda%d_wv_sha" % task]
+    reg_w, reg_v = ref_golden["sgda%d_reg_w" % task], ref_golden["sgda%d_reg_v" % task]
     assert np.array_equal(reg_w, p.reg_w) and np.array_equal(reg_v, p.reg_v)
     assert reg_w.max() > 0 and reg_v.max() > 0  # the lambda-steps did move the regularisation
