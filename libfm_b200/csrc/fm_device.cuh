@@ -97,6 +97,10 @@ __device__ __forceinline__ void red_add_f4(float* p, float a, float b, float c, 
 __device__ __forceinline__ void red_add_f(float* p, float a) {
   asm volatile("red.relaxed.gpu.global.add.f32 [%0], %1;" ::"l"(p), "f"(a) : "memory");
 }
+// atomicAdd on 64-bit integers compiles to ATOMG even when its result is unused
+__device__ __forceinline__ void red_add_u64(unsigned long long* p, unsigned long long a) {
+  asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(p), "l"(a) : "memory");
+}
 
 // named barrier 1: producer warp arrives (non-blocking), consumer warps sync
 __device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {

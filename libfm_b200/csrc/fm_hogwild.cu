@@ -380,7 +380,11 @@ static HogwildArgs make_args(fmb200_ctx* c, const DataSlot& d, uint64_t n_tiles,
   a.feat_cnt = d.feat_cnt;
   a.conc_scale = 1.f;
   a.w0_conc = 1.f;
-  a.acc_w0 = a.acc_w = a.acc_v = a.acc_bad = nullptr;
+  a.acc_w0 = a.acc_w = a.acc_v = a.acc_bad = a.acc = nullptr;
+  a.state = nullptr;
+  a.n_acc = 0;
+  a.ramp_tiles = 0;
+  a.ramp_conc_scale = a.ramp_w0_conc = 1.f;
   a.sched = c->d_sched;
   a.global_entries = 0;
   return a;
@@ -454,9 +458,9 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, const DataSlot& d, bool* handle
     fn<<<grid, launch_threads, smem_ws, c->stream>>>(a);
     c->launches++;
   } else {
-    // The epoch as a sequence of launches of at most grid tiles each (the window of rows the
-    // free-running kernel has in flight); each launch reads the state the previous one left and
-    // its steps are folded in after it: the same result on every run.  A ramp launch is one tile.
+    // The epoch as a sequence of windows of grid tiles each (the rows the free-running kernel has
+    // in flight), in one cooperative launch; each window reads the state the previous one left and
+    // its steps are folded in after it: the same result on every run.  A ramp window is one tile.
     const uint64_t n_acc = c->p32.n_floats;
     if (c->d_acc == nullptr) {  // + the flag word of acc_add
       e = cudaMalloc(&c->d_acc, (n_acc + 1) * sizeof(unsigned long long));
@@ -469,27 +473,21 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, const DataSlot& d, bool* handle
     a.acc_w = c->d_acc + (a.w - base);
     a.acc_v = c->d_acc + (a.v - base);
     a.acc_bad = c->d_acc + n_acc;
-    const int fold_grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((n_acc + 255) / 256, (uint64_t)c->sm_count * 4));
-    uint64_t t0 = 0;
-    while (t0 < n_tiles) {
-      const bool ramp_tile = ramp && t0 < kRampTiles;
-      const uint64_t nt = ramp_tile ? 1 : std::min<uint64_t>((uint64_t)grid, n_tiles - t0);
-      HogwildArgs w = a;
-      const uint64_t skip = t0 * (uint64_t)TR;  // a multiple of 32: TMA source alignment holds
-      w.row_ptr += skip;
-      w.target += skip;
-      w.n_rows = std::min<uint64_t>(nt * (uint64_t)TR, d.n_rows - skip);
-      w.n_tiles = (uint32_t)nt;
-      if (ramp_tile) {
-        w.conc_scale = (float)((double)TR / (double)d.n_rows);
-        w.w0_conc = (float)TR;
-      }
-      fn<<<(int)nt, launch_threads, smem_ws, c->stream>>>(w);
-      e = fold_acc(base, c->d_acc, n_acc, fold_grid, c->stream);
-      if (e != cudaSuccess) return e;
-      c->launches += 2;
-      t0 += nt;
+    a.state = base;
+    a.acc = c->d_acc;
+    a.n_acc = n_acc;
+    if (ramp) {
+      a.ramp_tiles = (uint32_t)kRampTiles;
+      a.ramp_conc_scale = (float)((double)TR / (double)d.n_rows);
+      a.ramp_w0_conc = (float)TR;
     }
+    // cooperative: the grid barriers between windows need every CTA resident; a grid that cannot be
+    // fails to launch instead of hanging (grid <= occ * SMs holds by construction)
+    void* args[] = {&a};
+    e = cudaLaunchCooperativeKernel((const void*)fn, dim3(grid), dim3(launch_threads), args, (size_t)smem_ws,
+                                    c->stream);
+    if (e != cudaSuccess) return e;
+    c->launches++;
   }
   c->last_cfg = EpochConfig{1, (int)std::max<uint32_t>(1, d.max_row_nnz), TR, grid, launch_threads, smem_ws, damp ? 1 : 0};
   *handled = true;

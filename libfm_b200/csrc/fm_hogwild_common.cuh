@@ -35,23 +35,29 @@ struct HogwildArgs {
   unsigned int* sched;    // [0] next unclaimed tile, [1] CTAs that ran dry (both 0 between launches)
   int global_entries;     // rows too long for the staging ring: ids / values are read from global
                           // memory, only row offsets and targets are staged (tile_cap == 0)
-  // fm_sgd_rowlane_kernel: the steps of a launch accumulate here as fixed point (acc_add), element i
-  // beside element i of the packed state, and fold_acc adds them to the state after the launch
+  // fm_sgd_rowlane_kernel: the steps of a window accumulate here as fixed point (acc_add), element i
+  // beside element i of the packed state, and are folded into the state after the window
   unsigned long long *acc_w0, *acc_w, *acc_v;
   unsigned long long* acc_bad;  // set when a step was not finite or too large for the fixed point
+  float* state;                 // the packed state [n_acc] ...
+  unsigned long long* acc;      // ... and its accumulator [n_acc + 1]; acc[n_acc] is acc_bad
+  uint64_t n_acc;
+  // fm_sgd_rowlane_kernel: the first ramp_tiles windows are one tile each, with these concurrencies
+  uint32_t ramp_tiles;
+  float ramp_conc_scale, ramp_w0_conc;
 };
 
 // Fixed point of the accumulated steps: integer sums do not depend on the order in which the
-// reductions arrive, so an epoch built from such launches computes the same state on every run.
+// reductions arrive, so an epoch built from such windows computes the same state on every run.
 // Resolution 2^-32; the int64 range holds sums up to 2^31.  A step that is not finite or not below
-// kAccStepMax (a diverging run) is not added but raises *bad, and fold_acc then turns the whole state
+// kAccStepMax (a diverging run) is not added but raises *bad, and the fold then turns the whole state
 // into NaN, as the free-running fp32 reductions would have spread it: with at most 2^20 rows per
-// launch the sums stay below 2^31.
+// window the sums stay below 2^31.
 constexpr float kAccScale = 0x1p32f;
 constexpr float kAccStepMax = 0x1p11f;
 
 __device__ __forceinline__ void acc_add(unsigned long long* p, float d, unsigned long long* bad) {
-  if (fabsf(d) < kAccStepMax) atomicAdd(p, (unsigned long long)__float2ll_rn(d * kAccScale));
+  if (fabsf(d) < kAccStepMax) red_add_u64(p, (unsigned long long)__float2ll_rn(d * kAccScale));
   else atomicOr(bad, 1ull);  // also NaN: the comparison is false
 }
 
@@ -165,12 +171,10 @@ struct TileSched {
 
 using HogwildKernelFn = void (*)(const HogwildArgs);
 
-// fm_rowlane.cu: kernel for (float4 chunks per row gp in {1,2}, rows of at most Z entries)
+// fm_rowlane.cu: kernel for (float4 chunks per row gp in {1,2}, rows of at most Z entries); a
+// cooperative launch whose grid size is the window size
 HogwildKernelFn pick_rowlane_kernel(int gp, int max_row_nnz, bool damp, bool combine);
 // warp-specialised variant: blockDim = rows_per_tile + 32, smem header 512 B
 HogwildKernelFn pick_rowlane_ws_kernel(int gp, int max_row_nnz, bool damp, bool combine);
-// state[i] += acc[i] (fixed point), acc[i] = 0 for i < n: the end of one fm_sgd_rowlane_kernel launch.
-// acc[n] is the flag of acc_add: while it is set every state element becomes NaN.
-cudaError_t fold_acc(float* state, unsigned long long* acc, uint64_t n, int grid, cudaStream_t s);
 
 }  // namespace fmb

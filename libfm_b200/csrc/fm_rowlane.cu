@@ -23,7 +23,11 @@
 //  * GP == 1 (k <= 4): a factor row is a single float4; every lane fetches its own.
 #include <algorithm>
 
+#include <cooperative_groups.h>
+
 #include "fm_hogwild_common.cuh"
+
+namespace cg = cooperative_groups;
 
 namespace fmb {
 
@@ -243,21 +247,33 @@ __device__ __forceinline__ void rowlane_tile(const HogwildArgs& a, const uint64_
   hjoint_out = valid ? hjoint : 0.f;
 }
 
-// Reads the state and accumulates its steps in a.acc_* (fold_acc applies them after the launch):
-// every row of a launch sees the state as the previous launch left it, whichever CTA runs it and
-// whenever, so the launch computes the same steps on every run.  The launcher sizes a launch to the
-// rows the free-running kernel would have in flight.
+// The whole epoch in one cooperative launch, as a sequence of windows separated by grid barriers.
+// Window j covers tiles [t0_j, t0_j + nt_j): the first a.ramp_tiles windows are one tile each (the
+// bias ramp, with its own concurrency a.ramp_*), every later one gridDim.x tiles (the rows the
+// free-running kernel has in flight), the last one what is left.  CTA b runs tile t0_j + b of each
+// window, if there is one.  A window reads the state and accumulates its steps in a.acc_*; after a
+// grid barrier every CTA folds its slice of the accumulator into the state, and after a second one
+// the next window starts.  So every row of a window sees the state as the previous window left it,
+// whichever CTA runs it and whenever, and the epoch computes the same state on every run.
+// Every CTA runs every window's barriers and fold, with or without a tile in it.
 template <int GP, int Z, bool DAMP, bool COMBINE>
 __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const HogwildArgs a) {
-  constexpr int K = 4 * GP;
   extern __shared__ __align__(128) unsigned char smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem);
   float* s_acc = reinterpret_cast<float*>(smem + 64);
+  cg::grid_group grid = cg::this_grid();
 
   const int tid = threadIdx.x;
   const int lane = tid & 31;
-  const int odd = lane & 1;
   const int TR = a.tile_rows;  // == blockDim.x
+  const uint32_t G = gridDim.x;
+  const uint32_t R = a.ramp_tiles;
+  const uint32_t n_win = R + (a.n_tiles - R + G - 1) / G;
+  // this CTA's tile of window j, or HW_NO_TILE
+  auto tile_of = [&](uint32_t j) -> uint32_t {
+    const uint32_t t = j < R ? (blockIdx.x == 0 ? j : HW_NO_TILE) : R + (j - R) * G + blockIdx.x;
+    return t < a.n_tiles ? t : HW_NO_TILE;
+  };
 
   uint64_t policy = 0;
   if (tid == 0) {
@@ -266,106 +282,108 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const
   }
   if (tid == (int)blockDim.x - 32) policy = policy_evict_first();
   __syncthreads();
-  uint32_t* s_tile = reinterpret_cast<uint32_t*>(smem + 208);  // [HW_NSTAGE] tile staged per stage
-  TileSched sched{a.sched, a.n_tiles, false};
-  // producer duties (tile claims, TMA issue, bias reduction) sit on lane 0 of the LAST
-  // warp; warp 0 fetches and publishes the bias -- nobody waits on the producer before
-  // the end-of-tile barrier
+  // producer duties (TMA issue, bias reduction) sit on lane 0 of the LAST warp; warp 0
+  // fetches and publishes the bias -- nobody waits on the producer before the end-of-tile
+  // barrier.  The CSR is read-only, so the producer stages this CTA's tiles of the coming
+  // windows HW_NSTAGE tiles ahead, across the window barriers.
   const int ptid = (int)blockDim.x - 32;
-  uint32_t claim_raw = HW_NO_TILE;  // producer: a claim in flight (resolved one tile later)
+  uint32_t pj = 0;  // producer: the next window whose tile is not staged yet
+  auto next_tile = [&]() -> uint32_t {
+    for (; pj < n_win; ++pj)
+      if (tile_of(pj) != HW_NO_TILE) return tile_of(pj++);
+    return HW_NO_TILE;
+  };
   if (tid == ptid) {
     for (int i = 0; i < HW_NSTAGE; i++) {
-      const uint32_t t = sched.claim();
-      s_tile[i] = t;
+      const uint32_t t = next_tile();
       if (t != HW_NO_TILE) {
         const uint64_t r0 = (uint64_t)t * TR, r1 = min(r0 + (uint64_t)TR, a.n_rows);
         issue_tile(a, smem, bars, t, i, policy, __ldg(a.row_ptr + r0), __ldg(a.row_ptr + r1));
       }
     }
-    claim_raw = sched.fire();
   }
   __syncthreads();
 
-  const float4* V4 = reinterpret_cast<const float4*>(a.v);
-  const bool use_w = a.use_w != 0;
   const bool use_w0 = a.use_w0 != 0;
   const float lr = a.lr;
+  const uint64_t fold_stride = (uint64_t)G * blockDim.x;
 
-  int it = 0;
-  for (;; ++it) {
-    const int stage = it % HW_NSTAGE;
-    const uint32_t parity = (uint32_t)(it / HW_NSTAGE) & 1u;
-    const uint64_t tile = s_tile[stage];
-    if (tile == HW_NO_TILE) break;  // this CTA's claims ran dry
-    uint32_t nt = HW_NO_TILE;
-    uint64_t nt_nb = 0, nt_ne = 0;
-    if (tid == ptid) {
-      nt = sched.resolve(claim_raw);  // fired a tile ago: long since returned
-      claim_raw = sched.fire();       // not looked at before the next tile
-      if (nt != HW_NO_TILE) {
-        const uint64_t r0 = (uint64_t)nt * TR, r1 = min(r0 + (uint64_t)TR, a.n_rows);
-        nt_nb = __ldg(a.row_ptr + r0);
-        nt_ne = __ldg(a.row_ptr + r1);
-      }
-    }
-    BiasFetch bias;
-    bias.slot = reinterpret_cast<float*>(smem + 192);
-    bias.issue(a, use_w0, tid);
-    mbar_wait(bars + stage, parity);
-
-    unsigned char* sb = stage_base(smem, a, stage);
-    const uint64_t* rp = reinterpret_cast<const uint64_t*>(sb);
-    const float* ys = reinterpret_cast<const float*>(sb + (size_t)(TR + 2) * 8);
-    const uint32_t* ids = reinterpret_cast<const uint32_t*>(sb + (size_t)(TR + 2) * 8 + (size_t)TR * 4);
-    const float* xs = reinterpret_cast<const float*>(ids + a.tile_cap);
-    const uint64_t row0 = tile * (uint64_t)TR;
-    const int rows_here = (int)min((uint64_t)TR, a.n_rows - row0);
-    const uint64_t ab = rp[0] & ~3ull;
-
-    float mult, hj, w0 = 0.f;
-    rowlane_tile<GP, Z, DAMP, COMBINE, true>(
-        a, rp, ys, ids, xs, rows_here, tid,
-        [&]() { return w0 = bias.get(use_w0, tid, it, (int)blockDim.x); }, mult, hj);
-    // ---- bias: one damped reduction into the global w0 per tile ----
-    float2* s_part = reinterpret_cast<float2*>(s_acc) + (it & 1) * 8;  // [2 slots][8 warps]
-    if (use_w0) {
-      const float msum = warp_sum(mult);
-      const float hsum = warp_sum(hj);
-      if (lane == 0) s_part[tid >> 5] = make_float2(msum, hsum);
-    }
-    __syncthreads();
-    if (tid == ptid) {
-      s_tile[stage] = nt;
-      if (nt != HW_NO_TILE) issue_tile(a, smem, bars, nt, stage, policy, nt_nb, nt_ne);
-      if (use_w0) {
-        float M = 0.f, H = 0.f;
-        for (int i = 0; i < (int)(blockDim.x >> 5); i++) {
-          M += s_part[i].x;
-          H += s_part[i].y;
+  int it = 0;  // tiles this CTA has run
+  for (uint32_t j = 0; j < n_win; ++j) {
+    const uint32_t tile = tile_of(j);
+    if (tile != HW_NO_TILE) {
+      const int stage = it % HW_NSTAGE;
+      const uint32_t parity = (uint32_t)(it / HW_NSTAGE) & 1u;
+      // producer: fetch the entry range of the tile that will refill this stage now,
+      // so the two dependent global loads overlap this tile's compute
+      uint32_t nt = HW_NO_TILE;
+      uint64_t nt_nb = 0, nt_ne = 0;
+      if (tid == ptid) {
+        nt = next_tile();
+        if (nt != HW_NO_TILE) {
+          const uint64_t r0 = (uint64_t)nt * TR, r1 = min(r0 + (uint64_t)TR, a.n_rows);
+          nt_nb = __ldg(a.row_ptr + r0);
+          nt_ne = __ldg(a.row_ptr + r1);
         }
-        const float T = (float)rows_here;
-        M += T * a.reg0 * w0;
-        const float gsc = gamma_scale(fmaxf(a.w0_conc, 1.f), lr * (H / T + a.reg0));
-        acc_add(a.acc_w0, -lr * gsc * M, a.acc_bad);
       }
+      HogwildArgs w = a;  // the window's concurrency
+      if (j < R) {
+        w.conc_scale = a.ramp_conc_scale;
+        w.w0_conc = a.ramp_w0_conc;
+      }
+      BiasFetch bias;
+      bias.slot = reinterpret_cast<float*>(smem + 192);
+      bias.issue(a, use_w0, tid);
+      mbar_wait(bars + stage, parity);
+
+      unsigned char* sb = stage_base(smem, a, stage);
+      const uint64_t* rp = reinterpret_cast<const uint64_t*>(sb);
+      const float* ys = reinterpret_cast<const float*>(sb + (size_t)(TR + 2) * 8);
+      const uint32_t* ids = reinterpret_cast<const uint32_t*>(sb + (size_t)(TR + 2) * 8 + (size_t)TR * 4);
+      const float* xs = reinterpret_cast<const float*>(ids + a.tile_cap);
+      const uint64_t row0 = (uint64_t)tile * TR;
+      const int rows_here = (int)min((uint64_t)TR, a.n_rows - row0);
+
+      float mult, hj, w0 = 0.f;
+      rowlane_tile<GP, Z, DAMP, COMBINE, true>(
+          w, rp, ys, ids, xs, rows_here, tid,
+          [&]() { return w0 = bias.get(use_w0, tid, it, (int)blockDim.x); }, mult, hj);
+      // ---- bias: one damped reduction into the global w0 per tile ----
+      float2* s_part = reinterpret_cast<float2*>(s_acc) + (it & 1) * 8;  // [2 slots][8 warps]
+      if (use_w0) {
+        const float msum = warp_sum(mult);
+        const float hsum = warp_sum(hj);
+        if (lane == 0) s_part[tid >> 5] = make_float2(msum, hsum);
+      }
+      __syncthreads();
+      if (tid == ptid) {
+        if (nt != HW_NO_TILE) issue_tile(a, smem, bars, nt, stage, policy, nt_nb, nt_ne);
+        if (use_w0) {
+          float M = 0.f, H = 0.f;
+          for (int i = 0; i < (int)(blockDim.x >> 5); i++) {
+            M += s_part[i].x;
+            H += s_part[i].y;
+          }
+          const float T = (float)rows_here;
+          M += T * a.reg0 * w0;
+          const float gsc = gamma_scale(fmaxf(w.w0_conc, 1.f), lr * (H / T + a.reg0));
+          acc_add(a.acc_w0, -lr * gsc * M, a.acc_bad);
+        }
+      }
+      ++it;
     }
+    grid.sync();  // every step of the window is in the accumulator
+    // ---- fold: state[i] += acc[i] (fixed point), acc[i] = 0; all NaN once a step overflowed ----
+    // acc and state through L2 (ld.global.cg): an L1 line from an earlier window would be stale
+    const bool bad = __ldcg(a.acc + a.n_acc) != 0ull;
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + tid; i < a.n_acc; i += fold_stride) {
+      const long long q = (long long)__ldcg(a.acc + i);
+      if (bad) a.state[i] = __int_as_float(0x7fffffff);
+      else if (q != 0) a.state[i] = __ldcg(a.state + i) + (float)((double)q * (1.0 / (double)kAccScale));
+      if (q != 0) a.acc[i] = 0ull;
+    }
+    if (j + 1 < n_win) grid.sync();  // the next window reads the folded state into a zero accumulator
   }
-  if (tid == ptid) sched.finish(gridDim.x, claim_raw);
-}
-
-__global__ void fm_fold_acc_kernel(float* state, unsigned long long* acc, uint64_t n) {
-  const bool bad = acc[n] != 0ull;
-  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-    const long long q = (long long)acc[i];
-    if (bad) state[i] = __int_as_float(0x7fffffff);
-    else if (q != 0) state[i] += (float)((double)q * (1.0 / (double)kAccScale));
-    if (q != 0) acc[i] = 0ull;
-  }
-}
-
-cudaError_t fold_acc(float* state, unsigned long long* acc, uint64_t n, int grid, cudaStream_t s) {
-  fm_fold_acc_kernel<<<grid, 256, 0, s>>>(state, acc, n);
-  return cudaGetLastError();
 }
 
 // ---------------------------------------------------------------------------
