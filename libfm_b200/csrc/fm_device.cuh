@@ -73,6 +73,29 @@ __device__ __forceinline__ uint64_t policy_evict_last() {
   return p;
 }
 
+// ---- TMA 1-D bulk reduction shared -> global (UBLKRED), per-thread bulk-group completion ----------
+// dst, src 16-byte aligned; bytes a non-zero multiple of 16.
+__device__ __forceinline__ void bulk_red_add_u64(unsigned long long* gdst, const void* smem_src, uint32_t bytes) {
+  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.u64 [%0], [%1], %2;" ::"l"(gdst),
+               "r"(smem_u32(smem_src)), "r"(bytes)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// all but the N most recent bulk groups of this thread have finished reading their shared-memory sources
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// every bulk group of this thread has completed its writes
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// order generic-proxy accesses against async-proxy (TMA) accesses of the same memory
+__device__ __forceinline__ void fence_proxy_async_shared() {
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+__device__ __forceinline__ void fence_proxy_async_global() {
+  asm volatile("fence.proxy.async.global;" ::: "memory");
+}
+
 // ---- cp.async (LDGSTS): 16-byte L2 -> shared copies, per-thread completion groups ---------
 __device__ __forceinline__ void cp_async_16(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");

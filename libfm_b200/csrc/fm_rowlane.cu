@@ -17,9 +17,11 @@
 //    instruction; instead lane PAIRS (2j, 2j+1) co-operate: instruction A fetches
 //    the row of lane 2j (even lane low half, odd lane high half), instruction B the
 //    row of lane 2j+1, and one 4-float __shfl_xor swaps the halves into place.
-//    The write-back mirrors it: after the swap each lane owns half a sector of one
-//    row.  fm_sgd_rowlane_kernel adds it to the fixed-point accumulator (acc_add);
-//    the warp-specialised variant issues red.global.add.v4.f32 into the state.
+//    The warp-specialised variant's write-back mirrors it: after the swap each lane
+//    owns half a sector of one row and issues red.global.add.v4.f32 into the state.
+//    fm_sgd_rowlane_kernel adds its steps to a fixed-point accumulator of u64 instead:
+//    each lane stages its whole quantised row in shared memory and issues one TMA bulk
+//    reduction for it (acc_add_row).
 //  * GP == 1 (k <= 4): a factor row is a single float4; every lane fetches its own.
 #include <algorithm>
 
@@ -35,6 +37,31 @@ template <int GP>
 struct FactorRow {
   float v[4 * GP];
 };
+
+// Adds the steps d[] of this lane's factor row (feature `id`, if `live`) to the fixed-point accumulator as
+// ONE bulk reduction (cp.reduce.async.bulk .add.u64, SASS UBLKRED) of the quantised row staged in shared
+// memory.  Scalar 64-bit reductions would take 4*GP instructions per row, each sending the L2 one 8-byte
+// request per lane, and the L2 charges per request more than per byte (DESIGN.md section 3.3).  Every
+// element is quantised by acc_quantise, the expression of acc_add, so the integer sums are the same.
+// Each lane owns two slots of s_wb and alternates them over the row's entries; a slot is rewritten only
+// once the bulk read of its previous contents is done.  The kernel waits for the writes before the
+// window's grid barrier.
+template <int GP, int Z>
+__device__ __forceinline__ void acc_add_row(unsigned long long* acc_v, uint32_t id, bool live,
+                                            const float (&d)[4 * GP], int e, int tid, unsigned long long* bad) {
+  constexpr int K = 4 * GP;
+  __shared__ __align__(128) unsigned long long s_wb[2][HW_MAX_THREADS][K];
+  unsigned long long* slot = s_wb[e & 1][tid];
+  bulk_wait_read<Z == 1 ? 0 : 1>();  // Z == 1 reuses slot 0 for every row
+  if (live) {
+#pragma unroll
+    for (int f = 0; f < K; f += 2)
+      *reinterpret_cast<ulonglong2*>(slot + f) = make_ulonglong2(acc_quantise(d[f], bad), acc_quantise(d[f + 1], bad));
+    fence_proxy_async_shared();  // the generic-proxy stores above, before the bulk read of the slot
+    bulk_red_add_u64(acc_v + (size_t)id * K, slot, K * 8);
+  }
+  bulk_commit();
+}
 
 // One tile, one lane per row: gather, score, multiplier, write-back.  `get_w0` is called
 // once the gathers are in flight and returns the tile's bias.  Returns this lane's loss
@@ -194,7 +221,9 @@ __device__ __forceinline__ void rowlane_tile(const HogwildArgs& a, const uint64_
         on_c = on && (lane == first);
       }
     }
-    if (GP == 2) {
+    if constexpr (ACC) {
+      acc_add_row<GP, Z>(a.acc_v, id[e], on_c, d, e, tid, a.acc_bad);
+    } else if (GP == 2) {
       // swap halves inside the lane pair so that each reduction covers a full sector
       const uint32_t pid = __shfl_xor_sync(0xffffffffu, id[e], 1);
       const bool pon = __shfl_xor_sync(0xffffffffu, (int)on_c, 1) != 0;
@@ -219,23 +248,10 @@ __device__ __forceinline__ void rowlane_tile(const HogwildArgs& a, const uint64_
       const float4 va = odd ? recv : keep;
       // row B (odd lane's): even writes the received low half, odd writes its high half
       const float4 vb = odd ? keep : recv;
-      if (ACC) {
-        unsigned long long* pa = a.acc_v + ((size_t)idA * 2 + odd) * 4;
-        unsigned long long* pb = a.acc_v + ((size_t)idB * 2 + odd) * 4;
-        if (onA) { acc_add(pa, va.x, a.acc_bad); acc_add(pa + 1, va.y, a.acc_bad); acc_add(pa + 2, va.z, a.acc_bad); acc_add(pa + 3, va.w, a.acc_bad); }
-        if (onB) { acc_add(pb, vb.x, a.acc_bad); acc_add(pb + 1, vb.y, a.acc_bad); acc_add(pb + 2, vb.z, a.acc_bad); acc_add(pb + 3, vb.w, a.acc_bad); }
-      } else {
-        if (onA) red_add_f4(a.v + ((size_t)idA * 2 + odd) * 4, va.x, va.y, va.z, va.w);
-        if (onB) red_add_f4(a.v + ((size_t)idB * 2 + odd) * 4, vb.x, vb.y, vb.z, vb.w);
-      }
+      if (onA) red_add_f4(a.v + ((size_t)idA * 2 + odd) * 4, va.x, va.y, va.z, va.w);
+      if (onB) red_add_f4(a.v + ((size_t)idB * 2 + odd) * 4, vb.x, vb.y, vb.z, vb.w);
     } else if (on_c) {
-      if (ACC) {
-        unsigned long long* pv = a.acc_v + (size_t)id[e] * 4;
-#pragma unroll
-        for (int f = 0; f < 4; ++f) acc_add(pv + f, d[f], a.acc_bad);
-      } else {
-        red_add_f4(a.v + (size_t)id[e] * 4, d[0], d[1], d[2], d[3]);
-      }
+      red_add_f4(a.v + (size_t)id[e] * 4, d[0], d[1], d[2], d[3]);
     }
     if (on_c && use_w) {
       if (ACC) acc_add(a.acc_w + (size_t)id[e] * a.ws, dw, a.acc_bad);
@@ -372,7 +388,11 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const
       }
       ++it;
     }
-    grid.sync();  // every step of the window is in the accumulator
+    // every step of the window is in the accumulator: the bulk reductions' writes are complete and,
+    // through the proxy fence, ordered before the barrier's release like the generic reductions
+    bulk_wait_all();
+    fence_proxy_async_global();
+    grid.sync();
     // ---- fold: state[i] += acc[i] (fixed point), acc[i] = 0; all NaN once a step overflowed ----
     // acc and state through L2 (ld.global.cg): an L1 line from an earlier window would be stale
     const bool bad = __ldcg(a.acc + a.n_acc) != 0ull;
@@ -383,6 +403,7 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const
       if (q != 0) a.acc[i] = 0ull;
     }
     if (j + 1 < n_win) grid.sync();  // the next window reads the folded state into a zero accumulator
+    fence_proxy_async_global();      // ... and its bulk reductions add to the fold's zeros
   }
 }
 

@@ -1,5 +1,7 @@
-// Microbenchmark: cost model of fire-and-forget fp32 reductions (REDG).
-// Each warp issues NITER reduction instructions to pseudo-random rows of a table.
+// Microbenchmark: cost model of fire-and-forget fp32 reductions (REDG), and of three write-back forms
+// of 64-byte records of 64-bit integers (REDG.E.ADD.64 scattered or sector-coalesced, UBLKRED).
+// Each warp issues NITER reduction instructions (or record write-backs) to pseudo-random rows of a table.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o red_bench red_bench.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
@@ -57,6 +59,70 @@ __global__ void k(float* tab, uint32_t rows32 /*number of 32B rows*/, int niter,
   }
   if (acc == 123.456f) *sink = acc;
 }
+// ---- 64-bit integer reductions into 64-byte records (8 x u64: a k=8 factor row of a fixed-point
+// accumulator).  Every lane writes back one record per iteration; the three forms differ in how:
+// mode 0: scattered, as after a lane-pair half swap: lanes 2j, 2j+1 share a record, lane 2j owns its
+//         low 32-byte sector, 2j+1 the high one; 4 scalar REDs per sector, 8 instructions for 2 records
+//         per lane pair, and every instruction touches 32 sectors with 8 bytes each
+// mode 1: sector-coalesced: the 4 lanes of a quad cover one 32-byte sector (4 x 8 B contiguous); the
+//         same 8 instructions per 32 records, each touching 8 full sectors
+// mode 2: bulk: one cp.reduce.async.bulk .add.u64 of the lane's 64-byte record from shared memory
+__device__ __forceinline__ void red_u64(unsigned long long* p, unsigned long long a) {
+  asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(p), "l"(a) : "memory");
+}
+__device__ __forceinline__ void bulk_red_u64(unsigned long long* g, const void* s, uint32_t bytes) {
+  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.u64 [%0], [%1], %2;" ::"l"(g),
+               "r"((uint32_t)__cvta_generic_to_shared(s)), "r"(bytes) : "memory");
+}
+template <int MODE>
+__global__ void __launch_bounds__(256) k64(unsigned long long* tab, uint32_t recs, int niter) {
+  __shared__ __align__(128) unsigned long long stage[256 * 8];  // 64 B per thread (mode 2)
+  const int tid = threadIdx.x, lane = tid & 31;
+  const uint32_t gw = (blockIdx.x * blockDim.x + tid) >> 5;
+  for (int i = 0; i < 8; i++) stage[tid * 8 + i] = 1ull;
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> bulk reads
+  __syncthreads();
+  for (int i = 0; i < niter; i++) {
+    const uint32_t base = hash(gw * 7919u + i * 104729u);
+    if (MODE == 0) {
+      const uint32_t ra = hash(base + (lane & ~1)) % recs, rb = hash(base + (lane | 1)) % recs;
+      unsigned long long* pa = tab + (size_t)ra * 8 + (lane & 1) * 4;
+      unsigned long long* pb = tab + (size_t)rb * 8 + (lane & 1) * 4;
+#pragma unroll
+      for (int e = 0; e < 4; e++) red_u64(pa + e, 1ull);
+#pragma unroll
+      for (int e = 0; e < 4; e++) red_u64(pb + e, 1ull);
+    }
+    if (MODE == 1) {
+#pragma unroll
+      for (int r = 0; r < 4; r++) {
+        const uint32_t rec = hash(base + ((lane & ~3) | r)) % recs;
+#pragma unroll
+        for (int h = 0; h < 2; h++) red_u64(tab + (size_t)rec * 8 + h * 4 + (lane & 3), 1ull);
+      }
+    }
+    if (MODE == 2) {
+      bulk_red_u64(tab + (size_t)(hash(base + lane) % recs) * 8, stage + tid * 8, 64);
+      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+      if ((i & 7) == 7) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+    }
+  }
+  if (MODE == 2) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+}
+template <int MODE>
+void run64(const char* name, unsigned long long* tab, uint32_t recs, int grid, int block, int niter) {
+  cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
+  k64<MODE><<<grid, block>>>(tab, recs, niter);
+  cudaEventRecord(a);
+  k64<MODE><<<grid, block>>>(tab, recs, niter);
+  cudaEventRecord(b); cudaEventSynchronize(b);
+  float ms; cudaEventElapsedTime(&ms, a, b);
+  const cudaError_t e = cudaGetLastError();
+  const double records = (double)grid * block * niter;
+  printf("%-44s recs=%6u grid=%4d: %8.1f us  %6.2f G records/s  %7.2f ps/record  %6.2f cyc/record/SM  %s\n", name,
+         recs, grid, ms * 1e3, records / ms / 1e6, ms * 1e9 / records, ms * 1e-3 * g_hz * g_sms / records,
+         e == cudaSuccess ? "" : cudaGetErrorString(e));
+}
 template <int MODE>
 void run(const char* name, float* tab, uint32_t rows32, int grid, int block, int niter, float* sink) {
   cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
@@ -84,6 +150,14 @@ int main() {
     run<11>("LD+RED same word, 32B stride", tab, rows32, grid, block, niter, sink);
     run<0>("v4 paired RED (16 sectors)", tab, rows32, grid, block, niter, sink);
     run<7>("v4 paired LD (16 sectors)", tab, rows32, grid, block, niter, sink);
+  }
+  // 64-byte u64 records of the k=8 accumulator; 9746 = the C2 feature count
+  unsigned long long* tab64 = reinterpret_cast<unsigned long long*>(tab);
+  for (uint32_t recs : {9746u, 82248u}) {
+    const int grid = g_sms * 4;
+    run64<0>("u64 (a) scattered, 8 REDs/record, 32 sectors", tab64, recs, grid, block, niter);
+    run64<1>("u64 (b) quad per sector, 8 REDs/record, 8 sec", tab64, recs, grid, block, niter);
+    run64<2>("u64 (c) bulk reduce, 64 B/record", tab64, recs, grid, block, niter);
   }
   return 0;
 }
