@@ -137,6 +137,37 @@ int fmb200_predict(fmb200_ctx* ctx, int slot, int transform, double* out);
  * Uses the fp64 state (INORDER / ORDERED mode): fmb200_set_params after every draw_all(). */
 int fmb200_mcmc_eterms(fmb200_ctx* ctx, int slot, double* e_out);
 
+/* Replaces: fm_learn_mcmc_simultaneous (fm_learn_mcmc.h, fm_learn_mcmc_simultaneous.h) on data sets without
+ * relations: -method mcmc (do_sample = do_multilevel = 1) and -method als (both 0).  The parameters, the
+ * hyperparameters, the NaN/Inf counters and the test predictions after every iteration are bit-identical to
+ * the reference's.  Uses the fp64 state (INORDER / ORDERED mode).
+ *  _begin:     fm_learn_mcmc::init + the prologue of _learn (:56-86).  The caller has set the model as
+ *              libfm.cpp:245-283 leaves it (fm.init(), then w ~ N(init_mean, init_stdev)), the task and
+ *              min/max_target (fmb200_set_hparams).  attr_group[n] (NULL: one group) and
+ *              attr_per_group[n_groups] (NULL: counted from attr_group) are DataMetaInfo's; reg0,
+ *              w_lambda[n_groups] and v_lambda[n_groups][num_factor] are what -regular sets
+ *              (libfm.cpp:326-364).  Builds the transposed training set and its feature runs.
+ *  _iteration: one pass of the iteration loop (:88-200): draw_all, re-prediction of train and test, the
+ *              test prediction sums and the target step.  The draws take libc rand() of the calling
+ *              process in the reference's order, so the caller seeds it with srand (libfm.cpp:115-116)
+ *              before initialising the model.  train_metric receives the RMSE (regression) or accuracy
+ *              (classification) the #Iter line prints as Train; counters[16] the NaN and Inf counts of
+ *              alpha, w0, w, v, w_mu, w_lambda, v_mu, v_lambda in that order.  One deviation: a sampled draw
+ *              the reference would skip without consuming a random number (posterior variance not finite
+ *              or zero, which only a diverged state gives) fails the call, naming the parameter and the
+ *              iteration, instead of desynchronising the random stream.
+ *  _get_hyper: alpha, w_mu[n_groups], w_lambda[n_groups], v_mu[n_groups][num_factor], v_lambda (any NULL).
+ *  _get_pred:  pred_this, pred_sum_all, pred_sum_all_but5 over the test set (any NULL).
+ *  _runs:      how many runs of conflict-free feature ids the sweep walks. */
+int fmb200_mcmc_begin(fmb200_ctx* ctx, int train_slot, int test_slot, int do_sample, int do_multilevel,
+                      uint32_t n_groups, const uint32_t* attr_group, const uint32_t* attr_per_group, double reg0,
+                      const double* w_lambda, const double* v_lambda);
+int fmb200_mcmc_iteration(fmb200_ctx* ctx, double* train_metric, uint32_t* counters);
+int fmb200_mcmc_get_hyper(fmb200_ctx* ctx, double* alpha, double* w_mu, double* w_lambda, double* v_mu,
+                          double* v_lambda);
+int fmb200_mcmc_get_pred(fmb200_ctx* ctx, double* pred_this, double* pred_sum_all, double* pred_sum_all_but5);
+int fmb200_mcmc_runs(fmb200_ctx* ctx, uint32_t* n_runs);
+
 /* Replaces: fm_learn_sgd_element_adapt_reg (SGDA, fm_learn_sgd_element_adapt_reg.h).
  *  _begin: init() + the prologue of learn() (:60-90, :281-292): stored gradients and the per-group
  *          regularisation values start at 0, fm->w is zeroed; attr_group[n] = DataMetaInfo::attr_group

@@ -46,6 +46,12 @@ SYMBOLS = {
     "fmb200_sgda_epoch": (C.c_int, [_ctx, C.c_int, C.c_int, C.c_int, _f64p]),
     "fmb200_sgda_get_reg": (C.c_int, [_ctx, _f64p, _f64p]),
     "fmb200_mcmc_eterms": (C.c_int, [_ctx, C.c_int, _f64p]),
+    "fmb200_mcmc_begin": (C.c_int, [_ctx, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint32, _u32p, _u32p, C.c_double,
+                                    _f64p, _f64p]),
+    "fmb200_mcmc_iteration": (C.c_int, [_ctx, _f64p, _u32p]),
+    "fmb200_mcmc_get_hyper": (C.c_int, [_ctx] + [_f64p] * 5),
+    "fmb200_mcmc_get_pred": (C.c_int, [_ctx] + [_f64p] * 3),
+    "fmb200_mcmc_runs": (C.c_int, [_ctx, _u32p]),
     "fmb200_params_device": (C.c_int, [_ctx, C.POINTER(C.c_void_p), _u64p]),
     "fmb200_scale_params": (C.c_int, [_ctx, C.c_double]),
     "fmb200_params_layout": (C.c_int, [_ctx, _u64p, _intp, _u64p, _intp]),

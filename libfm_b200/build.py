@@ -36,9 +36,10 @@ CU_SOURCES = {
     "fm_inorder.cu": ["--fmad=false"],
     "fm_ordered.cu": [],
     "fm_upload.cu": [],
+    "fm_mcmc.cu": ["--fmad=false"],
 }
 CU_HEADERS = ["fm_device.cuh", "fm_rowgroup.cuh", "fm_hogwild_common.cuh", "fmb200_internal.h",
-              "fm_inorder_wavefront.cuh", "fm_ordered.cuh"]
+              "fm_inorder_wavefront.cuh", "fm_ordered.cuh", "fm_roworder.cuh"]
 
 
 def _newer(target: str, deps: list[str]) -> bool:

@@ -312,6 +312,7 @@ void fmb200_destroy(fmb200_ctx* c) {
   if (c->sgda_reg_w) cudaFree(c->sgda_reg_w);
   if (c->sgda_reg_v) cudaFree(c->sgda_reg_v);
   if (c->sgda_group) cudaFree(c->sgda_group);
+  mcmc_free(c);
   if (c->d_partials) cudaFree(c->d_partials);
   if (c->d_pred) cudaFree(c->d_pred);
   if (c->d_sched) cudaFree(c->d_sched);
@@ -800,6 +801,64 @@ int fmb200_mcmc_eterms(fmb200_ctx* c, int slot, double* e_out) {
   CK(launch_mcmc_eterms(c, d, c->d_pred));
   CK(cudaMemcpyAsync(e_out, c->d_pred, d.n_rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+int fmb200_mcmc_begin(fmb200_ctx* c, int train_slot, int test_slot, int do_sample, int do_multilevel,
+                      uint32_t n_groups, const uint32_t* attr_group, const uint32_t* attr_per_group, double reg0,
+                      const double* w_lambda, const double* v_lambda) {
+  NEED_CTX(c);
+  if (need_slot(c, train_slot) || need_slot(c, test_slot)) return 1;
+  if (bind(c)) return 1;
+  if (c->mode == FMB200_MODE_HOGWILD)
+    return fail("MCMC / ALS run on the fp64 state: set INORDER or ORDERED mode first");
+  if (!w_lambda || (!v_lambda && c->k > 0)) return fail("null w_lambda / v_lambda");
+  if (c->peer_world > 1) return fail("MCMC / ALS run on one GPU: this context is attached to a multi-GPU peer world");
+  return guarded([&]() {
+    const std::string e = mcmc_begin(c, train_slot, test_slot, do_sample, do_multilevel, n_groups, attr_group,
+                                      attr_per_group, reg0, w_lambda, v_lambda);
+    if (!e.empty()) {
+      mcmc_free(c);
+      return fail("fmb200_mcmc_begin: %s", e.c_str());
+    }
+    return 0;
+  });
+}
+
+int fmb200_mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counters) {
+  NEED_CTX(c);
+  if (!c->mcmc) return fail("call fmb200_mcmc_begin first");
+  if (c->mode == FMB200_MODE_HOGWILD)
+    return fail("MCMC / ALS run on the fp64 state: set INORDER or ORDERED mode first");
+  if (bind(c)) return 1;
+  return guarded([&]() {
+    double m = 0.0;
+    const std::string e = mcmc_iteration(c, &m, counters);
+    if (!e.empty()) return fail("fmb200_mcmc_iteration: %s", e.c_str());
+    if (train_metric) *train_metric = m;
+    return 0;
+  });
+}
+
+int fmb200_mcmc_get_hyper(fmb200_ctx* c, double* alpha, double* w_mu, double* w_lambda, double* v_mu,
+                          double* v_lambda) {
+  NEED_CTX(c);
+  if (!mcmc_get(c, alpha, w_mu, w_lambda, v_mu, v_lambda, nullptr, nullptr, nullptr, nullptr))
+    return fail("call fmb200_mcmc_begin first");
+  return 0;
+}
+
+int fmb200_mcmc_get_pred(fmb200_ctx* c, double* pred_this, double* pred_sum_all, double* pred_sum_all_but5) {
+  NEED_CTX(c);
+  if (!mcmc_get(c, nullptr, nullptr, nullptr, nullptr, nullptr, pred_this, pred_sum_all, pred_sum_all_but5, nullptr))
+    return fail("call fmb200_mcmc_begin first");
+  return 0;
+}
+
+int fmb200_mcmc_runs(fmb200_ctx* c, uint32_t* n_runs) {
+  NEED_CTX(c);
+  if (!mcmc_get(c, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, n_runs))
+    return fail("call fmb200_mcmc_begin first");
   return 0;
 }
 

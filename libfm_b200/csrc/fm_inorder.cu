@@ -18,6 +18,7 @@
 #include "fm_device.cuh"
 #include "fmb200_internal.h"
 #include "fm_inorder_wavefront.cuh"
+#include "fm_roworder.cuh"
 
 namespace fmb {
 
@@ -256,49 +257,7 @@ __global__ void __launch_bounds__(256)
 // association than fm_model::predict:
 //   e = sum_f 0.5 q_f^2 ;  q = sum_f sum_i -0.5 v_if^2 x_i^2  (+ sum_i w_i x_i) ;  e = (e + q) + w0
 // One thread per case, every operation in that order (this TU is compiled with --fmad=false):
-// bit-identical e-terms.  Rows whose ids are not ascending are visited through a per-thread
-// order array (rows of <= ET_LOCAL entries) or by repeated selection (longer rows).
-constexpr int ET_LOCAL = 64;
-
-struct RowOrder {
-  const uint32_t* c;
-  uint32_t size;
-  bool sorted;
-  unsigned short ord[ET_LOCAL];
-  __device__ __forceinline__ void init(const uint32_t* col, uint32_t n) {
-    c = col;
-    size = n;
-    sorted = true;
-    for (uint32_t i = 1; i < n; i++)
-      if (col[i] < col[i - 1]) sorted = false;
-    if (!sorted && n <= (uint32_t)ET_LOCAL) {  // stable insertion sort by id
-      for (uint32_t i = 0; i < n; i++) ord[i] = (unsigned short)i;
-      for (uint32_t i = 1; i < n; i++) {
-        const unsigned short o = ord[i];
-        uint32_t j = i;
-        while (j > 0 && col[ord[j - 1]] > col[o]) {
-          ord[j] = ord[j - 1];
-          j--;
-        }
-        ord[j] = o;
-      }
-    }
-  }
-  // position of the i-th entry in (id, position) order; `prev` = position of the (i-1)-th
-  __device__ __forceinline__ uint32_t at(uint32_t i, uint32_t prev) const {
-    if (sorted) return i;
-    if (size <= (uint32_t)ET_LOCAL) return ord[i];
-    // selection: the smallest (id, position) greater than (c[prev], prev)
-    uint32_t best = 0xffffffffu;
-    for (uint32_t j = 0; j < size; j++) {
-      const bool after = (i == 0) || c[j] > c[prev] || (c[j] == c[prev] && j > prev);
-      if (!after) continue;
-      if (best == 0xffffffffu || c[j] < c[best]) best = j;
-    }
-    return best;
-  }
-};
-
+// bit-identical e-terms.  RowOrder (fm_roworder.cuh) gives that order for unsorted rows.
 __global__ void __launch_bounds__(128)
     fm_eterm64_kernel(Params64 p, int k, int use_w0, int use_w, uint64_t n_rows,
                       const uint64_t* __restrict__ row_ptr, const uint32_t* __restrict__ col,

@@ -160,7 +160,7 @@ int grid_for(const fmb200_ctx* c, uint64_t work) {
 }  // namespace
 
 // Build link[] / rowdep[] of a data set on c->stream (no host sync).
-cudaError_t build_ordered_links(fmb200_ctx* c, DataSlot& d) {
+cudaError_t build_ordered_links(fmb200_ctx* c, DataSlot& d, bool keep_scratch) {
   if (d.links_ready) return cudaSuccess;
   if (d.nnz >= 0xffffffffull) return cudaErrorInvalidValue;
   cudaError_t e;
@@ -207,7 +207,7 @@ cudaError_t build_ordered_links(fmb200_ctx* c, DataSlot& d) {
     ord_link_kernel<<<grid_for(c, d.nnz), 256, 0, c->stream>>>(ids, ent, d.nnz, d.row_ptr, d.n_rows, d.link, d.rowdep);
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     c->launches += 3;  // iota, link + the library's sort passes counted as one
-    if (d.nnz > (64ull << 20)) {
+    if (d.nnz > (64ull << 20) && !keep_scratch) {
       if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) return e;
       cudaFree(d.ord_scratch);
       d.ord_scratch = nullptr;

@@ -1,0 +1,52 @@
+// fm_roworder.cuh -- a case's entries in (feature id, position) order, the order in which the
+// MCMC / ALS learner reaches them through the transposed data (reference Data.h:292-341).
+// Shared by the e-term pass (fm_inorder.cu) and the q rebuild of the Gibbs sweep (fm_mcmc.cu).
+#pragma once
+#include <stdint.h>
+
+namespace fmb {
+
+// Rows whose ids are not ascending are visited through a per-thread order array (rows of
+// <= ET_LOCAL entries) or by repeated selection (longer rows).
+constexpr int ET_LOCAL = 64;
+
+struct RowOrder {
+  const uint32_t* c;
+  uint32_t size;
+  bool sorted;
+  unsigned short ord[ET_LOCAL];
+  __device__ __forceinline__ void init(const uint32_t* col, uint32_t n) {
+    c = col;
+    size = n;
+    sorted = true;
+    for (uint32_t i = 1; i < n; i++)
+      if (col[i] < col[i - 1]) sorted = false;
+    if (!sorted && n <= (uint32_t)ET_LOCAL) {  // stable insertion sort by id
+      for (uint32_t i = 0; i < n; i++) ord[i] = (unsigned short)i;
+      for (uint32_t i = 1; i < n; i++) {
+        const unsigned short o = ord[i];
+        uint32_t j = i;
+        while (j > 0 && col[ord[j - 1]] > col[o]) {
+          ord[j] = ord[j - 1];
+          j--;
+        }
+        ord[j] = o;
+      }
+    }
+  }
+  // position of the i-th entry in (id, position) order; `prev` = position of the (i-1)-th
+  __device__ __forceinline__ uint32_t at(uint32_t i, uint32_t prev) const {
+    if (sorted) return i;
+    if (size <= (uint32_t)ET_LOCAL) return ord[i];
+    // selection: the smallest (id, position) greater than (c[prev], prev)
+    uint32_t best = 0xffffffffu;
+    for (uint32_t j = 0; j < size; j++) {
+      const bool after = (i == 0) || c[j] > c[prev] || (c[j] == c[prev] && j > prev);
+      if (!after) continue;
+      if (best == 0xffffffffu || c[j] < c[best]) best = j;
+    }
+    return best;
+  }
+};
+
+}  // namespace fmb

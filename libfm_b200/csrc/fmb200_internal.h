@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <string>
+
 #include "../../include/fmb200.h"
 
 namespace fmb {
@@ -76,6 +78,8 @@ struct HParams {
 // (the sliced exchange needs world x grid entries)
 constexpr int FMB_PEER_PART = 4096;
 
+struct McmcState;  // fm_mcmc.cu
+
 struct EpochConfig {
   int lanes_per_row = 0, slots = 0, rows_per_tile = 0, grid = 0, block = 0, smem = 0, damp = 0;
 };
@@ -132,6 +136,7 @@ struct fmb200_ctx {
   uint32_t sgda_groups = 0;
   int tune_damp = 0;  // 0 auto, 1 force on, -1 force off
   int tune_variant = 0;  // 0 auto, 1 row-group kernel, 2 row-lane kernel when eligible
+  fmb::McmcState* mcmc = nullptr;  // MCMC / ALS learner state (fm_mcmc.cu)
 };
 
 namespace fmb {
@@ -145,9 +150,18 @@ cudaError_t launch_predict64(fmb200_ctx* c, const DataSlot& d, int transform, do
 // fm_ordered.cu: sequentially consistent fp64 epoch (runs of independent rows in parallel, bias by
 // affine scan).  *handled = false: shape not eligible, nothing launched (caller uses launch_sgd_inorder)
 cudaError_t launch_sgd_ordered(fmb200_ctx* c, DataSlot& d, bool* handled);
-cudaError_t build_ordered_links(fmb200_ctx* c, DataSlot& d);
+// keep_scratch: keep the (id, entry) sort in d.ord_scratch whatever the data set's size
+cudaError_t build_ordered_links(fmb200_ctx* c, DataSlot& d, bool keep_scratch = false);
 // fm_inorder.cu: the MCMC / ALS e-term pass (fm_learn_mcmc.h:148-378), bit-identical accumulation
 cudaError_t launch_mcmc_eterms(fmb200_ctx* c, const DataSlot& d, double* e_out);
+// fm_mcmc.cu: MCMC / ALS learning (fm_learn_mcmc_simultaneous); "" on success, else the error
+std::string mcmc_begin(fmb200_ctx* c, int train, int test, int do_sample, int do_multilevel, uint32_t n_groups,
+                       const uint32_t* attr_group, const uint32_t* attr_per_group, double reg0,
+                       const double* w_lambda0, const double* v_lambda0);
+std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counters);
+bool mcmc_get(const fmb200_ctx* c, double* alpha, double* w_mu, double* w_lambda, double* v_mu, double* v_lambda,
+              double* pred_this, double* pred_sum_all, double* pred_sum_all_but5, uint32_t* n_runs);
+void mcmc_free(fmb200_ctx* c);
 // fm_inorder.cu: one SGDA epoch (theta-step per training row, lambda-step per validation row)
 cudaError_t launch_sgda_epoch(fmb200_ctx* c, const DataSlot& tr, const DataSlot& va, int lambda_steps);
 // fm_hogwild.cu: throughput epoch

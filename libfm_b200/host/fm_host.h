@@ -377,4 +377,191 @@ class GpuSgdLearner {
   bool use_peer_ = false;
 };
 
+// fm_learn_mcmc_simultaneous (MCMC / ALS, one GPU, no relations): every iteration is one
+// fmb200_mcmc_iteration; this class prints and logs what the reference's _learn does
+// (fm_learn_mcmc_simultaneous.h:88-270) and writes -out like fm_learn_mcmc::predict.
+class GpuMcmcLearner {
+ public:
+  HostModel* fm = nullptr;
+  double min_target = 0, max_target = 0;
+  int task = FMB200_TASK_REGRESSION;
+  int num_iter = 100;
+  bool do_sample = true, do_multilevel = true;
+  int mode = FMB200_MODE_INORDER;
+  int device = 0;
+  RLog* log = nullptr;
+  std::vector<uint32_t> attr_group;  // DataMetaInfo (Data.h:33-96)
+  std::vector<uint32_t> attr_per_group;
+  std::vector<double> w_lambda, v_lambda;  // [G], [G][k]: what -regular sets (libfm.cpp:326-364)
+
+  ~GpuMcmcLearner() {
+    if (ctx_) fmb200_destroy(ctx_);
+  }
+  static void ck(int rc) {
+    if (rc != 0) throw std::string(fmb200_last_error());
+  }
+
+  // fm_learn::init + fm_learn_mcmc::init (fm_learn.h:73-91, fm_learn_mcmc.h:1099-1158): the rlog fields
+  void init() {
+    const uint32_t G = (uint32_t)attr_per_group.size();
+    if (log) {
+      const double nan = std::numeric_limits<double>::quiet_NaN();
+      if (task == FMB200_TASK_REGRESSION) {
+        log->add_field("rmse", nan);
+        log->add_field("mae", nan);
+      } else {
+        log->add_field("accuracy", nan);
+      }
+      for (const char* f : {"time_pred", "time_learn", "time_learn2", "time_learn4", "alpha"}) log->add_field(f, nan);
+      const char* const* names = task == FMB200_TASK_REGRESSION ? reg_fields_ : cls_fields_;
+      for (int i = 0; i < (task == FMB200_TASK_REGRESSION ? 3 : 6); i++) log->add_field(names[i], nan);
+      for (uint32_t g = 0; g < G; g++) {
+        log->add_field("wmu[" + std::to_string(g) + "]", nan);
+        log->add_field("wlambda[" + std::to_string(g) + "]", nan);
+        for (int f = 0; f < fm->num_factor; f++) {
+          log->add_field("vmu[" + std::to_string(g) + "," + std::to_string(f) + "]", nan);
+          log->add_field("vlambda[" + std::to_string(g) + "," + std::to_string(f) + "]", nan);
+        }
+      }
+    }
+    ck(fmb200_create(&ctx_, device, fm->num_attribute, fm->num_factor, fm->k0, fm->k1));
+    ck(fmb200_set_mode(ctx_, mode));
+  }
+
+  void learn(const SparseData& train, const SparseData& test) {
+    ck(fmb200_set_hparams(ctx_, task, 0.0, fm->reg0, fm->regw, fm->regv, min_target, max_target));
+    ck(fmb200_set_params(ctx_, fm->w0, fm->w.data(), fm->v.data()));
+    ck(fmb200_upload_data(ctx_, 0, train.num_cases(), train.num_values(), train.row_ptr.data(), train.col.data(),
+                          train.val.data(), train.target.data()));
+    ck(fmb200_upload_data(ctx_, 1, test.num_cases(), test.num_values(), test.row_ptr.data(), test.col.data(),
+                          test.val.data(), test.target.data()));
+    const uint32_t G = (uint32_t)attr_per_group.size();
+    const int k = fm->num_factor;
+    ck(fmb200_mcmc_begin(ctx_, 0, 1, do_sample, do_multilevel, G, attr_group.data(), attr_per_group.data(),
+                         fm->reg0, w_lambda.data(), v_lambda.data()));
+    const uint64_t nt = test.num_cases();
+    pred_this_.assign(nt, 0.0);
+    pred_all_.assign(nt, 0.0);
+    std::vector<double> but5(nt), w_mu(G), wl(G), v_mu((size_t)G * k), vl((size_t)G * k);
+    static const char* cnt_names[8] = {"alpha", "w0", "w", "v", "w_mu", "w_lambda", "v_mu", "v_lambda"};
+    for (uint32_t i = 0; i < (uint32_t)num_iter; i++) {
+      const double t0 = user_seconds();
+      const clock_t c0 = clock();
+      const auto w0 = std::chrono::steady_clock::now();
+      double train_metric = 0;
+      uint32_t cnt[16];
+      ck(fmb200_mcmc_iteration(ctx_, &train_metric, cnt));
+      for (int p = 0; p < 8; p++)  // fm_learn_mcmc_simultaneous.h:96-119
+        if (cnt[2 * p] > 0 || cnt[2 * p + 1] > 0)
+          std::cout << "#nans in " << cnt_names[p] << ":\t" << cnt[2 * p] << "\t#inf_in_" << cnt_names[p] << ":\t"
+                    << cnt[2 * p + 1] << std::endl;
+      double alpha = 0;
+      ck(fmb200_mcmc_get_hyper(ctx_, &alpha, w_mu.data(), wl.data(), v_mu.data(), vl.data()));
+      ck(fmb200_mcmc_get_pred(ctx_, pred_this_.data(), pred_all_.data(), but5.data()));
+      if (log) {
+        log->log("alpha", alpha);
+        for (uint32_t g = 0; g < G; g++) {
+          log->log("wmu[" + std::to_string(g) + "]", w_mu[g]);
+          log->log("wlambda[" + std::to_string(g) + "]", wl[g]);
+          for (int f = 0; f < k; f++) {
+            log->log("vmu[" + std::to_string(g) + "," + std::to_string(f) + "]", v_mu[(size_t)g * k + f]);
+            log->log("vlambda[" + std::to_string(g) + "," + std::to_string(f) + "]", vl[(size_t)g * k + f]);
+          }
+        }
+        // the reference's clocks are user-CPU time; the iteration runs on the GPU, so wall time goes in too
+        log->log("time_learn", user_seconds() - t0);
+        log->log("time_learn2", (double)(clock() - c0) / CLOCKS_PER_SEC);
+        log->log("time_learn4", std::chrono::duration<double>(std::chrono::steady_clock::now() - w0).count());
+      }
+      // the normalisers keep the reference's unsigned arithmetic: 1/(i-5+1) wraps for i < 4
+      const double n_all = 1.0 / (i + 1), n_but5 = 1.0 / (uint32_t)(i - 5 + 1);
+      if (task == FMB200_TASK_REGRESSION) {
+        double r[3], m[3];
+        eval_reg(pred_this_, test, 1.0, &r[0], &m[0]);
+        eval_reg(pred_all_, test, n_all, &r[1], &m[1]);
+        eval_reg(but5, test, n_but5, &r[2], &m[2]);
+        std::cout << "#Iter=" << std::setw(3) << i << "\tTrain=" << train_metric << "\tTest=" << r[1] << std::endl;
+        if (log) {
+          log->log("rmse", r[1]);
+          log->log("mae", m[1]);
+          for (int q = 0; q < 3; q++) log->log(reg_fields_[q], r[q]);
+          log->new_line();
+        }
+      } else {
+        double a[3], ll[3];
+        eval_cls(pred_this_, test, 1.0, &a[0], &ll[0]);
+        eval_cls(pred_all_, test, n_all, &a[1], &ll[1]);
+        eval_cls(but5, test, n_but5, &a[2], &ll[2]);
+        std::cout << "#Iter=" << std::setw(3) << i << "\tTrain=" << train_metric << "\tTest=" << a[1]
+                  << "\tTest(ll)=" << ll[1] << std::endl;
+        if (log) {
+          log->log("accuracy", a[1]);
+          for (int q = 0; q < 3; q++) {
+            log->log(cls_fields_[q], a[q]);
+            log->log(cls_fields_[3 + q], ll[q]);
+          }
+          log->new_line();
+        }
+      }
+    }
+    ck(fmb200_get_params(ctx_, &fm->w0, fm->w.data(), fm->v.data()));
+  }
+
+  // fm_learn_mcmc::predict (fm_learn_mcmc.h:380-404)
+  void predict_test(std::vector<double>& out) const {
+    out.resize(pred_this_.size());
+    for (size_t c = 0; c < out.size(); c++) {
+      double p = do_sample ? pred_all_[c] / num_iter : pred_this_[c];
+      if (task == FMB200_TASK_REGRESSION) {
+        p = std::min(max_target, p);
+        p = std::max(min_target, p);
+      } else {
+        p = std::min(1.0, p);
+        p = std::max(0.0, p);
+      }
+      out[c] = p;
+    }
+  }
+
+ private:
+  // fm_learn_mcmc_simultaneous::_evaluate / _evaluate_class (:272-309) over all test cases
+  void eval_reg(const std::vector<double>& pred, const SparseData& t, double norm, double* rmse, double* mae) const {
+    double r = 0, m = 0;
+    uint32_t n = 0;
+    for (size_t c = 0; c < pred.size(); c++) {
+      double p = pred[c] * norm;
+      p = std::min(max_target, p);
+      p = std::max(min_target, p);
+      const double err = p - t.target[c];
+      r += err * err;
+      m += std::abs((double)err);
+      n++;
+    }
+    *rmse = std::sqrt(r / n);
+    *mae = m / n;
+  }
+  void eval_cls(const std::vector<double>& pred, const SparseData& t, double norm, double* acc, double* ll) const {
+    double l = 0.0;
+    uint32_t a = 0, n = 0;
+    for (size_t c = 0; c < pred.size(); c++) {
+      const double p = pred[c] * norm;
+      if (((p >= 0.5) && (t.target[c] > 0.0)) || ((p < 0.5) && (t.target[c] < 0.0))) a++;
+      const double m = (t.target[c] + 1.0) * 0.5;
+      double pll = p;
+      if (pll > 0.99) pll = 0.99;
+      if (pll < 0.01) pll = 0.01;
+      l -= m * log10(pll) + (1 - m) * log10(1 - pll);
+      n++;
+    }
+    *ll = l / n;
+    *acc = (double)a / n;
+  }
+
+  static constexpr const char* reg_fields_[3] = {"rmse_mcmc_this", "rmse_mcmc_all", "rmse_mcmc_all_but5"};
+  static constexpr const char* cls_fields_[6] = {"acc_mcmc_this", "acc_mcmc_all", "acc_mcmc_all_but5",
+                                                 "ll_mcmc_this",  "ll_mcmc_all",  "ll_mcmc_all_but5"};
+  fmb200_ctx* ctx_ = nullptr;
+  std::vector<double> pred_this_, pred_all_;
+};
+
 }  // namespace host

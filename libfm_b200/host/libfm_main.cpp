@@ -2,9 +2,9 @@
 //
 // Keeps the reference's flags, defaults, stdout lines and file formats
 // (reference src/libfm/libfm.cpp:62-441) and swaps the learner for one whose
-// passes over the data run in libfmb200 (include/fmb200.h).  Only `-method sgd`
-// is in scope (SURVEY.md section 8); mcmc / als / sgda are refused with a clear
-// error instead of silently doing something else.
+// passes over the data run in libfmb200 (include/fmb200.h).  `-method sgd` runs in every mode;
+// `-method mcmc|als` (data sets without relations, one GPU) run with -mode inorder or ordered, the
+// fp64 state; sgda is refused with a clear error instead of silently doing something else.
 //
 // New, optional flags (old command lines are unaffected):
 //   -mode hogwild|ordered|inorder   throughput (default); sequentially consistent fp64 (parallel over
@@ -16,6 +16,7 @@
 #include <chrono>
 #include <cstdlib>
 #include <ctime>
+#include <fstream>
 #include <iostream>
 #include <string>
 #include <vector>
@@ -24,6 +25,138 @@
 #include "fm_host.h"
 
 using namespace host;
+
+// -method mcmc | als (libfm.cpp:135-139: ALS is MCMC without sampling and hyperparameter inference), following
+// libfm.cpp:141-434 for data sets without relations
+static int run_mcmc(const CmdLine& cmd, bool sample, int mode) {
+  std::cout << "Loading train...\t" << std::endl;
+  SparseData train;
+  train.load(cmd.str("train"));
+  std::cout << "Loading test... \t" << std::endl;
+  SparseData test;
+  test.load(cmd.str("test"));
+  if (cmd.has("validation"))
+    std::cout << "WARNING: Validation data is only used for SGDA. The data is ignored." << std::endl;
+  std::cout << "#relations: " << 0 << std::endl;
+  std::cout << "Loading meta data...\t" << std::endl;
+  const uint32_t n = (uint32_t)std::max(train.num_feature, test.num_feature);  // :203
+  // DataMetaInfo (Data.h:76-96): -meta holds one group id per attribute, read with >>; a value the file
+  // lacks reads as 0 and is counted in group 0
+  std::vector<uint32_t> group(n, 0u);
+  uint32_t G = 1;
+  if (cmd.has("meta")) {
+    std::ifstream in(cmd.str("meta").c_str());
+    if (!in.is_open()) throw "Unable to open file " + cmd.str("meta");
+    G = 0;
+    for (uint32_t i = 0; i < n; i++) {
+      unsigned int v = 0;
+      in >> v;
+      group[i] = v;
+      G = std::max(G, v + 1);
+    }
+  }
+  std::vector<uint32_t> per_group(G, 0u);
+  for (uint32_t i = 0; i < n; i++) per_group[group[i]]++;
+
+  HostModel fm;  // :245-283
+  fm.num_attribute = n;
+  fm.init_stdev = cmd.num("init_stdev", 0.1);
+  {
+    std::vector<int> dim = cmd.int_list("dim");
+    if (dim.size() != 3) throw "-dim needs three values 'k0,k1,k2'";
+    fm.k0 = dim[0] != 0;
+    fm.k1 = dim[1] != 0;
+    fm.num_factor = dim[2];
+  }
+  fm.init();
+  if (cmd.has("load_model")) {  // ALS only: MCMC returned above
+    std::cout << "Reading FM model... \t" << std::endl;
+    if (!fm.load(cmd.str("load_model"))) {
+      std::cout << "WARNING: malformed model file. Nothing will be loaded." << std::endl;
+      fm.init();
+    }
+  }
+  for (uint32_t i = 0; i < n; i++)  // fm.w.init_normal: overwrites a loaded w, as the reference does
+    fm.w[i] = (fm.init_stdev == 0.0 || std::isnan(fm.init_stdev)) ? fm.init_mean
+                                                                   : fm.init_mean + fm.init_stdev * ran_gaussian();
+
+  GpuMcmcLearner fml;
+  fml.fm = &fm;
+  fml.num_iter = (int)cmd.integer("iter", 100);
+  fml.do_sample = fml.do_multilevel = sample;
+  fml.mode = mode;
+  fml.max_target = train.max_target;
+  fml.min_target = train.min_target;
+  const std::string task = cmd.str("task");
+  if (task == "r") {
+    fml.task = FMB200_TASK_REGRESSION;
+  } else if (task == "c") {
+    fml.task = FMB200_TASK_CLASSIFICATION;
+    train.binarize_targets();
+    test.binarize_targets();
+  } else {
+    throw "unknown task";
+  }
+  RLog* rlog = nullptr;
+  std::ofstream* rlog_file = nullptr;
+  if (cmd.has("rlog")) {
+    const std::string f = cmd.str("rlog");
+    rlog_file = new std::ofstream(f.c_str());
+    if (!rlog_file->is_open()) throw "Unable to open file " + f;
+    std::cout << "logging to " << f << std::endl;
+    rlog = new RLog(rlog_file);
+  }
+  fml.log = rlog;
+  fml.attr_group = group;
+  fml.attr_per_group = per_group;
+  const int k = fm.num_factor;
+  if (getenv("CUDA_VISIBLE_DEVICES") == nullptr) {
+    setenv("CUDA_VISIBLE_DEVICES", std::to_string(cmd.integer("device", 0)).c_str(), 1);
+  } else {
+    fml.device = (int)cmd.integer("device", 0);
+  }
+  fml.init();
+  {  // regularisation per group, :326-364
+    std::vector<double> reg = cmd.num_list("regular");
+    if (!(reg.size() == 0 || reg.size() == 1 || reg.size() == 3 || reg.size() == 1 + 2 * (size_t)G))
+      throw "-regular needs 0, 1, 3 or 1+2*#groups values";  // assert at :330
+    fml.w_lambda.assign(G, 0.0);
+    fml.v_lambda.assign((size_t)G * k, 0.0);
+    if (reg.size() == 1 || reg.size() == 3) {
+      fm.reg0 = reg[0];
+      fm.regw = reg.size() == 1 ? reg[0] : reg[1];
+      fm.regv = reg.size() == 1 ? reg[0] : reg[2];
+      fml.w_lambda.assign(G, fm.regw);
+      fml.v_lambda.assign((size_t)G * k, fm.regv);
+    } else if (reg.size() == 1 + 2 * (size_t)G && reg.size() > 3) {
+      fm.reg0 = reg[0];
+      for (uint32_t g = 0; g < G; g++) fml.w_lambda[g] = reg[1 + g];
+      for (uint32_t g = 0; g < G; g++)
+        for (int f = 0; f < k; f++) fml.v_lambda[(size_t)g * k + f] = reg[1 + G + g];
+    }
+  }
+  if (rlog) rlog->init();
+  if (cmd.integer("verbosity", 0) > 0) fm.debug();
+  fml.learn(train, test);
+  // no Final line for MCMC / ALS (:417-420)
+  if (cmd.has("out")) {
+    std::vector<double> pred;
+    fml.predict_test(pred);
+    std::ofstream out(cmd.str("out").c_str());
+    if (out.is_open()) {
+      for (double p : pred) out << p << std::endl;
+    } else {
+      std::cout << "Unable to open file " << cmd.str("out");
+    }
+  }
+  if (cmd.has("save_model")) {  // ALS only
+    std::cout << "Writing FM model to " << cmd.str("save_model") << std::endl;
+    fm.save(cmd.str("save_model"));
+  }
+  delete rlog;
+  delete rlog_file;
+  return 0;
+}
 
 int main(int argc, char** argv) {
   const auto t_start = std::chrono::steady_clock::now();
@@ -78,6 +211,24 @@ int main(int argc, char** argv) {
     if (!cmd.has(p_dim)) cmd.set(p_dim, "1,1,8");
 
     const std::string method = cmd.str(p_method);
+    // libfm.cpp:123-133: MCMC keeps no model file
+    if (method == "mcmc" && cmd.has(p_save)) {
+      std::cout << "WARNING: -save_model enabled only for SGD and ALS." << std::endl;
+      return 0;
+    }
+    if (method == "mcmc" && cmd.has(p_load)) {
+      std::cout << "WARNING: -load_model enabled only for SGD and ALS." << std::endl;
+      return 0;
+    }
+    if (method == "mcmc" || method == "als") {
+      const std::string mode = cmd.str(p_mode, "hogwild");
+      if (mode != "inorder" && mode != "ordered")
+        throw std::string("method '" + method + "' is outside the libfm_b200 scope in -mode " + mode +
+                          " (the fp32 SGD path); use -mode inorder");
+      if (cmd.integer(p_gpus, 1) != 1) throw std::string("-method " + method + " runs on one GPU: -gpus must be 1");
+      if (!cmd.list(p_rel).empty()) throw std::string("relations (-relation) are not supported with -method " + method);
+      return run_mcmc(cmd, method == "mcmc", mode == "inorder" ? FMB200_MODE_INORDER : FMB200_MODE_ORDERED);
+    }
     if (method != "sgd") {
       if (method == "mcmc" || method == "als" || method == "sgda")
         throw std::string("method '" + method + "' is outside the libfm_b200 scope (SGD hot path only); use -method sgd");

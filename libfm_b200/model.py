@@ -372,6 +372,49 @@ class FmLearnSgdElement:
         self._check(self.lib.fmb200_mcmc_eterms(self._ctx, self._slot_of(data), _p(out, C.c_double)))
         return out
 
+    # -- MCMC / ALS: fm_learn_mcmc_simultaneous ---------------------------------
+    def mcmc_begin(self, train: Data, test: Data, do_sample: bool, do_multilevel: bool, reg0: float,
+                   w_lambda, v_lambda, attr_group=None, attr_per_group=None) -> None:
+        """fm_learn_mcmc::init + the prologue of _learn.  w_lambda [G], v_lambda [G][k] as -regular sets
+        them (libfm.cpp:326-364); attr_group / attr_per_group as DataMetaInfo holds them (None: one group)."""
+        self.push_hparams()
+        wl = np.ascontiguousarray(w_lambda, dtype=np.float64)
+        self._mcmc_groups = int(wl.shape[0])
+        vl = np.ascontiguousarray(v_lambda, dtype=np.float64).reshape(self._mcmc_groups, self.fm.num_factor)
+        g = None if attr_group is None else np.ascontiguousarray(attr_group, dtype=np.uint32)
+        pg = None if attr_per_group is None else np.ascontiguousarray(attr_per_group, dtype=np.uint32)
+        self._check(self.lib.fmb200_mcmc_begin(
+            self._ctx, self._slot_of(train), self._slot_of(test), int(do_sample), int(do_multilevel),
+            self._mcmc_groups, None if g is None else _p(g, C.c_uint32), None if pg is None else _p(pg, C.c_uint32),
+            float(reg0), _p(wl, C.c_double), _p(vl, C.c_double)))
+
+    def mcmc_iteration(self):
+        """One iteration of fm_learn_mcmc_simultaneous::_learn; returns (train metric, counters[16])."""
+        m = C.c_double()
+        cnt = np.zeros(16, dtype=np.uint32)
+        self._check(self.lib.fmb200_mcmc_iteration(self._ctx, C.byref(m), _p(cnt, C.c_uint32)))
+        return m.value, cnt
+
+    def mcmc_hyper(self) -> dict:
+        G, k = self._mcmc_groups, self.fm.num_factor
+        alpha = C.c_double()
+        out = {"w_mu": np.zeros(G), "w_lambda": np.zeros(G), "v_mu": np.zeros((G, k)), "v_lambda": np.zeros((G, k))}
+        self._check(self.lib.fmb200_mcmc_get_hyper(self._ctx, C.byref(alpha), *[_p(out[n], C.c_double) for n in
+                                                                               ("w_mu", "w_lambda", "v_mu", "v_lambda")]))
+        out["alpha"] = alpha.value
+        return out
+
+    def mcmc_pred(self, test: Data):
+        """(pred_this, pred_sum_all, pred_sum_all_but5) over the test set."""
+        out = [np.zeros(test.num_cases) for _ in range(3)]
+        self._check(self.lib.fmb200_mcmc_get_pred(self._ctx, *[_p(a, C.c_double) for a in out]))
+        return tuple(out)
+
+    def mcmc_runs(self) -> int:
+        n = C.c_uint32()
+        self._check(self.lib.fmb200_mcmc_runs(self._ctx, C.byref(n)))
+        return n.value
+
     def learn(self, train: Data, test: Data, log=None):
         """fm_learn_sgd_element::learn (fm_learn_sgd_element.h:48-78)."""
         self.push_hparams()
