@@ -1,7 +1,9 @@
-// fm_hogwild_common.cuh -- pieces shared by the two HOGWILD epoch kernels
-// (fm_hogwild.cu: sub-warp row groups, any k / row length; fm_rowlane.cu: one lane
-// per row for short rows with k <= 8): launch arguments, the TMA tile producer and
-// the mean-field step scale.  See fm_hogwild.cu for the design notes.
+// fm_hogwild_common.cuh -- the tile protocol shared by the three HOGWILD epoch kernels
+// (fm_hogwild.cu: sub-warp row groups, any k / row length; fm_rowlane.cu: one lane per row
+// for short rows with k <= 8, block-synchronous and warp-specialised): launch arguments,
+// the staging ring's stage layout, set-up and TMA producer, the loss multiplier, the
+// per-warp bias partials and the mean-field step scale.  See fm_hogwild.cu for the design
+// notes.
 #pragma once
 #include "fm_device.cuh"
 #include "fmb200_internal.h"
@@ -10,7 +12,24 @@ namespace fmb {
 
 constexpr int HW_NSTAGE = 3;
 constexpr int HW_MAX_THREADS = 256;
+constexpr uint32_t HW_NO_TILE = 0xffffffffu;
 constexpr int HW_HDR_BYTES = 256;  // mbarriers [0,64) + per-warp bias partials [64,192): [2 slots][8 warps] float2
+// header of the warp-specialised kernel: full[3] @0, empty[3] @64, tile[3] @128, w0[3] @160,
+// per-warp bias partials @192: [3 stages][8 warps] float2
+constexpr int HW_WS_HDR_BYTES = 512;
+
+// One stage of the ring: [row offsets (TR+2)·u64 | targets TR·f32 | ids cap·u32 | values cap·f32],
+// padded to 16 bytes.  TR is a multiple of 32 and cap of 4, so every part starts 16-byte aligned as
+// the bulk copies need.  cap == 0 stages only the row offsets and targets.
+// T is the width of the arithmetic: uint32_t for the bulk-copy byte counts, uint64_t for the launchers.
+template <typename T>
+__host__ __device__ inline T hw_rp_bytes(int TR) { return (T)(TR + 2) * 8; }
+template <typename T>
+__host__ __device__ inline T hw_y_bytes(int TR) { return (T)TR * 4; }
+// 64-bit: the launcher sizes the stage of a tile of very long rows, whose cap exceeds 32 bits
+__host__ __device__ inline uint64_t hw_stage_bytes(int TR, uint64_t cap) {
+  return (hw_rp_bytes<uint64_t>(TR) + hw_y_bytes<uint64_t>(TR) + 2 * cap * 4 + 15) & ~15ull;
+}
 
 struct HogwildArgs {
   const uint64_t* row_ptr;
@@ -67,23 +86,26 @@ __device__ __forceinline__ unsigned long long acc_quantise(float d, unsigned lon
   return 0ull;
 }
 
+// stage `stage` of the ring, which follows a shared-memory header of `hdr` bytes
 __device__ __forceinline__ unsigned char* stage_base(unsigned char* smem, const HogwildArgs& a,
-                                                     int stage) {
-  return smem + HW_HDR_BYTES + (size_t)stage * a.stage_bytes;
+                                                     int stage, int hdr = HW_HDR_BYTES) {
+  return smem + hdr + (size_t)stage * a.stage_bytes;
 }
 
-// TMA producer: stage one tile whose entry range [nb, ne) is already known.
-__device__ __forceinline__ void issue_tile(const HogwildArgs& a, unsigned char* smem,
-                                           uint64_t* bars, uint32_t tile, int stage,
-                                           uint64_t policy, uint64_t nb, uint64_t ne) {
+// TMA producer: stage one tile whose entry range [nb, ne) is already known into stage `stage` of
+// the ring behind a header of `hdr` bytes, completing on bars[stage].  The barrier's arrival
+// releases the producer's earlier shared stores.
+__device__ __forceinline__ void issue_tile(const HogwildArgs& a, unsigned char* smem, uint64_t* bars,
+                                           uint32_t tile, int stage, uint64_t policy, uint64_t nb,
+                                           uint64_t ne, int hdr = HW_HDR_BYTES) {
   const int TR = a.tile_rows;
   const uint64_t r0 = (uint64_t)tile * TR;
   const uint64_t ab = nb & ~3ull;
   const uint64_t ae = (ne + 3ull) & ~3ull;
   const uint32_t ebytes = a.global_entries ? 0u : (uint32_t)(ae - ab) * 4u;
-  const uint32_t rp_bytes = (uint32_t)(TR + 2) * 8u;
-  const uint32_t y_bytes = (uint32_t)TR * 4u;
-  unsigned char* sb = stage_base(smem, a, stage);
+  const uint32_t rp_bytes = hw_rp_bytes<uint32_t>(TR);
+  const uint32_t y_bytes = hw_y_bytes<uint32_t>(TR);
+  unsigned char* sb = stage_base(smem, a, stage, hdr);
   uint64_t* bar = bars + stage;
   mbar_arrive_expect_tx(bar, rp_bytes + y_bytes + 2u * ebytes);
   bulk_g2s_hint(sb, a.row_ptr + r0, rp_bytes, bar, policy);
@@ -93,6 +115,41 @@ __device__ __forceinline__ void issue_tile(const HogwildArgs& a, unsigned char* 
     bulk_g2s_hint(cb, a.col + ab, ebytes, bar, policy);
     bulk_g2s_hint(cb + (size_t)a.tile_cap * 4u, a.val + ab, ebytes, bar, policy);
   }
+}
+
+// Set-up of the block-synchronous kernels (one mbarrier per stage, HW_HDR_BYTES header): thread 0
+// initialises the barriers and the producer, lane 0 of the last warp, takes the evict-first
+// policy, which this returns.
+__device__ __forceinline__ uint64_t ring_init(unsigned char* smem, int tid) {
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem);
+  uint64_t policy = 0;
+  if (tid == 0) {
+    for (int i = 0; i < HW_NSTAGE; i++) mbar_init(bars + i, 1);
+    fence_mbar_init();
+  }
+  if (tid == (int)blockDim.x - 32) policy = policy_evict_first();
+  __syncthreads();
+  return policy;
+}
+
+// fm_learn_sgd_element.h:58-65: the loss multiplier of score p against target y, and the secant
+// curvature of the loss w.r.t. the raw score (1 where the clamp is inactive; logistic: s(1-s))
+struct LossStep {
+  float mult, curv;
+};
+__device__ __forceinline__ LossStep loss_step(const HogwildArgs& a, float p, float y) {
+  LossStep l;
+  if (a.task == FMB200_TASK_REGRESSION) {
+    const float pc = fmaxf(a.min_target, fminf(a.max_target, p));
+    l.mult = pc - y;
+    const float den = p - y;
+    l.curv = (pc == p) ? 1.f : (fabsf(den) > 1e-12f ? fminf(fmaxf(l.mult / den, 0.f), 1.f) : 0.f);
+  } else {  // y in {-1,+1}
+    const float sg = 1.f / (1.f + __expf(-y * p));
+    l.mult = -y * (1.f - sg);
+    l.curv = sg * (1.f - sg);
+  }
+  return l;
 }
 
 // gamma(c, u) = (1 - (1-u)^c) / (c*u): scale of each of c concurrent steps whose
@@ -106,6 +163,12 @@ __device__ __forceinline__ float gamma_scale(float c, float u) {
   return fminf(1.f, (1.f - ac) / q);
 }
 
+// the bias partials of a warp: lane 0 stores the warp's sums of (mult, hjoint) at part[warp]
+__device__ __forceinline__ void bias_partial(float2* part, float mult, float hjoint, int tid) {
+  mult = warp_sum(mult);
+  hjoint = warp_sum(hjoint);
+  if ((tid & 31) == 0) part[tid >> 5] = make_float2(mult, hjoint);
+}
 
 // The bias sector is reduced into by every CTA once per tile; loads of it queue behind
 // those reductions at its single L2 slice.  So ONE lane per CTA fetches it per tile
@@ -138,7 +201,6 @@ struct BiasFetch {
 // the tail of the epoch is balanced (a static round-robin leaves 1/9 of the CTAs a whole
 // tile short on C2) and the rows in flight stay one contiguous window.  Used by thread 0
 // only.  The last CTA to run dry resets the two words for the next launch.
-constexpr uint32_t HW_NO_TILE = 0xffffffffu;
 struct TileSched {
   unsigned int* w;
   uint32_t n_tiles;
@@ -180,7 +242,7 @@ using HogwildKernelFn = void (*)(const HogwildArgs);
 // fm_rowlane.cu: kernel for (float4 chunks per row gp in {1,2}, rows of at most Z entries); a
 // cooperative launch whose grid size is the window size
 HogwildKernelFn pick_rowlane_kernel(int gp, int max_row_nnz, bool damp, bool combine);
-// warp-specialised variant: blockDim = rows_per_tile + 32, smem header 512 B
+// warp-specialised variant: blockDim = rows_per_tile + 32, smem header HW_WS_HDR_BYTES
 HogwildKernelFn pick_rowlane_ws_kernel(int gp, int max_row_nnz, bool damp, bool combine);
 
 }  // namespace fmb

@@ -100,7 +100,7 @@ __global__ void __launch_bounds__(256) fm_predict32_kernel(const PredictArgs a) 
 
 using PredictFn = void (*)(const PredictArgs);
 
-// the same (R, RW) register-cache classes as the training kernel: all of a row's gathers
+// the (R, RW) register-cache classes 0..2 of the training kernel: all of a row's gathers
 // are in flight before the first is consumed
 template <int G, int S>
 static PredictFn pick_predict_r(int cls) {
@@ -128,11 +128,9 @@ static PredictFn pick_predict_s(int S, int cls) {
 cudaError_t launch_predict32(fmb200_ctx* c, const DataSlot& d, int transform, double* out_pred,
                              double* partials, int n_blocks) {
   if (c->kp / 4 > 32) return cudaErrorInvalidValue;
-  int G, S;
-  pick_geometry(c->kp, d.n_rows, d.nnz, &G, &S);
-  const double avg = d.n_rows ? (double)d.nnz / (double)d.n_rows : 1.0;
-  const int iters = (int)((avg + S - 1) / S);
-  const int cls = iters <= 2 ? 0 : (iters <= 8 ? 1 : 2);
+  int G, S, cls;
+  pick_geometry(c->kp, d.n_rows, d.nnz, &G, &S, &cls);
+  cls = std::clamp(cls, 0, 2);  // the training kernel's classes -1 and 3 are not instantiated here
   PredictFn fn;
   switch (G) {
     case 1: fn = pick_predict_s<1>(S, cls); break;

@@ -196,7 +196,8 @@ uint64_t aos_scan_tiles(uint64_t n_rows);
 cudaError_t launch_onehot_fill(fmb200_ctx* c, uint64_t n_rows, uint32_t z, uint64_t* row_ptr, float* val);
 
 // pick the sub-warp geometry for a data set: G lanes per V row (power of two
-// covering kp/4 float4 chunks), S entry slots per row group
-void pick_geometry(int kp, uint64_t n_rows, uint64_t nnz, int* G, int* S);
+// covering kp/4 float4 chunks), S entry slots per row group, and the row-group
+// register-cache class (fm_hogwild.cu, pick_r: -1 .. 3 from short to long rows)
+void pick_geometry(int kp, uint64_t n_rows, uint64_t nnz, int* G, int* S, int* cls);
 
 }  // namespace fmb
