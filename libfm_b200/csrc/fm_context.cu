@@ -54,50 +54,30 @@ int bind(fmb200_ctx* c) {
   return 0;
 }
 
-void free_slot(DataSlot& s) {
-  if (s.row_ptr) cudaFree(s.row_ptr);
-  if (s.col) cudaFree(s.col);
-  if (s.val) cudaFree(s.val);
-  if (s.target) cudaFree(s.target);
-  if (s.feat_cnt) cudaFree(s.feat_cnt);
-  if (s.link) cudaFree(s.link);
-  if (s.rowdep) cudaFree(s.rowdep);
-  if (s.ord_scratch) cudaFree(s.ord_scratch);
-  if (s.d_flag) cudaFree(s.d_flag);
-  if (s.h_flag) cudaFreeHost(s.h_flag);
-  if (s.ready) cudaEventDestroy(s.ready);
-  s = DataSlot();
-}
-
-// slack (in elements) behind every CSR array so that whole-tile TMA bulk copies
-// of the last tile stay inside the allocation
-constexpr uint64_t kRowSlack = 512 + 8;
-constexpr uint64_t kEntrySlack = 16;
-
 // Make `slot` ready to receive a data set of (n_rows, nnz): drain an earlier asynchronous
 // upload, (re)allocate, reset the bookkeeping.  Enqueues only the memsets of fresh buffers.
 int upload_begin(fmb200_ctx* c, int slot, uint64_t n_rows, uint64_t nnz, cudaStream_t st) {
   DataSlot& s = c->slots[slot];
   if (s.pending) {  // an earlier asynchronous upload into this slot: drain it first
-    CK(cudaEventSynchronize(s.ready));
+    CK(cudaEventSynchronize(s.ready.get()));
     s.pending = false;
   }
   // re-uploads into a slot reuse its buffers when they are large enough
   if (!(s.row_ptr && s.cap_rows >= n_rows && s.cap_nnz >= nnz)) {
-    free_slot(s);
-    CK(cudaMalloc(&s.row_ptr, (n_rows + 1 + kRowSlack) * sizeof(uint64_t)));
-    CK(cudaMalloc(&s.target, (n_rows + kRowSlack) * sizeof(float)));
-    CK(cudaMalloc(&s.col, (nnz + kEntrySlack) * sizeof(uint32_t)));
-    CK(cudaMalloc(&s.val, (nnz + kEntrySlack) * sizeof(float)));
-    CK(cudaMalloc(&s.feat_cnt, sizeof(float) * (size_t)(c->n ? c->n : 1)));
-    CK(cudaMalloc(&s.d_flag, 16 * sizeof(unsigned int)));
-    CK(cudaHostAlloc((void**)&s.h_flag, 16 * sizeof(unsigned int), cudaHostAllocDefault));
-    CK(cudaEventCreateWithFlags(&s.ready, cudaEventDisableTiming));
+    s = DataSlot();  // releases the slot's buffers, its ORDERED index and the index scratch
+    CK(alloc(s.row_ptr, n_rows + 1 + kRowSlack));
+    CK(alloc(s.target, n_rows + kRowSlack));
+    CK(alloc(s.col, nnz + kEntrySlack));
+    CK(alloc(s.val, nnz + kEntrySlack));
+    CK(alloc(s.feat_cnt, c->n));
+    CK(alloc(s.d_flag, 16));
+    CK(host_alloc(s.h_flag, 16));
+    CK(event_create(s.ready, cudaEventDisableTiming));
     // the slack is only ever read by whole-tile bulk copies and never used
-    CK(cudaMemsetAsync(s.row_ptr, 0, (n_rows + 1 + kRowSlack) * sizeof(uint64_t), st));
-    CK(cudaMemsetAsync(s.target, 0, (n_rows + kRowSlack) * sizeof(float), st));
-    CK(cudaMemsetAsync(s.col, 0, (nnz + kEntrySlack) * sizeof(uint32_t), st));
-    CK(cudaMemsetAsync(s.val, 0, (nnz + kEntrySlack) * sizeof(float), st));
+    CK(cudaMemsetAsync(s.row_ptr.get(), 0, (n_rows + 1 + kRowSlack) * sizeof(uint64_t), st));
+    CK(cudaMemsetAsync(s.target.get(), 0, (n_rows + kRowSlack) * sizeof(float), st));
+    CK(cudaMemsetAsync(s.col.get(), 0, (nnz + kEntrySlack) * sizeof(uint32_t), st));
+    CK(cudaMemsetAsync(s.val.get(), 0, (nnz + kEntrySlack) * sizeof(float), st));
     s.cap_rows = n_rows;
     s.cap_nnz = nnz;
   }
@@ -115,17 +95,12 @@ int upload_begin(fmb200_ctx* c, int slot, uint64_t n_rows, uint64_t nnz, cudaStr
 // Leaves the results in the slot's pinned flag mirror; upload_finish() collects them.
 int upload_inspect(fmb200_ctx* c, int slot, cudaStream_t st) {
   DataSlot& s = c->slots[slot];
-  cudaStream_t saved = c->stream;
-  c->stream = st;  // the launch helpers enqueue on c->stream
-  cudaError_t e1 = cudaMemsetAsync(s.d_flag, 0, 16 * sizeof(unsigned int), st);
-  cudaError_t e2 = launch_csr_inspect(c, s.row_ptr, s.n_rows, s.nnz, s.d_flag);
-  cudaError_t e3 = launch_feature_counts(c, s.col, s.nnz, s.feat_cnt, s.d_flag + 8, s.d_flag + 9);
-  c->stream = saved;
-  CK(e1);
-  CK(e2);
-  CK(e3);
-  CK(cudaMemcpyAsync(s.h_flag, s.d_flag, 16 * sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
-  CK(cudaEventRecord(s.ready, st));
+  unsigned int* flag = s.d_flag.get();
+  CK(cudaMemsetAsync(flag, 0, 16 * sizeof(unsigned int), st));
+  CK(launch_csr_inspect(c, st, s.row_ptr.get(), s.n_rows, s.nnz, flag));
+  CK(launch_feature_counts(c, st, s.col.get(), s.nnz, s.feat_cnt.get(), flag + 8, flag + 9));
+  CK(cudaMemcpyAsync(s.h_flag.get(), flag, 16 * sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
+  CK(cudaEventRecord(s.ready.get(), st));
   s.pending = true;
   return 0;
 }
@@ -135,10 +110,10 @@ int upload_enqueue(fmb200_ctx* c, int slot, uint64_t n_rows, uint64_t nnz, const
                    const uint32_t* col, const float* val, const float* target, cudaStream_t st) {
   if (upload_begin(c, slot, n_rows, nnz, st)) return 1;
   DataSlot& s = c->slots[slot];
-  CK(cudaMemcpyAsync(s.row_ptr, row_ptr, (n_rows + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(s.target, target, n_rows * sizeof(float), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(s.col, col, nnz * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(s.val, val, nnz * sizeof(float), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(s.row_ptr.get(), row_ptr, (n_rows + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(s.target.get(), target, n_rows * sizeof(float), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(s.col.get(), col, nnz * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(s.val.get(), val, nnz * sizeof(float), cudaMemcpyHostToDevice, st));
   return upload_inspect(c, slot, st);
 }
 
@@ -149,31 +124,19 @@ int upload_onehot_enqueue(fmb200_ctx* c, int slot, uint64_t n_rows, uint32_t z, 
   const uint64_t nnz = n_rows * z;
   if (upload_begin(c, slot, n_rows, nnz, st)) return 1;
   DataSlot& s = c->slots[slot];
-  CK(cudaMemcpyAsync(s.target, target, n_rows * sizeof(float), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(s.col, ids, nnz * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-  cudaStream_t saved = c->stream;
-  c->stream = st;
-  cudaError_t e = launch_onehot_fill(c, n_rows, z, s.row_ptr, s.val);
-  c->stream = saved;
-  CK(e);
+  CK(cudaMemcpyAsync(s.target.get(), target, n_rows * sizeof(float), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(s.col.get(), ids, nnz * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+  CK(launch_onehot_fill(c, st, n_rows, z, s.row_ptr.get(), s.val.get()));
   return upload_inspect(c, slot, st);
 }
-
-// RAII for the temporaries of the AoS upload
-struct DevTmp {
-  void* p = nullptr;
-  ~DevTmp() {
-    if (p) cudaFree(p);
-  }
-};
 
 // The one host sync of an upload: wait for the slot's event and read the verdict.
 int upload_finish(fmb200_ctx* c, int slot) {
   DataSlot& s = c->slots[slot];
   if (!s.pending) return 0;
-  CK(cudaEventSynchronize(s.ready));
+  CK(cudaEventSynchronize(s.ready.get()));
   s.pending = false;
-  const unsigned int* h = s.h_flag;
+  const unsigned int* h = s.h_flag.get();
   if (h[0] & 1u) return fail("row_ptr[0] must be 0");
   if (h[0] & 2u) return fail("row_ptr is not monotone");
   if (h[0] & 4u) return fail("row_ptr[n_rows] != nnz");
@@ -200,23 +163,6 @@ int need_slot(fmb200_ctx* c, int slot) {
   return 0;
 }
 
-int ensure_partials(fmb200_ctx* c, int n_blocks) {
-  if (c->n_partials < n_blocks) {
-    if (c->d_partials) cudaFree(c->d_partials);
-    c->d_partials = nullptr;
-    CK(cudaMalloc(&c->d_partials, sizeof(double) * 3 * n_blocks));
-    c->n_partials = n_blocks;
-  }
-  return 0;
-}
-
-int metric_blocks(fmb200_ctx* c, const DataSlot& s) {
-  uint64_t want = (s.n_rows + 255) / 256;
-  uint64_t cap = (uint64_t)c->sm_count * 8;
-  uint64_t b = want < cap ? want : cap;
-  return (int)(b < 1 ? 1 : b);
-}
-
 }  // namespace
 
 // Everything of fmb200_create that can fail after the context object exists; the caller
@@ -233,8 +179,8 @@ static int create_resources(fmb200_ctx* c, int device, const cudaDeviceProp& pro
   c->k1 = use_w != 0;
   CK(cudaSetDevice(device));
   CK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-  CK(cudaEventCreate(&c->ev0));
-  CK(cudaEventCreate(&c->ev1));
+  CK(event_create(c->ev0, cudaEventDefault));
+  CK(event_create(c->ev1, cudaEventDefault));
   c->p32.ws = (n_attr <= 131072u) ? 8 : 1;
   const uint64_t n4 = ((uint64_t)n_attr * c->p32.ws + 3) & ~3ull;
   c->p32.off_w = 4;
@@ -242,26 +188,22 @@ static int create_resources(fmb200_ctx* c, int device, const cudaDeviceProp& pro
   c->p32.n_floats = 4 + n4 + (uint64_t)n_attr * c->kp;
   c->p64.off_v = Params64::off_w + (((uint64_t)n_attr + 1) & ~1ull);
   c->p64.n_doubles = c->p64.off_v + (uint64_t)n_attr * num_factor + 2;
-  c->comm_buf_bytes = (c->p32.n_floats * sizeof(float) + 255) & ~(size_t)255;
-  c->comm_cnt_floats = ((size_t)n_attr + 63) & ~(size_t)63;
-  const size_t comm_total = c->comm_hdr + 3 * c->comm_buf_bytes + (3 * c->comm_cnt_floats + 2 * (size_t)fmb::FMB_PEER_PART) * sizeof(float);
-  CK(cudaMalloc(&c->comm_base, comm_total));
-  CK(cudaMemsetAsync(c->comm_base, 0, comm_total, c->stream));
-  c->p32.base = reinterpret_cast<float*>(c->comm_base + c->comm_hdr);
-  c->peer_base[0] = c->comm_base;
-  CK(cudaMalloc(&c->p64.base, c->p64.n_doubles * sizeof(double)));
+  c->comm = CommLayout(c->p32.n_floats, n_attr);
+  CK(alloc(c->comm_base, c->comm.total_bytes()));
+  CK(cudaMemsetAsync(c->comm_base.get(), 0, c->comm.total_bytes(), c->stream));
+  c->p32.base = c->comm.buf(c->comm_base.get(), 0);
+  c->peer_base[0] = c->comm_base.get();
+  CK(alloc(c->p64_buf, c->p64.n_doubles));
+  c->p64.base = c->p64_buf.get();
   CK(cudaMemsetAsync(c->p32.base, 0, c->p32.n_floats * sizeof(float), c->stream));
   CK(cudaMemsetAsync(c->p64.base, 0, c->p64.n_doubles * sizeof(double), c->stream));
-  CK(cudaMalloc(&c->d_sched, 2 * sizeof(unsigned int)));
-  CK(cudaMemsetAsync(c->d_sched, 0, 2 * sizeof(unsigned int), c->stream));
-  CK(cudaMalloc(&c->d_flag, 16 * sizeof(unsigned int)));
-  CK(cudaHostAlloc((void**)&c->h_flag, 16 * sizeof(unsigned int), cudaHostAllocDefault));
+  CK(alloc(c->d_sched, 2));
+  CK(cudaMemsetAsync(c->d_sched.get(), 0, 2 * sizeof(unsigned int), c->stream));
+  CK(alloc(c->d_flag, 16));
+  CK(host_alloc(c->h_flag, 16));
   {
     const size_t need = std::max(c->p32.n_floats * sizeof(float), c->p64.n_doubles * sizeof(double));
-    if (need <= (64u << 20)) {
-      CK(cudaHostAlloc(&c->h_stage, need, cudaHostAllocDefault));
-      c->h_stage_bytes = need;
-    }
+    if (need <= (64u << 20)) CK(host_alloc(c->h_stage, need));
   }
   CK(cudaStreamSynchronize(c->stream));
   return 0;
@@ -301,29 +243,12 @@ void fmb200_destroy(fmb200_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
   if (c->stream) cudaStreamSynchronize(c->stream);
-  for (int i = 0; i < FMB200_MAX_SLOTS; i++) free_slot(c->slots[i]);
   for (int q = 0; q < FMB200_MAX_PEERS; q++)
     if (c->peer_ipc[q] && c->peer_base[q]) cudaIpcCloseMemHandle(c->peer_base[q]);
-  if (c->comm_base) cudaFree(c->comm_base);
-  if (c->d_acc) cudaFree(c->d_acc);
-  if (c->p64.base) cudaFree(c->p64.base);
-  if (c->sgda_grad_w) cudaFree(c->sgda_grad_w);
-  if (c->sgda_grad_v) cudaFree(c->sgda_grad_v);
-  if (c->sgda_reg_w) cudaFree(c->sgda_reg_w);
-  if (c->sgda_reg_v) cudaFree(c->sgda_reg_v);
-  if (c->sgda_group) cudaFree(c->sgda_group);
-  mcmc_free(c);
-  if (c->d_partials) cudaFree(c->d_partials);
-  if (c->d_pred) cudaFree(c->d_pred);
-  if (c->d_sched) cudaFree(c->d_sched);
-  if (c->d_flag) cudaFree(c->d_flag);
-  if (c->h_flag) cudaFreeHost(c->h_flag);
-  if (c->h_stage) cudaFreeHost(c->h_stage);
-  if (c->ev0) cudaEventDestroy(c->ev0);
-  if (c->ev1) cudaEventDestroy(c->ev1);
-  if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
-  if (c->stream) cudaStreamDestroy(c->stream);
-  delete c;
+  cudaStream_t stream = c->stream, copy_stream = c->copy_stream;
+  delete c;  // the owning handles release every buffer and event
+  if (copy_stream) cudaStreamDestroy(copy_stream);
+  if (stream) cudaStreamDestroy(stream);
 }
 
 int fmb200_set_hparams(fmb200_ctx* c, int task, double learn_rate, double reg0, double regw,
@@ -445,27 +370,30 @@ int fmb200_upload_data_aos(fmb200_ctx* c, int slot, uint64_t n_rows, const void*
   }
   const unsigned long long base = (unsigned long long)(uintptr_t)r[first].data;
   cudaStream_t st = c->stream;
-  DevTmp d_rows, d_rp, d_scr, d_ent;
-  unsigned int* flag = c->d_flag;
-  CK(cudaMalloc(&d_rows.p, n_rows * sizeof(AosRow)));
-  CK(cudaMalloc(&d_rp.p, (n_rows + 1) * sizeof(uint64_t)));
-  CK(cudaMalloc(&d_scr.p, (aos_scan_tiles(n_rows) + 1) * sizeof(unsigned long long)));
+  // temporaries of the upload, released on return
+  DevPtr<AosRow> d_rows;
+  DevPtr<uint64_t> d_rp;
+  DevPtr<unsigned long long> d_scr;
+  DevPtr<AosEntry> d_ent;
+  unsigned int* flag = c->d_flag.get();
+  CK(alloc(d_rows, n_rows));
+  CK(alloc(d_rp, n_rows + 1));
+  CK(alloc(d_scr, aos_scan_tiles(n_rows) + 1));
   CK(cudaMemsetAsync(flag, 0, 16 * sizeof(unsigned int), st));
-  CK(cudaMemcpyAsync(d_rows.p, r, n_rows * sizeof(AosRow), cudaMemcpyHostToDevice, st));
-  CK(launch_aos_to_csr(c, d_rows.p, nullptr, n_rows, 0, base, static_cast<unsigned long long*>(d_scr.p),
-                       static_cast<uint64_t*>(d_rp.p), nullptr, nullptr, flag));
+  CK(cudaMemcpyAsync(d_rows.get(), r, n_rows * sizeof(AosRow), cudaMemcpyHostToDevice, st));
+  CK(launch_aos_to_csr(c, st, d_rows.get(), nullptr, n_rows, 0, base, d_scr.get(), d_rp.get(), nullptr, nullptr, flag));
   uint64_t nnz = 0;
-  CK(cudaMemcpyAsync(c->h_flag, flag, sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(&nnz, static_cast<uint64_t*>(d_rp.p) + n_rows, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(c->h_flag.get(), flag, sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(&nnz, d_rp.get() + n_rows, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  if (c->h_flag[0] & 1u) return upload_aos_host_gather(c, slot, n_rows, r, target);
+  if (c->h_flag.get()[0] & 1u) return upload_aos_host_gather(c, slot, n_rows, r, target);
   if (upload_begin(c, slot, n_rows, nnz, st)) return 1;
   DataSlot& s = c->slots[slot];
-  CK(cudaMalloc(&d_ent.p, (nnz ? nnz : 1) * sizeof(AosEntry)));
-  CK(cudaMemcpyAsync(d_ent.p, r[first].data, nnz * sizeof(AosEntry), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(s.row_ptr, d_rp.p, (n_rows + 1) * sizeof(uint64_t), cudaMemcpyDeviceToDevice, st));
-  CK(cudaMemcpyAsync(s.target, target, n_rows * sizeof(float), cudaMemcpyHostToDevice, st));
-  CK(launch_aos_split(c, d_ent.p, nnz, s.col, s.val));
+  CK(alloc(d_ent, nnz));
+  CK(cudaMemcpyAsync(d_ent.get(), r[first].data, nnz * sizeof(AosEntry), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(s.row_ptr.get(), d_rp.get(), (n_rows + 1) * sizeof(uint64_t), cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemcpyAsync(s.target.get(), target, n_rows * sizeof(float), cudaMemcpyHostToDevice, st));
+  CK(launch_aos_split(c, st, d_ent.get(), nnz, s.col.get(), s.val.get()));
   if (upload_inspect(c, slot, st)) return 1;
   return upload_finish(c, slot);  // syncs: the temporaries may be released
 }
@@ -509,8 +437,8 @@ int fmb200_free_data(fmb200_ctx* c, int slot) {
   if (slot < 0 || slot >= FMB200_MAX_SLOTS) return fail("slot %d out of range", slot);
   if (bind(c)) return 1;
   CK(cudaStreamSynchronize(c->stream));
-  if (c->slots[slot].pending) CK(cudaEventSynchronize(c->slots[slot].ready));
-  free_slot(c->slots[slot]);
+  if (c->slots[slot].pending) CK(cudaEventSynchronize(c->slots[slot].ready.get()));
+  c->slots[slot] = DataSlot();
   return 0;
 }
 
@@ -537,8 +465,7 @@ int fmb200_set_params(fmb200_ctx* c, double w0, const double* w, const double* v
       for (uint32_t i = 0; i < n; i++) hv32[(size_t)i * kp + f] = (float)v[(size_t)f * n + i];
     CK(cudaMemcpyAsync(c->p64.base, h64.data(), h64.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
     CK(cudaMemcpyAsync(c->p32.base, h32.data(), h32.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-    // a fresh state: clear the divergence flag of the fixed-point accumulator (fm_rowlane.cu)
-    if (c->d_acc) CK(cudaMemsetAsync(c->d_acc + c->p32.n_floats, 0, sizeof(unsigned long long), c->stream));
+    CK(clear_acc_flag(c));
     CK(cudaStreamSynchronize(c->stream));
     c->peer_base_valid = false;
     c->hogwild_fresh = true;
@@ -555,7 +482,7 @@ int fmb200_get_params(fmb200_ctx* c, double* w0, double* w, double* v) {
     const int k = c->k, kp = c->kp;
     if (c->mode != FMB200_MODE_HOGWILD) {
       std::vector<double> pageable;
-      double* h = static_cast<double*>(c->h_stage);  // pinned staging for small models
+      double* h = reinterpret_cast<double*>(c->h_stage.get());  // pinned staging for small models
       if (h == nullptr) {
         pageable.resize(c->p64.n_doubles);
         h = pageable.data();
@@ -569,7 +496,7 @@ int fmb200_get_params(fmb200_ctx* c, double* w0, double* w, double* v) {
         for (uint32_t i = 0; i < n; i++) v[(size_t)f * n + i] = hv[(size_t)i * k + f];
     } else {
       std::vector<float> pageable;
-      float* h = static_cast<float*>(c->h_stage);
+      float* h = reinterpret_cast<float*>(c->h_stage.get());
       if (h == nullptr) {
         pageable.resize(c->p32.n_floats);
         h = pageable.data();
@@ -618,13 +545,13 @@ int fmb200_sync(fmb200_ctx* c) {
 int fmb200_sgd_epoch(fmb200_ctx* c, int slot, double* device_seconds) {
   NEED_CTX(c);
   if (bind(c)) return 1;
-  CK(cudaEventRecord(c->ev0, c->stream));
+  CK(cudaEventRecord(c->ev0.get(), c->stream));
   if (fmb200_sgd_epoch_async(c, slot)) return 1;
-  CK(cudaEventRecord(c->ev1, c->stream));
+  CK(cudaEventRecord(c->ev1.get(), c->stream));
   CK(cudaStreamSynchronize(c->stream));
   if (device_seconds) {
     float ms = 0.f;
-    CK(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
+    CK(cudaEventElapsedTime(&ms, c->ev0.get(), c->ev1.get()));
     *device_seconds = (double)ms * 1e-3;
   }
   return 0;
@@ -638,27 +565,21 @@ int fmb200_evaluate(fmb200_ctx* c, int slot, double* sum_sq_err, double* sum_abs
   const DataSlot& d = c->slots[slot];
   double sq = 0, ab = 0, ok = 0;
   if (d.n_rows > 0) {
-    const int nb = metric_blocks(c, d);
-    if (ensure_partials(c, nb)) return 1;
+    const int nb = grid_for(c, d.n_rows);
+    CK(grow(c->d_partials, c->n_partials, 3 * (uint64_t)nb));
     if (c->mode != FMB200_MODE_HOGWILD && c->hp.task == FMB200_TASK_REGRESSION) {
       // fp64 modes: the reference sums err*err and |err| left to right over the rows
       // (fm_learn.h:136-146); a tree reduction may differ in the last ulps and flip a printed
       // digit.  The kernel writes the per-row error, the host adds them in row order.
-      if (c->pred_cap < d.n_rows) {
-        if (c->d_pred) cudaFree(c->d_pred);
-        c->d_pred = nullptr;
-        c->pred_cap = 0;
-        CK(cudaMalloc(&c->d_pred, d.n_rows * sizeof(double)));
-        c->pred_cap = d.n_rows;
-      }
-      CK(launch_predict64(c, d, 2, c->d_pred, nullptr, nb));
+      CK(grow(c->d_pred, c->pred_cap, d.n_rows));
+      CK(launch_predict64(c, d, 2, c->d_pred.get(), nullptr, nb));
       std::vector<double> err;
       try {
         err.resize(d.n_rows);
       } catch (const std::bad_alloc&) {
         return fail("out of host memory");
       }
-      CK(cudaMemcpyAsync(err.data(), c->d_pred, d.n_rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+      CK(cudaMemcpyAsync(err.data(), c->d_pred.get(), d.n_rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
       CK(cudaStreamSynchronize(c->stream));
       for (uint64_t i = 0; i < d.n_rows; i++) {
         sq += err[i] * err[i];
@@ -666,9 +587,9 @@ int fmb200_evaluate(fmb200_ctx* c, int slot, double* sum_sq_err, double* sum_abs
       }
     } else {
       if (c->mode != FMB200_MODE_HOGWILD) {
-        CK(launch_predict64(c, d, 0, nullptr, c->d_partials, nb));
+        CK(launch_predict64(c, d, 0, nullptr, c->d_partials.get(), nb));
       } else {
-        CK(launch_predict32(c, d, 0, nullptr, c->d_partials, nb));
+        CK(launch_predict32(c, d, 0, nullptr, c->d_partials.get(), nb));
       }
       std::vector<double> h;
       try {
@@ -676,7 +597,7 @@ int fmb200_evaluate(fmb200_ctx* c, int slot, double* sum_sq_err, double* sum_abs
       } catch (const std::bad_alloc&) {
         return fail("out of host memory");
       }
-      CK(cudaMemcpyAsync(h.data(), c->d_partials, h.size() * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+      CK(cudaMemcpyAsync(h.data(), c->d_partials.get(), h.size() * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
       CK(cudaStreamSynchronize(c->stream));
       for (int b = 0; b < nb; b++) {  // fixed order: deterministic result
         sq += h[3 * b + 0];
@@ -698,20 +619,14 @@ int fmb200_predict(fmb200_ctx* c, int slot, int transform, double* out) {
   const DataSlot& d = c->slots[slot];
   if (d.n_rows == 0) return 0;
   if (!out) return fail("null output pointer");
-  if (c->pred_cap < d.n_rows) {
-    if (c->d_pred) cudaFree(c->d_pred);
-    c->d_pred = nullptr;
-    c->pred_cap = 0;
-    CK(cudaMalloc(&c->d_pred, d.n_rows * sizeof(double)));
-    c->pred_cap = d.n_rows;
-  }
-  const int nb = metric_blocks(c, d);
+  CK(grow(c->d_pred, c->pred_cap, d.n_rows));
+  const int nb = grid_for(c, d.n_rows);
   if (c->mode != FMB200_MODE_HOGWILD) {
-    CK(launch_predict64(c, d, transform, c->d_pred, nullptr, nb));
+    CK(launch_predict64(c, d, transform, c->d_pred.get(), nullptr, nb));
   } else {
-    CK(launch_predict32(c, d, transform, c->d_pred, nullptr, nb));
+    CK(launch_predict32(c, d, transform, c->d_pred.get(), nullptr, nb));
   }
-  CK(cudaMemcpyAsync(out, c->d_pred, d.n_rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaMemcpyAsync(out, c->d_pred.get(), d.n_rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -728,26 +643,24 @@ int fmb200_sgda_begin(fmb200_ctx* c, uint32_t n_groups, const uint32_t* attr_gro
   const size_t n1 = c->n ? c->n : 1, nk = (size_t)c->n * c->k ? (size_t)c->n * c->k : 1;
   const size_t gk = (size_t)n_groups * (c->k ? c->k : 1);
   if (!c->sgda_grad_w) {
-    CK(cudaMalloc(&c->sgda_grad_w, n1 * sizeof(double)));
-    CK(cudaMalloc(&c->sgda_grad_v, nk * sizeof(double)));
-    CK(cudaMalloc(&c->sgda_group, n1 * sizeof(uint32_t)));
+    CK(alloc(c->sgda_grad_w, n1));
+    CK(alloc(c->sgda_grad_v, nk));
+    CK(alloc(c->sgda_group, n1));
   }
   if (c->sgda_groups != n_groups) {
-    if (c->sgda_reg_w) cudaFree(c->sgda_reg_w);
-    if (c->sgda_reg_v) cudaFree(c->sgda_reg_v);
-    c->sgda_reg_w = c->sgda_reg_v = nullptr;
-    CK(cudaMalloc(&c->sgda_reg_w, n_groups * sizeof(double)));
-    CK(cudaMalloc(&c->sgda_reg_v, gk * sizeof(double)));
+    c->sgda_groups = 0;
+    CK(alloc(c->sgda_reg_w, n_groups));
+    CK(alloc(c->sgda_reg_v, gk));
     c->sgda_groups = n_groups;
   }
   // init(): grad_w = grad_v = 0 (:73-74); learn(): w = 0, reg_w = reg_v = 0 (:283-291)
-  CK(cudaMemsetAsync(c->sgda_grad_w, 0, n1 * sizeof(double), c->stream));
-  CK(cudaMemsetAsync(c->sgda_grad_v, 0, nk * sizeof(double), c->stream));
-  CK(cudaMemsetAsync(c->sgda_reg_w, 0, n_groups * sizeof(double), c->stream));
-  CK(cudaMemsetAsync(c->sgda_reg_v, 0, gk * sizeof(double), c->stream));
+  CK(cudaMemsetAsync(c->sgda_grad_w.get(), 0, n1 * sizeof(double), c->stream));
+  CK(cudaMemsetAsync(c->sgda_grad_v.get(), 0, nk * sizeof(double), c->stream));
+  CK(cudaMemsetAsync(c->sgda_reg_w.get(), 0, n_groups * sizeof(double), c->stream));
+  CK(cudaMemsetAsync(c->sgda_reg_v.get(), 0, gk * sizeof(double), c->stream));
   CK(cudaMemsetAsync(c->p64.w(), 0, n1 * sizeof(double), c->stream));
-  if (attr_group) CK(cudaMemcpyAsync(c->sgda_group, attr_group, c->n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
-  else CK(cudaMemsetAsync(c->sgda_group, 0, n1 * sizeof(uint32_t), c->stream));
+  if (attr_group) CK(cudaMemcpyAsync(c->sgda_group.get(), attr_group, c->n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+  else CK(cudaMemsetAsync(c->sgda_group.get(), 0, n1 * sizeof(uint32_t), c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -759,13 +672,13 @@ int fmb200_sgda_epoch(fmb200_ctx* c, int train_slot, int val_slot, int lambda_st
   if (c->mode == FMB200_MODE_HOGWILD) return fail("SGDA runs on the fp64 state: set INORDER or ORDERED mode first");
   if (c->sgda_groups == 0) return fail("call fmb200_sgda_begin first");
   if (c->k > 256) return fail("num_factor > 256 is not supported in the fp64 modes");
-  CK(cudaEventRecord(c->ev0, c->stream));
+  CK(cudaEventRecord(c->ev0.get(), c->stream));
   CK(launch_sgda_epoch(c, c->slots[train_slot], c->slots[val_slot], lambda_steps));
-  CK(cudaEventRecord(c->ev1, c->stream));
+  CK(cudaEventRecord(c->ev1.get(), c->stream));
   CK(cudaStreamSynchronize(c->stream));
   if (device_seconds) {
     float ms = 0.f;
-    CK(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
+    CK(cudaEventElapsedTime(&ms, c->ev0.get(), c->ev1.get()));
     *device_seconds = (double)ms * 1e-3;
   }
   return 0;
@@ -775,9 +688,9 @@ int fmb200_sgda_get_reg(fmb200_ctx* c, double* reg_w, double* reg_v) {
   NEED_CTX(c);
   if (bind(c)) return 1;
   if (c->sgda_groups == 0) return fail("call fmb200_sgda_begin first");
-  if (reg_w) CK(cudaMemcpyAsync(reg_w, c->sgda_reg_w, c->sgda_groups * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  if (reg_w) CK(cudaMemcpyAsync(reg_w, c->sgda_reg_w.get(), c->sgda_groups * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   if (reg_v && c->k)
-    CK(cudaMemcpyAsync(reg_v, c->sgda_reg_v, (size_t)c->sgda_groups * c->k * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaMemcpyAsync(reg_v, c->sgda_reg_v.get(), (size_t)c->sgda_groups * c->k * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -791,15 +704,9 @@ int fmb200_mcmc_eterms(fmb200_ctx* c, int slot, double* e_out) {
   const DataSlot& d = c->slots[slot];
   if (d.n_rows == 0) return 0;
   if (!e_out) return fail("null output pointer");
-  if (c->pred_cap < d.n_rows) {
-    if (c->d_pred) cudaFree(c->d_pred);
-    c->d_pred = nullptr;
-    c->pred_cap = 0;
-    CK(cudaMalloc(&c->d_pred, d.n_rows * sizeof(double)));
-    c->pred_cap = d.n_rows;
-  }
-  CK(launch_mcmc_eterms(c, d, c->d_pred));
-  CK(cudaMemcpyAsync(e_out, c->d_pred, d.n_rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  CK(grow(c->d_pred, c->pred_cap, d.n_rows));
+  CK(launch_mcmc_eterms(c, d, c->d_pred.get()));
+  CK(cudaMemcpyAsync(e_out, c->d_pred.get(), d.n_rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -818,7 +725,7 @@ int fmb200_mcmc_begin(fmb200_ctx* c, int train_slot, int test_slot, int do_sampl
     const std::string e = mcmc_begin(c, train_slot, test_slot, do_sample, do_multilevel, n_groups, attr_group,
                                       attr_per_group, reg0, w_lambda, v_lambda);
     if (!e.empty()) {
-      mcmc_free(c);
+      c->mcmc.reset();
       return fail("fmb200_mcmc_begin: %s", e.c_str());
     }
     return 0;
@@ -894,7 +801,7 @@ int fmb200_peer_export(fmb200_ctx* c, void* handle) {
   if (bind(c)) return 1;
   static_assert(sizeof(cudaIpcMemHandle_t) == FMB200_IPC_HANDLE_BYTES, "IPC handle size");
   cudaIpcMemHandle_t h;
-  CK(cudaIpcGetMemHandle(&h, c->comm_base));
+  CK(cudaIpcGetMemHandle(&h, c->comm_base.get()));
   memcpy(handle, &h, sizeof(h));
   return 0;
 }
@@ -915,7 +822,7 @@ int fmb200_peer_attach_ipc(fmb200_ctx* c, int world, int rank, const void* handl
   const unsigned char* hb = static_cast<const unsigned char*>(handles);
   for (int q = 0; q < world; q++) {
     if (q == rank) {
-      c->peer_base[q] = c->comm_base;
+      c->peer_base[q] = c->comm_base.get();
       continue;
     }
     cudaIpcMemHandle_t h;
@@ -947,7 +854,7 @@ int fmb200_peer_attach_local(fmb200_ctx* c, int world, int rank, fmb200_ctx* con
         return fail("cudaDeviceEnablePeerAccess failed: %s", cudaGetErrorString(e));
       (void)cudaGetLastError();
     }
-    c->peer_base[q] = all[q]->comm_base;
+    c->peer_base[q] = all[q]->comm_base.get();
   }
   CK(peer_preload_kernels());
   c->peer_world = world;
@@ -1015,10 +922,10 @@ int fmb200_download_data(fmb200_ctx* c, int slot, uint64_t* n_rows, uint64_t* nn
   const DataSlot& d = c->slots[slot];
   if (n_rows) *n_rows = d.n_rows;
   if (nnz) *nnz = d.nnz;
-  if (row_ptr) CK(cudaMemcpyAsync(row_ptr, d.row_ptr, (d.n_rows + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
-  if (col && d.nnz) CK(cudaMemcpyAsync(col, d.col, d.nnz * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
-  if (val && d.nnz) CK(cudaMemcpyAsync(val, d.val, d.nnz * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-  if (target && d.n_rows) CK(cudaMemcpyAsync(target, d.target, d.n_rows * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+  if (row_ptr) CK(cudaMemcpyAsync(row_ptr, d.row_ptr.get(), (d.n_rows + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
+  if (col && d.nnz) CK(cudaMemcpyAsync(col, d.col.get(), d.nnz * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+  if (val && d.nnz) CK(cudaMemcpyAsync(val, d.val.get(), d.nnz * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+  if (target && d.n_rows) CK(cudaMemcpyAsync(target, d.target.get(), d.n_rows * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return 0;
 }
@@ -1031,9 +938,9 @@ int fmb200_ordered_index(fmb200_ctx* c, int slot, uint32_t* link, uint32_t* rowd
   if (d.nnz >= 0xffffffffull) return fail("the ORDERED index needs nnz < 2^32-1");
   CK(build_ordered_links(c, d));
   if (link && d.nnz)
-    CK(cudaMemcpyAsync(link, d.link, d.nnz * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaMemcpyAsync(link, d.link.get(), d.nnz * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
   if (rowdep && d.n_rows)
-    CK(cudaMemcpyAsync(rowdep, d.rowdep, d.n_rows * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaMemcpyAsync(rowdep, d.rowdep.get(), d.n_rows * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return 0;
 }

@@ -359,10 +359,10 @@ static cudaError_t fit_grid(fmb200_ctx* c, HogwildKernelFn fn, int threads, int 
 static HogwildArgs make_args(fmb200_ctx* c, const DataSlot& d, uint64_t n_tiles, int TR,
                              uint32_t tile_cap, uint32_t sbytes) {
   HogwildArgs a;
-  a.row_ptr = d.row_ptr;
-  a.col = d.col;
-  a.val = d.val;
-  a.target = d.target;
+  a.row_ptr = d.row_ptr.get();
+  a.col = d.col.get();
+  a.val = d.val.get();
+  a.target = d.target.get();
   a.n_rows = d.n_rows;
   a.n_tiles = (uint32_t)n_tiles;
   a.tile_rows = TR;
@@ -382,7 +382,7 @@ static HogwildArgs make_args(fmb200_ctx* c, const DataSlot& d, uint64_t n_tiles,
   a.regv = (float)c->hp.regv;
   a.min_target = (float)c->hp.min_target;
   a.max_target = (float)c->hp.max_target;
-  a.feat_cnt = d.feat_cnt;
+  a.feat_cnt = d.feat_cnt.get();
   a.conc_scale = 1.f;
   a.w0_conc = 1.f;
   a.acc_w0 = a.acc_w = a.acc_v = a.acc_bad = a.acc = nullptr;
@@ -390,9 +390,18 @@ static HogwildArgs make_args(fmb200_ctx* c, const DataSlot& d, uint64_t n_tiles,
   a.n_acc = 0;
   a.ramp_tiles = 0;
   a.ramp_conc_scale = a.ramp_w0_conc = 1.f;
-  a.sched = c->d_sched;
+  a.sched = c->d_sched.get();
   a.global_entries = 0;
   return a;
+}
+
+// The fixed-point accumulator of the reproducible row-lane epoch: one u64 per float of the packed state,
+// then the flag word of acc_add (set when a step was not finite or too large for the fixed point).
+// Allocated zeroed on first use; every launch leaves the steps zero behind it.
+static unsigned long long* acc_flag(fmb200_ctx* c) { return c->d_acc.get() + c->p32.n_floats; }
+
+cudaError_t clear_acc_flag(fmb200_ctx* c) {
+  return c->d_acc ? cudaMemsetAsync(acc_flag(c), 0, sizeof(unsigned long long), c->stream) : cudaSuccess;
 }
 
 // one-lane-per-row variant (fm_rowlane.cu) for k <= 8 and rows of at most 4 entries
@@ -457,19 +466,19 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, const DataSlot& d, bool* handle
     // in flight), in one cooperative launch; each window reads the state the previous one left and
     // its steps are folded in after it: the same result on every run.  A ramp window is one tile.
     const uint64_t n_acc = c->p32.n_floats;
-    if (c->d_acc == nullptr) {  // + the flag word of acc_add
-      e = cudaMalloc(&c->d_acc, (n_acc + 1) * sizeof(unsigned long long));
-      if (e != cudaSuccess) return e;
-      e = cudaMemsetAsync(c->d_acc, 0, (n_acc + 1) * sizeof(unsigned long long), c->stream);
+    if (!c->d_acc) {
+      if ((e = alloc(c->d_acc, n_acc + 1)) != cudaSuccess) return e;
+      e = cudaMemsetAsync(c->d_acc.get(), 0, (n_acc + 1) * sizeof(unsigned long long), c->stream);
       if (e != cudaSuccess) return e;
     }
+    unsigned long long* acc = c->d_acc.get();
     float* base = c->p32.base;
-    a.acc_w0 = c->d_acc + (a.w0 - base);
-    a.acc_w = c->d_acc + (a.w - base);
-    a.acc_v = c->d_acc + (a.v - base);
-    a.acc_bad = c->d_acc + n_acc;
+    a.acc_w0 = acc + (a.w0 - base);
+    a.acc_w = acc + (a.w - base);
+    a.acc_v = acc + (a.v - base);
+    a.acc_bad = acc_flag(c);
     a.state = base;
-    a.acc = c->d_acc;
+    a.acc = acc;
     a.n_acc = n_acc;
     if (ramp) {
       a.ramp_tiles = (uint32_t)kRampTiles;

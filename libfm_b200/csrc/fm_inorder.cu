@@ -310,8 +310,8 @@ cudaError_t launch_mcmc_eterms(fmb200_ctx* c, const DataSlot& d, double* e_out) 
   if (d.n_rows == 0) return cudaSuccess;
   const uint64_t blocks = (d.n_rows + 127) / 128;
   const int grid = (int)(blocks < (uint64_t)c->sm_count * 16 ? blocks : (uint64_t)c->sm_count * 16);
-  fm_eterm64_kernel<<<grid, 128, 0, c->stream>>>(c->p64, c->k, c->k0, c->k1, d.n_rows, d.row_ptr, d.col, d.val,
-                                                 e_out);
+  fm_eterm64_kernel<<<grid, 128, 0, c->stream>>>(c->p64, c->k, c->k0, c->k1, d.n_rows, d.row_ptr.get(), d.col.get(),
+                                                 d.val.get(), e_out);
   c->launches++;
   return cudaGetLastError();
 }
@@ -516,11 +516,11 @@ cudaError_t launch_sgda_epoch(fmb200_ctx* c, const DataSlot& tr, const DataSlot&
   if (c->k > 32 * KF_MAX) return cudaErrorInvalidValue;
   SgdaArgs a;
   a.p = c->p64;
-  a.grad_w = c->sgda_grad_w;
-  a.grad_v = c->sgda_grad_v;
-  a.reg_w = c->sgda_reg_w;
-  a.reg_v = c->sgda_reg_v;
-  a.group = c->sgda_group;
+  a.grad_w = c->sgda_grad_w.get();
+  a.grad_v = c->sgda_grad_v.get();
+  a.reg_w = c->sgda_reg_w.get();
+  a.reg_v = c->sgda_reg_v.get();
+  a.group = c->sgda_group.get();
   a.n_groups = c->sgda_groups;
   a.k = c->k;
   a.use_w0 = c->k0;
@@ -528,15 +528,15 @@ cudaError_t launch_sgda_epoch(fmb200_ctx* c, const DataSlot& tr, const DataSlot&
   a.lambda_steps = lambda_steps;
   a.hp = c->hp;
   a.n_rows = tr.n_rows;
-  a.row_ptr = tr.row_ptr;
-  a.col = tr.col;
-  a.val = tr.val;
-  a.target = tr.target;
+  a.row_ptr = tr.row_ptr.get();
+  a.col = tr.col.get();
+  a.val = tr.val.get();
+  a.target = tr.target.get();
   a.v_rows = va.n_rows;
-  a.v_row_ptr = va.row_ptr;
-  a.v_col = va.col;
-  a.v_val = va.val;
-  a.v_target = va.target;
+  a.v_row_ptr = va.row_ptr.get();
+  a.v_col = va.col.get();
+  a.v_val = va.val.get();
+  a.v_target = va.target.get();
   const size_t smem = sizeof(double) * ((size_t)c->sgda_groups * (2 + 3 * (size_t)c->k));
   if (smem > (size_t)c->max_smem_optin) return cudaErrorInvalidConfiguration;
   const int kf = (c->k + 31) / 32;
@@ -565,8 +565,8 @@ cudaError_t launch_sgd_inorder(fmb200_ctx* c, const DataSlot& d) {
   if (c->tune_variant != 1 && c->k <= WF_K && d.max_row_nnz <= (uint32_t)WF_Z && d.n_rows > 0) {
 #define FMB_WAVEFRONT(K0, TASK)                                                                       \
   fm_sgd_inorder_wavefront_kernel<K0, TASK><<<1, 32, 0, c->stream>>>(c->p64, c->k, c->k0, c->k1, c->hp, \
-                                                                     d.n_rows, d.row_ptr, d.col, d.val, \
-                                                                     d.target)
+                                                                     d.n_rows, d.row_ptr.get(), d.col.get(),  \
+                                                                     d.val.get(), d.target.get())
     const bool reg = c->hp.task == FMB200_TASK_REGRESSION;
     if (c->k0 && reg) FMB_WAVEFRONT(true, FMB200_TASK_REGRESSION);
     else if (c->k0) FMB_WAVEFRONT(true, FMB200_TASK_CLASSIFICATION);
@@ -580,7 +580,7 @@ cudaError_t launch_sgd_inorder(fmb200_ctx* c, const DataSlot& d) {
   const int kf = (c->k + 31) / 32;
 #define FMB_INORDER(KF)                                                                         \
   fm_sgd_inorder_kernel<KF><<<1, 32, 0, c->stream>>>(c->p64, c->k, c->k0, c->k1, c->hp, d.n_rows, \
-                                                     d.row_ptr, d.col, d.val, d.target)
+                                                     d.row_ptr.get(), d.col.get(), d.val.get(), d.target.get())
   if (kf <= 1) FMB_INORDER(1);
   else if (kf <= 2) FMB_INORDER(2);
   else if (kf <= 4) FMB_INORDER(4);
@@ -597,8 +597,9 @@ cudaError_t launch_predict64(fmb200_ctx* c, const DataSlot& d, int transform, do
   const int kf = (c->k + 31) / 32;
 #define FMB_PREDICT64(KF)                                                                          \
   fm_predict64_kernel<KF><<<n_blocks, 256, 0, c->stream>>>(c->p64, c->k, c->k0, c->k1, c->hp,      \
-                                                           transform, d.n_rows, d.row_ptr, d.col, \
-                                                           d.val, d.target, out_pred, partials)
+                                                           transform, d.n_rows, d.row_ptr.get(),     \
+                                                           d.col.get(), d.val.get(), d.target.get(), \
+                                                           out_pred, partials)
   if (kf <= 1) FMB_PREDICT64(1);
   else if (kf <= 2) FMB_PREDICT64(2);
   else if (kf <= 4) FMB_PREDICT64(4);

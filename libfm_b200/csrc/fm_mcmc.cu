@@ -24,7 +24,6 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
-#include <memory>
 #include <vector>
 
 #include "fm_roworder.cuh"
@@ -56,23 +55,14 @@ struct McmcState {
   uint32_t iter = 0;
   uint32_t counters[16] = {0};
   // device
-  uint32_t *col_ptr = nullptr, *cs_case = nullptr, *dup = nullptr, *group_d = nullptr, *runs_d = nullptr;
-  float* cs_x = nullptr;
-  double *e_d = nullptr, *q_d = nullptr, *e_test_d = nullptr, *z_d = nullptr, *hyp_d = nullptr;
-  unsigned int* flag_d = nullptr;
+  DevPtr<uint32_t> col_ptr, cs_case, dup, group_d, runs_d;
+  DevPtr<float> cs_x;
+  DevPtr<double> e_d, q_d, e_test_d, z_d, hyp_d;
+  DevPtr<unsigned int> flag_d;
   int grid = 0;
 };
 
-void mcmc_free(fmb200_ctx* c) {
-  McmcState* s = c->mcmc;
-  if (!s) return;
-  for (void* p : {(void*)s->col_ptr, (void*)s->cs_case, (void*)s->dup, (void*)s->group_d, (void*)s->runs_d,
-                  (void*)s->cs_x, (void*)s->e_d, (void*)s->q_d, (void*)s->e_test_d, (void*)s->z_d,
-                  (void*)s->hyp_d, (void*)s->flag_d})
-    if (p) cudaFree(p);
-  delete s;
-  c->mcmc = nullptr;
-}
+void McmcDelete::operator()(McmcState* s) const { delete s; }
 
 namespace {
 
@@ -163,11 +153,6 @@ double as_erf(double x) {
 double cdf_gaussian(double x) { return 0.5 + 0.5 * as_erf(0.707106781 * x); }
 
 // ---- device: index build -------------------------------------------------------------------
-int grid_of(const fmb200_ctx* c, uint64_t work) {
-  const uint64_t b = (work + 255) / 256, cap = (uint64_t)c->sm_count * 8;
-  return (int)std::max<uint64_t>(1, std::min(b, cap));
-}
-
 __device__ __forceinline__ uint32_t row_of(const uint64_t* rp, uint64_t n_rows, uint64_t e) {
   uint64_t lo = 0, hi = n_rows;  // largest r with rp[r] <= e
   while (hi - lo > 1) {
@@ -386,19 +371,13 @@ __global__ void __launch_bounds__(256) mcmc_sweep_kernel(const SweepArgs a) {
 
 namespace {
 
-template <class T>
-std::string dalloc(T** p, size_t count) {
-  MK(cudaMalloc(p, sizeof(T) * (count ? count : 1)));
-  return "";
-}
-
 std::string repredict(fmb200_ctx* c, McmcState& s) {
   const DataSlot& tr = c->slots[s.train];
   const DataSlot& te = c->slots[s.test];
-  MK(launch_mcmc_eterms(c, tr, s.e_d));
-  MK(launch_mcmc_eterms(c, te, s.e_test_d));
-  MK(cudaMemcpyAsync(s.e.data(), s.e_d, tr.n_rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  if (te.n_rows) MK(cudaMemcpyAsync(s.e_test.data(), s.e_test_d, te.n_rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  MK(launch_mcmc_eterms(c, tr, s.e_d.get()));
+  MK(launch_mcmc_eterms(c, te, s.e_test_d.get()));
+  MK(cudaMemcpyAsync(s.e.data(), s.e_d.get(), tr.n_rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  if (te.n_rows) MK(cudaMemcpyAsync(s.e_test.data(), s.e_test_d.get(), te.n_rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   MK(cudaStreamSynchronize(c->stream));
   return "";
 }
@@ -413,10 +392,8 @@ std::string mcmc_begin(fmb200_ctx* c, int train, int test, int do_sample, int do
   if (d.n_rows == 0) return "the training set is empty";
   if (d.n_rows >= 0xffffffffull || d.nnz >= 0xffffffffull) return "training sets of 2^32 cases or entries and more are not supported";
   if (G == 0) return "n_groups must be >= 1";
-  mcmc_free(c);
-  McmcState* sp = new McmcState();
-  c->mcmc = sp;
-  McmcState& s = *sp;
+  c->mcmc.reset(new McmcState());
+  McmcState& s = *c->mcmc;
   const uint32_t n = c->n;
   const int k = c->k;
   s.train = train;
@@ -449,41 +426,40 @@ std::string mcmc_begin(fmb200_ctx* c, int train, int test, int do_sample, int do
   s.pred_this.assign(dt.n_rows, 0.0);
   s.pred_all.assign(dt.n_rows, 0.0);
   s.pred_but5.assign(dt.n_rows, 0.0);
-  std::string err;
-  if (!(err = dalloc(&s.col_ptr, n + 1)).empty() || !(err = dalloc(&s.cs_case, d.nnz)).empty() ||
-      !(err = dalloc(&s.cs_x, d.nnz)).empty() || !(err = dalloc(&s.dup, n)).empty() ||
-      !(err = dalloc(&s.group_d, n)).empty() || !(err = dalloc(&s.e_d, d.n_rows)).empty() ||
-      !(err = dalloc(&s.q_d, d.n_rows)).empty() || !(err = dalloc(&s.e_test_d, dt.n_rows)).empty() ||
-      !(err = dalloc(&s.z_d, (size_t)(k + 1) * n)).empty() || !(err = dalloc(&s.hyp_d, 2 * G + 2 * (size_t)G * k)).empty() ||
-      !(err = dalloc(&s.flag_d, F_WORDS)).empty())
-    return err;
-  MK(cudaMemcpyAsync(s.y.data(), d.target, d.n_rows * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-  if (dt.n_rows) MK(cudaMemcpyAsync(s.y_test.data(), dt.target, dt.n_rows * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-  MK(cudaMemcpyAsync(s.group_d, s.group.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
-  MK(cudaMemsetAsync(s.dup, 0, n * sizeof(uint32_t), c->stream));
+  MK(alloc(s.col_ptr, n + 1));
+  MK(alloc(s.cs_case, d.nnz));
+  MK(alloc(s.cs_x, d.nnz));
+  MK(alloc(s.dup, n));
+  MK(alloc(s.group_d, n));
+  MK(alloc(s.e_d, d.n_rows));
+  MK(alloc(s.q_d, d.n_rows));
+  MK(alloc(s.e_test_d, dt.n_rows));
+  MK(alloc(s.z_d, (size_t)(k + 1) * n));
+  MK(alloc(s.hyp_d, 2 * G + 2 * (size_t)G * k));
+  MK(alloc(s.flag_d, F_WORDS));
+  MK(cudaMemcpyAsync(s.y.data(), d.target.get(), d.n_rows * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+  if (dt.n_rows) MK(cudaMemcpyAsync(s.y_test.data(), dt.target.get(), dt.n_rows * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+  MK(cudaMemcpyAsync(s.group_d.get(), s.group.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+  MK(cudaMemsetAsync(s.dup.get(), 0, n * sizeof(uint32_t), c->stream));
 
   // transposed training data + feature runs, from the (id, entry) sort of the ORDERED index
   std::vector<uint32_t> prev(n, 0u);
   if (d.nnz > 0) {
-    if (d.links_ready && !d.ord_scratch) d.links_ready = false;  // a large set released its sort: redo it
-    MK(build_ordered_links(c, d, true));
-    const size_t words = ((size_t)d.nnz + 63) & ~(size_t)63;
-    const uint32_t* ids = static_cast<const uint32_t*>(d.ord_scratch);
-    const uint32_t* ent = ids + 2 * words;
-    mcmc_csc_kernel<<<grid_of(c, d.nnz), 256, 0, c->stream>>>(ids, ent, d.nnz, d.row_ptr, d.n_rows, d.val, s.cs_case,
-                                                              s.cs_x, s.dup);
-    mcmc_colptr_kernel<<<grid_of(c, (uint64_t)n + 1), 256, 0, c->stream>>>(ids, d.nnz, n, s.col_ptr);
-    unsigned int* prev_d = nullptr;
-    if (!(err = dalloc(&prev_d, n)).empty()) return err;
-    std::unique_ptr<unsigned int, cudaError_t (*)(void*)> prev_owner(prev_d, cudaFree);
-    MK(cudaMemsetAsync(prev_d, 0, n * sizeof(unsigned int), c->stream));
-    mcmc_prev_kernel<<<grid_of(c, d.n_rows), 256, 0, c->stream>>>(d.row_ptr, d.col, d.n_rows, prev_d);
+    SortedEntries se;
+    MK(build_ordered_links(c, d, &se));
+    mcmc_csc_kernel<<<grid_for(c, d.nnz), 256, 0, c->stream>>>(se.ids, se.ent, d.nnz, d.row_ptr.get(), d.n_rows,
+                                                               d.val.get(), s.cs_case.get(), s.cs_x.get(), s.dup.get());
+    mcmc_colptr_kernel<<<grid_for(c, (uint64_t)n + 1), 256, 0, c->stream>>>(se.ids, d.nnz, n, s.col_ptr.get());
+    DevPtr<unsigned int> prev_d;
+    MK(alloc(prev_d, n));
+    MK(cudaMemsetAsync(prev_d.get(), 0, n * sizeof(unsigned int), c->stream));
+    mcmc_prev_kernel<<<grid_for(c, d.n_rows), 256, 0, c->stream>>>(d.row_ptr.get(), d.col.get(), d.n_rows, prev_d.get());
     c->launches += 3;
     MK(cudaGetLastError());
-    MK(cudaMemcpyAsync(prev.data(), prev_d, n * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+    MK(cudaMemcpyAsync(prev.data(), prev_d.get(), n * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
     MK(cudaStreamSynchronize(c->stream));
   } else {
-    MK(cudaMemsetAsync(s.col_ptr, 0, (n + 1) * sizeof(uint32_t), c->stream));
+    MK(cudaMemsetAsync(s.col_ptr.get(), 0, (n + 1) * sizeof(uint32_t), c->stream));
   }
   MK(cudaStreamSynchronize(c->stream));
   // cut greedily: j opens a new run when it shares a case with a feature of the current run
@@ -492,8 +468,8 @@ std::string mcmc_begin(fmb200_ctx* c, int train, int test, int do_sample, int do
   for (uint32_t j = 1; j < n; j++)
     if (prev[j] != 0 && prev[j] - 1 >= s.runs.back()) s.runs.push_back(j);
   s.runs.push_back(n);
-  if (!(err = dalloc(&s.runs_d, s.runs.size())).empty()) return err;
-  MK(cudaMemcpyAsync(s.runs_d, s.runs.data(), s.runs.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+  MK(alloc(s.runs_d, s.runs.size()));
+  MK(cudaMemcpyAsync(s.runs_d.get(), s.runs.data(), s.runs.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
 
   int occ = 0;
   MK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, mcmc_sweep_kernel, 256, 0));
@@ -501,9 +477,10 @@ std::string mcmc_begin(fmb200_ctx* c, int train, int test, int do_sample, int do
   s.grid = occ * c->sm_count;
 
   // fm_learn_mcmc_simultaneous.h:69-86: predict, then e := prediction - target (both tasks)
-  if (!(err = repredict(c, s)).empty()) return err;
+  const std::string err = repredict(c, s);
+  if (!err.empty()) return err;
   for (uint64_t i = 0; i < d.n_rows; i++) s.e[i] = s.e[i] - s.y[i];
-  MK(cudaMemcpyAsync(s.e_d, s.e.data(), d.n_rows * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  MK(cudaMemcpyAsync(s.e_d.get(), s.e.data(), d.n_rows * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   MK(cudaStreamSynchronize(c->stream));
   s.state.resize(c->p64.n_doubles);
   s.z.resize((size_t)(k + 1) * n);
@@ -524,8 +501,8 @@ std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counte
   uint32_t* cnt = s.counters;  // nan, inf of: alpha, w0, w, v, w_mu, w_lambda, v_mu, v_lambda
   std::fill(cnt, cnt + 16, 0u);
   MK(cudaMemcpyAsync(s.state.data(), c->p64.base, s.state.size() * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  MK(cudaMemsetAsync(s.flag_d, 0, F_SKIP * sizeof(unsigned int), c->stream));
-  MK(cudaMemsetAsync(s.flag_d + F_SKIP, 0xff, sizeof(unsigned int), c->stream));
+  MK(cudaMemsetAsync(s.flag_d.get(), 0, F_SKIP * sizeof(unsigned int), c->stream));
+  MK(cudaMemsetAsync(s.flag_d.get() + F_SKIP, 0xff, sizeof(unsigned int), c->stream));
   MK(cudaStreamSynchronize(c->stream));
   double& w0 = s.state[0];
   const double* w = s.state.data() + Params64::off_w;
@@ -644,24 +621,24 @@ std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counte
   std::copy(s.v_mu.begin(), s.v_mu.end(), s.hyp.begin() + 2 * G);
   std::copy(s.v_lambda.begin(), s.v_lambda.end(), s.hyp.begin() + 2 * G + (size_t)G * k);
   MK(cudaMemcpyAsync(c->p64.w0(), &w0, sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  MK(cudaMemcpyAsync(s.hyp_d, s.hyp.data(), s.hyp.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  if (sample) MK(cudaMemcpyAsync(s.z_d, s.z.data(), s.z.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  MK(cudaMemcpyAsync(s.hyp_d.get(), s.hyp.data(), s.hyp.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  if (sample) MK(cudaMemcpyAsync(s.z_d.get(), s.z.data(), s.z.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   SweepArgs a{};
-  a.col_ptr = s.col_ptr;
-  a.cs_case = s.cs_case;
-  a.cs_x = s.cs_x;
-  a.dup = s.dup;
-  a.group = s.group_d;
-  a.runs = s.runs_d;
+  a.col_ptr = s.col_ptr.get();
+  a.cs_case = s.cs_case.get();
+  a.cs_x = s.cs_x.get();
+  a.dup = s.dup.get();
+  a.group = s.group_d.get();
+  a.runs = s.runs_d.get();
   a.n_runs = (uint32_t)s.runs.size() - 1;
   a.n = n;
   a.G = G;
-  a.row_ptr = d.row_ptr;
-  a.col = d.col;
-  a.val = d.val;
+  a.row_ptr = d.row_ptr.get();
+  a.col = d.col.get();
+  a.val = d.val.get();
   a.n_rows = N;
-  a.e = s.e_d;
-  a.q = s.q_d;
+  a.e = s.e_d.get();
+  a.q = s.q_d.get();
   a.w = c->p64.w();
   a.v = c->p64.v();
   a.k = k;
@@ -670,16 +647,16 @@ std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counte
   a.shift = shift;
   a.alpha = alpha;
   a.e_shift = e_shift;
-  a.z = s.z_d;
-  a.hyp = s.hyp_d;
-  a.flag = s.flag_d;
+  a.z = s.z_d.get();
+  a.hyp = s.hyp_d.get();
+  a.flag = s.flag_d.get();
   if (a.shift || a.use_w || k > 0) {
     void* args[] = {(void*)&a};
     MK(cudaLaunchCooperativeKernel((const void*)mcmc_sweep_kernel, dim3(s.grid), dim3(256), args, 0, c->stream));
     c->launches++;
   }
   unsigned int flag[F_WORDS];
-  MK(cudaMemcpyAsync(flag, s.flag_d, sizeof(flag), cudaMemcpyDeviceToHost, c->stream));
+  MK(cudaMemcpyAsync(flag, s.flag_d.get(), sizeof(flag), cudaMemcpyDeviceToHost, c->stream));
   MK(cudaStreamSynchronize(c->stream));
   cnt[4] = flag[F_NAN_W];
   cnt[5] = flag[F_INF_W];
@@ -715,7 +692,7 @@ std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counte
       rmse += er * er;
     }
     *train_metric = std::sqrt(rmse / N);
-    mcmc_residual_kernel<<<grid_of(c, N), 256, 0, c->stream>>>(s.e_d, d.target, N);
+    mcmc_residual_kernel<<<grid_for(c, N), 256, 0, c->stream>>>(s.e_d.get(), d.target.get(), N);
     c->launches++;
     MK(cudaGetLastError());
     for (uint64_t t = 0; t < N; t++) s.e[t] = s.e[t] - s.y[t];
@@ -750,7 +727,7 @@ std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counte
       s.e[t] = s.e[t] - st;
     }
     *train_metric = (double)acc / N;
-    MK(cudaMemcpyAsync(s.e_d, s.e.data(), N * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    MK(cudaMemcpyAsync(s.e_d.get(), s.e.data(), N * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   }
   MK(cudaStreamSynchronize(c->stream));
   s.iter++;
@@ -762,7 +739,7 @@ std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counte
 
 bool mcmc_get(const fmb200_ctx* c, double* alpha, double* w_mu, double* w_lambda, double* v_mu, double* v_lambda,
               double* pred_this, double* pred_sum_all, double* pred_sum_all_but5, uint32_t* n_runs) {
-  const McmcState* s = c->mcmc;
+  const McmcState* s = c->mcmc.get();
   if (!s) return false;
   if (alpha) *alpha = s->alpha;
   if (w_mu) std::copy(s->w_mu.begin(), s->w_mu.end(), w_mu);

@@ -151,38 +151,40 @@ OrdFn pick_kernel(int k) {
   return fm_sgd_ordered_kernel<32, 8, TASK>;
 }
 
-int grid_for(const fmb200_ctx* c, uint64_t work) {
-  const uint64_t blocks = (work + 255) / 256;
-  const uint64_t cap = (uint64_t)c->sm_count * 8;
-  return (int)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap));
+// the stable (id, entry) sort in the scratch of the index build, [ids | ent_in | ent | sort temp]
+SortedEntries sorted_view(const DataSlot& d) {
+  const size_t words = ((size_t)d.nnz + 63) & ~(size_t)63;
+  const uint32_t* ids = reinterpret_cast<const uint32_t*>(d.ord_scratch.get());
+  return SortedEntries{ids, ids + 2 * words};
 }
 
 }  // namespace
 
-// Build link[] / rowdep[] of a data set on c->stream (no host sync).
-cudaError_t build_ordered_links(fmb200_ctx* c, DataSlot& d, bool keep_scratch) {
-  if (d.links_ready) return cudaSuccess;
+cudaError_t build_ordered_links(fmb200_ctx* c, DataSlot& d, SortedEntries* sorted) {
+  // (a large data set releases its sort once the index is built: a caller that needs it rebuilds)
+  if (d.links_ready && !(sorted && d.nnz > 0 && !d.ord_scratch)) {
+    if (sorted) *sorted = sorted_view(d);
+    return cudaSuccess;
+  }
   if (d.nnz >= 0xffffffffull) return cudaErrorInvalidValue;
   cudaError_t e;
-  const uint64_t cap_e = d.cap_nnz + 16, cap_r = d.cap_rows + 520;
-  if (!d.link) {
-    if ((e = cudaMalloc(&d.link, cap_e * sizeof(uint32_t))) != cudaSuccess) return e;
-    if ((e = cudaMalloc(&d.rowdep, (cap_r + 4) * sizeof(uint32_t))) != cudaSuccess) return e;  // + the shape word
-  }
-  d.ord_shape = d.rowdep + cap_r;
+  const uint64_t cap_e = d.cap_nnz + kEntrySlack, cap_r = d.cap_rows + kRowSlack;
+  if ((e = grow(d.link, d.link_cap, cap_e)) != cudaSuccess) return e;
+  if ((e = grow(d.rowdep, d.rowdep_cap, cap_r + 4)) != cudaSuccess) return e;  // + the shape word
+  d.ord_shape = d.rowdep.get() + cap_r;
   {
     if ((e = cudaMemsetAsync(d.ord_shape, 0x03, sizeof(uint32_t), c->stream)) != cudaSuccess) return e;
-    ord_shape_kernel<<<grid_for(c, d.nnz + d.n_rows), 256, 0, c->stream>>>(d.val, d.nnz, d.row_ptr, d.n_rows,
-                                                                           d.max_row_nnz, d.ord_shape);
+    ord_shape_kernel<<<grid_for(c, d.nnz + d.n_rows), 256, 0, c->stream>>>(d.val.get(), d.nnz, d.row_ptr.get(),
+                                                                           d.n_rows, d.max_row_nnz, d.ord_shape);
     c->launches++;
   }
-  if ((e = cudaMemsetAsync(d.link, 0xff, cap_e * sizeof(uint32_t), c->stream)) != cudaSuccess) return e;
-  if ((e = cudaMemsetAsync(d.rowdep, 0xff, cap_r * sizeof(uint32_t), c->stream)) != cudaSuccess) return e;
+  if ((e = cudaMemsetAsync(d.link.get(), 0xff, cap_e * sizeof(uint32_t), c->stream)) != cudaSuccess) return e;
+  if ((e = cudaMemsetAsync(d.rowdep.get(), 0xff, cap_r * sizeof(uint32_t), c->stream)) != cudaSuccess) return e;
   if (d.nnz > 0) {
     int bits = 1;
     while (bits < 32 && (1ull << bits) < (uint64_t)c->n) bits++;
     size_t tmp_bytes = 0;
-    e = cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, d.col, (uint32_t*)nullptr, (const uint32_t*)nullptr,
+    e = cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, d.col.get(), (uint32_t*)nullptr, (const uint32_t*)nullptr,
                                         (uint32_t*)nullptr, (uint64_t)d.nnz, 0, bits, c->stream);
     if (e != cudaSuccess) return e;
     // scratch of the index build: [ids | ent_in | ent | sort temp].  Kept with the slot for data sets up to
@@ -190,31 +192,27 @@ cudaError_t build_ordered_links(fmb200_ctx* c, DataSlot& d, bool keep_scratch) {
     // end-to-end path uploads a fresh data set every step); larger ones release it right away.
     const size_t words = ((size_t)d.nnz + 63) & ~(size_t)63;
     const size_t need = 3 * words * sizeof(uint32_t) + ((tmp_bytes + 255) & ~(size_t)255) + 256;
-    if (d.ord_scratch_bytes < need) {
-      if (d.ord_scratch) cudaFree(d.ord_scratch);
-      d.ord_scratch = nullptr;
-      d.ord_scratch_bytes = 0;
-      if ((e = cudaMalloc(&d.ord_scratch, need)) != cudaSuccess) return e;
-      d.ord_scratch_bytes = need;
-    }
-    uint32_t* ids = static_cast<uint32_t*>(d.ord_scratch);
+    if ((e = grow(d.ord_scratch, d.ord_scratch_bytes, need)) != cudaSuccess) return e;
+    uint32_t* ids = reinterpret_cast<uint32_t*>(d.ord_scratch.get());
     uint32_t* ent_in = ids + words;
     uint32_t* ent = ent_in + words;
     void* tmp = ent + words;
     ord_iota_kernel<<<grid_for(c, d.nnz), 256, 0, c->stream>>>(ent_in, d.nnz);
-    e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, d.col, ids, ent_in, ent, (uint64_t)d.nnz, 0, bits, c->stream);
+    e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, d.col.get(), ids, ent_in, ent, (uint64_t)d.nnz, 0, bits,
+                                        c->stream);
     if (e != cudaSuccess) return e;
-    ord_link_kernel<<<grid_for(c, d.nnz), 256, 0, c->stream>>>(ids, ent, d.nnz, d.row_ptr, d.n_rows, d.link, d.rowdep);
+    ord_link_kernel<<<grid_for(c, d.nnz), 256, 0, c->stream>>>(ids, ent, d.nnz, d.row_ptr.get(), d.n_rows,
+                                                                d.link.get(), d.rowdep.get());
     if ((e = cudaGetLastError()) != cudaSuccess) return e;
     c->launches += 3;  // iota, link + the library's sort passes counted as one
-    if (d.nnz > (64ull << 20) && !keep_scratch) {
+    if (d.nnz > (64ull << 20) && !sorted) {
       if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) return e;
-      cudaFree(d.ord_scratch);
-      d.ord_scratch = nullptr;
+      d.ord_scratch.reset();
       d.ord_scratch_bytes = 0;
     }
   }
   d.links_ready = true;
+  if (sorted) *sorted = sorted_view(d);
   return cudaSuccess;
 }
 
@@ -267,12 +265,12 @@ cudaError_t launch_sgd_ordered(fmb200_ctx* c, DataSlot& d, bool* handled) {
   if (e != cudaSuccess) return e;
 
   OrderedArgs a{};
-  a.row_ptr = d.row_ptr;
-  a.col = d.col;
-  a.val = d.val;
-  a.target = d.target;
-  a.link = d.link;
-  a.rowdep = d.rowdep;
+  a.row_ptr = d.row_ptr.get();
+  a.col = d.col.get();
+  a.val = d.val.get();
+  a.target = d.target.get();
+  a.link = d.link.get();
+  a.rowdep = d.rowdep.get();
   a.shape = d.ord_shape;
   a.n_rows = d.n_rows;
   a.n_tiles = (uint32_t)((d.n_rows + TR - 1) / TR);

@@ -45,9 +45,9 @@ struct PeerArgs {
 };
 
 __global__ void __launch_bounds__(256) fm_peer_mean_kernel(const PeerArgs a) {
-  if (blockIdx.x == 0 && threadIdx.x < a.world) st_release_sys(a.flags[threadIdx.x] + a.rank, a.seq);
+  if (blockIdx.x == 0 && threadIdx.x < a.world) st_release_sys(a.flags[threadIdx.x] + COMM_SEQ_WORD + a.rank, a.seq);
   if (threadIdx.x < a.world) {
-    const unsigned int* mine = a.flags[a.rank] + threadIdx.x;
+    const unsigned int* mine = a.flags[a.rank] + COMM_SEQ_WORD + threadIdx.x;
     while ((int)(ld_acquire_sys(mine) - a.seq) < 0) {
     }
   }
@@ -121,9 +121,9 @@ __device__ __forceinline__ float mf_gamma(float u, float G) {
 // header of both mean-field kernels: the leading barrier, h_V from the previous exchange's partials
 // (fixed order: identical in every block of every rank), the bias' gamma.  Returns (hv, g0).
 __device__ __forceinline__ void mf_barrier(const PeerArgs& p) {
-  if (blockIdx.x == 0 && threadIdx.x < p.world) st_release_sys(p.flags[threadIdx.x] + p.rank, p.seq);
+  if (blockIdx.x == 0 && threadIdx.x < p.world) st_release_sys(p.flags[threadIdx.x] + COMM_SEQ_WORD + p.rank, p.seq);
   if (threadIdx.x < p.world) {
-    const unsigned int* mine = p.flags[p.rank] + threadIdx.x;
+    const unsigned int* mine = p.flags[p.rank] + COMM_SEQ_WORD + threadIdx.x;
     while ((int)(ld_acquire_sys(mine) - p.seq) < 0) {
     }
   }
@@ -138,15 +138,16 @@ __global__ void __launch_bounds__(256) fm_peer_counts_mean_kernel(const MeanFiel
   const PeerArgs& p = a.p;
   mf_barrier(p);
   const float G = (float)p.world;
-  if (blockIdx.x == 0) {  // rows per shard (the peers' header words [64 + 16 parity + rank]), averaged in rank order
+  if (blockIdx.x == 0) {  // rows per shard (the peers' row-count words of this parity), averaged in rank order
     __shared__ unsigned int s_rows[FMB200_MAX_PEERS];
     if ((int)threadIdx.x < p.world)
-      s_rows[threadIdx.x] = __ldcv(p.flags[threadIdx.x] + 64 + 16 * (p.seq & 1u) + threadIdx.x);
+      s_rows[threadIdx.x] =
+          __ldcv(p.flags[threadIdx.x] + COMM_ROWS_WORD + COMM_ROWS_PARITY_STRIDE * (p.seq & 1u) + threadIdx.x);
     __syncthreads();
     if (threadIdx.x == 0) {
       float rows = 0.f;
       for (int q = 0; q < p.world; q++) rows += (float)s_rows[q];
-      p.flags[p.rank][100 + (p.seq & 1u)] = __float_as_uint(rows / G);
+      p.flags[p.rank][COMM_MEAN_ROWS_WORD + (p.seq & 1u)] = __float_as_uint(rows / G);
     }
   }
   for (uint64_t f = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; f < a.n; f += (uint64_t)gridDim.x * blockDim.x) {
@@ -178,7 +179,7 @@ __device__ __forceinline__ void mf_prologue(const MeanFieldArgs& a, float* s_red
   __syncthreads();
   // mean rows per shard: left in the LOCAL header by fm_peer_counts_mean_kernel (a loop over the peers' words
   // here was 8 NVLink round trips, one after the other, in every block's prologue at G = 8)
-  const float rows = __uint_as_float(__ldcv(p.flags[p.rank] + 100 + (p.seq & 1u)));
+  const float rows = __uint_as_float(__ldcv(p.flags[p.rank] + COMM_MEAN_ROWS_WORD + (p.seq & 1u)));
   *g0_out = mf_gamma(a.lr * (1.f + a.reg0) * rows, G);
 }
 
@@ -325,8 +326,8 @@ __global__ void fm_peer_counts_kernel(const float* __restrict__ src, float* __re
 // blocks, on its own flag row and sequence so it never interferes with the averaging.
 __global__ void fm_peer_barrier_kernel(const PeerArgs a) {
   if (threadIdx.x < a.world) {
-    st_release_sys(a.flags[threadIdx.x] + FMB200_MAX_PEERS + a.rank, a.seq);
-    const unsigned int* mine = a.flags[a.rank] + FMB200_MAX_PEERS + threadIdx.x;
+    st_release_sys(a.flags[threadIdx.x] + COMM_BAR_WORD + a.rank, a.seq);
+    const unsigned int* mine = a.flags[a.rank] + COMM_BAR_WORD + threadIdx.x;
     while ((int)(ld_acquire_sys(mine) - a.seq) < 0) {
     }
   }
@@ -351,7 +352,7 @@ cudaError_t peer_preload_kernels() {
 
 cudaError_t launch_peer_barrier(fmb200_ctx* c) {
   PeerArgs a;
-  for (int q = 0; q < c->peer_world; q++) a.flags[q] = reinterpret_cast<unsigned int*>(c->peer_base[q]);
+  for (int q = 0; q < c->peer_world; q++) a.flags[q] = CommLayout::words(c->peer_base[q]);
   a.world = c->peer_world;
   a.rank = c->peer_rank;
   a.seq = ++c->peer_bar_seq;
@@ -365,25 +366,16 @@ static int peer_grid(const fmb200_ctx* c, uint64_t n_vec) {
 }
 
 // called in front of a HOGWILD epoch when peers are attached: theta0 and the shard's counts
-// Where rank-local things live behind the two state buffers of the comm block:
-//   theta0 (comm_buf_bytes) | counts, parity 0 | |V|^2 partials (2 x FMB_PEER_PART) | mean counts | counts, parity 1
-// The published counts (and the row count word in the header) are double-buffered by the parity of the exchange
-// that will read them: a slow peer may still be reading exchange e's table while this rank already prepares e+1.
-static float* peer_cnt_ptr(const fmb200_ctx* c, unsigned char* base, unsigned parity) {
-  float* cnt0 = reinterpret_cast<float*>(base + c->comm_hdr + 3 * c->comm_buf_bytes);
-  return parity ? cnt0 + 2 * c->comm_cnt_floats + 2 * (size_t)FMB_PEER_PART : cnt0;
-}
-
 cudaError_t peer_before_epoch(fmb200_ctx* c, const DataSlot& d) {
   if (c->peer_world <= 1) return cudaSuccess;
+  const CommLayout& L = c->comm;
+  unsigned char* self = c->comm_base.get();
   const uint64_t n_vec = (c->p32.n_floats + 3) / 4;
-  unsigned char* extra = c->comm_base + c->comm_hdr + 2 * c->comm_buf_bytes;
-  float4* base = reinterpret_cast<float4*>(extra);
-  float* part = reinterpret_cast<float*>(extra + c->comm_buf_bytes) + c->comm_cnt_floats;
   if (!c->peer_base_valid) {
     const int grid = peer_grid(c, n_vec);
-    fm_peer_capture_kernel<<<grid, 256, 0, c->stream>>>(reinterpret_cast<const float4*>(c->p32.base), base, n_vec,
-                                                        c->p32.off_v / 4, part + (size_t)c->peer_part_cur * FMB_PEER_PART);
+    fm_peer_capture_kernel<<<grid, 256, 0, c->stream>>>(reinterpret_cast<const float4*>(c->p32.base),
+                                                        reinterpret_cast<float4*>(L.theta0(self)), n_vec,
+                                                        c->p32.off_v / 4, L.partials(self, c->peer_part_cur));
     c->peer_n_part = grid;
     c->peer_base_valid = true;
     c->launches++;
@@ -393,35 +385,40 @@ cudaError_t peer_before_epoch(fmb200_ctx* c, const DataSlot& d) {
   const unsigned parity = (c->peer_seq + 1u) & 1u;
   if (c->n > 0 && d.feat_cnt != nullptr && c->peer_cnt_stamp[parity] != d.upload_gen) {
     const int grid = (int)std::max<uint32_t>(1, std::min<uint32_t>((c->n + 255) / 256, 64));
-    fm_peer_counts_kernel<<<grid, 256, 0, c->stream>>>(
-        d.feat_cnt, peer_cnt_ptr(c, c->comm_base, parity), c->n,
-        reinterpret_cast<unsigned int*>(c->comm_base) + 64 + 16 * parity + c->peer_rank, (unsigned int)d.n_rows);
+    fm_peer_counts_kernel<<<grid, 256, 0, c->stream>>>(d.feat_cnt.get(), L.counts(self, parity), c->n,
+                                                       L.rows_word(self, parity, c->peer_rank), (unsigned int)d.n_rows);
     c->launches++;
     c->peer_cnt_stamp[parity] = d.upload_gen;
   }
   return cudaGetLastError();
 }
 
+// the exchange reads every rank's state buffer `cur` and leaves the result in the buffers `cur ^ 1`
+static void peer_swap(fmb200_ctx* c) {
+  c->peer_cur ^= 1;
+  c->p32.base = c->comm.buf(c->comm_base.get(), c->peer_cur);
+}
+
 cudaError_t launch_peer_meanfield(fmb200_ctx* c) {
+  const CommLayout& L = c->comm;
+  unsigned char* self = c->comm_base.get();
   MeanFieldArgs a;
   const int cur = c->peer_cur;
-  const size_t extra = c->comm_hdr + 2 * c->comm_buf_bytes;
   for (int q = 0; q < c->peer_world; q++) {
-    a.p.flags[q] = reinterpret_cast<unsigned int*>(c->peer_base[q]);
-    a.p.cur[q] = reinterpret_cast<const float4*>(c->peer_base[q] + c->comm_hdr + (size_t)cur * c->comm_buf_bytes);
-    a.cnt[q] = peer_cnt_ptr(c, c->peer_base[q], (c->peer_seq + 1u) & 1u);
+    a.p.flags[q] = CommLayout::words(c->peer_base[q]);
+    a.p.cur[q] = reinterpret_cast<const float4*>(L.buf(c->peer_base[q], cur));
+    a.cnt[q] = L.counts(c->peer_base[q], (c->peer_seq + 1u) & 1u);
   }
-  a.p.next_local = reinterpret_cast<float4*>(c->comm_base + c->comm_hdr + (size_t)(cur ^ 1) * c->comm_buf_bytes);
+  a.p.next_local = reinterpret_cast<float4*>(L.buf(self, cur ^ 1));
   a.p.world = c->peer_world;
   a.p.rank = c->peer_rank;
   a.p.seq = ++c->peer_seq;
   a.p.n_vec = (c->p32.n_floats + 3) / 4;
   a.p.inv_world = 1.f / (float)c->peer_world;
-  a.base_local = reinterpret_cast<float4*>(c->comm_base + extra);
-  float* part = reinterpret_cast<float*>(c->comm_base + extra + c->comm_buf_bytes) + c->comm_cnt_floats;
-  a.cntm = part + 2 * (size_t)FMB_PEER_PART;
-  a.part_in = part + (size_t)c->peer_part_cur * FMB_PEER_PART;
-  a.part_out = part + (size_t)(c->peer_part_cur ^ 1) * FMB_PEER_PART;
+  a.base_local = reinterpret_cast<float4*>(L.theta0(self));
+  a.cntm = L.mean_counts(self);
+  a.part_in = L.partials(self, c->peer_part_cur);
+  a.part_out = L.partials(self, c->peer_part_cur ^ 1);
   a.n_part = c->peer_n_part;
   a.off_w = c->p32.off_w;
   a.off_v = c->p32.off_v;
@@ -444,10 +441,9 @@ cudaError_t launch_peer_meanfield(fmb200_ctx* c) {
   if (sliced) {
     MeanFieldPush t;
     for (int q = 0; q < c->peer_world; q++) {
-      t.next[q] = reinterpret_cast<float4*>(c->peer_base[q] + c->comm_hdr + (size_t)(cur ^ 1) * c->comm_buf_bytes);
-      t.base[q] = reinterpret_cast<float4*>(c->peer_base[q] + extra);
-      t.part[q] = reinterpret_cast<float*>(c->peer_base[q] + extra + c->comm_buf_bytes) + c->comm_cnt_floats +
-                  (size_t)(c->peer_part_cur ^ 1) * FMB_PEER_PART;
+      t.next[q] = reinterpret_cast<float4*>(L.buf(c->peer_base[q], cur ^ 1));
+      t.base[q] = reinterpret_cast<float4*>(L.theta0(c->peer_base[q]));
+      t.part[q] = L.partials(c->peer_base[q], c->peer_part_cur ^ 1);
     }
     const uint64_t per = (a.p.n_vec + c->peer_world - 1) / c->peer_world;
     const int grid = std::min(peer_grid(c, per), FMB_PEER_PART / c->peer_world);
@@ -463,29 +459,28 @@ cudaError_t launch_peer_meanfield(fmb200_ctx* c) {
     c->peer_n_part = grid;
   }
   c->peer_part_cur ^= 1;
-  c->peer_cur = cur ^ 1;
-  c->p32.base = reinterpret_cast<float*>(c->comm_base + c->comm_hdr + (size_t)c->peer_cur * c->comm_buf_bytes);
+  peer_swap(c);
   return cudaGetLastError();
 }
 
 cudaError_t launch_peer_mean(fmb200_ctx* c) {
+  const CommLayout& L = c->comm;
   PeerArgs a;
   const int cur = c->peer_cur;
   for (int q = 0; q < c->peer_world; q++) {
-    a.flags[q] = reinterpret_cast<unsigned int*>(c->peer_base[q]);
-    a.cur[q] = reinterpret_cast<const float4*>(c->peer_base[q] + c->comm_hdr + (size_t)cur * c->comm_buf_bytes);
+    a.flags[q] = CommLayout::words(c->peer_base[q]);
+    a.cur[q] = reinterpret_cast<const float4*>(L.buf(c->peer_base[q], cur));
   }
-  a.next_local = reinterpret_cast<float4*>(c->comm_base + c->comm_hdr + (size_t)(cur ^ 1) * c->comm_buf_bytes);
+  a.next_local = reinterpret_cast<float4*>(L.buf(c->comm_base.get(), cur ^ 1));
   a.world = c->peer_world;
   a.rank = c->peer_rank;
   a.seq = ++c->peer_seq;
   a.n_vec = (c->p32.n_floats + 3) / 4;
   a.inv_world = 1.f / (float)c->peer_world;
-  const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((a.n_vec + 255) / 256, (uint64_t)c->sm_count * 2));
+  const int grid = peer_grid(c, a.n_vec);
   fm_peer_mean_kernel<<<grid, 256, 0, c->stream>>>(a);
   c->launches++;
-  c->peer_cur = cur ^ 1;
-  c->p32.base = reinterpret_cast<float*>(c->comm_base + c->comm_hdr + (size_t)c->peer_cur * c->comm_buf_bytes);
+  peer_swap(c);
   c->peer_base_valid = false;  // theta0 of the mean-field combine no longer matches
   return cudaGetLastError();
 }

@@ -141,10 +141,10 @@ cudaError_t launch_predict32(fmb200_ctx* c, const DataSlot& d, int transform, do
     default: fn = pick_predict_s<32>(S, cls); break;
   }
   PredictArgs a;
-  a.row_ptr = d.row_ptr;
-  a.col = d.col;
-  a.val = d.val;
-  a.target = d.target;
+  a.row_ptr = d.row_ptr.get();
+  a.col = d.col.get();
+  a.val = d.val.get();
+  a.target = d.target.get();
   a.n_rows = d.n_rows;
   a.w0 = c->p32.w0();
   a.w = c->p32.w();
@@ -286,11 +286,6 @@ __global__ void csr_inspect_kernel(const uint64_t* __restrict__ rp, uint64_t n_r
   }
 }
 
-static int grid_for(fmb200_ctx* c, uint64_t work) {
-  uint64_t blocks = (work + 255) / 256;
-  return (int)std::max<uint64_t>(1, std::min<uint64_t>(blocks, (uint64_t)c->sm_count * 8));
-}
-
 cudaError_t launch_p64_to_p32(fmb200_ctx* c) {
   p64_to_p32_kernel<<<grid_for(c, (uint64_t)c->n * (c->kp + 1)), 256, 0, c->stream>>>(c->p64, c->p32,
                                                                                c->n, c->k, c->kp);
@@ -312,30 +307,30 @@ cudaError_t launch_scale_p32(fmb200_ctx* c, float factor) {
   return cudaGetLastError();
 }
 
-cudaError_t launch_csr_inspect(fmb200_ctx* c, const uint64_t* rp, uint64_t n_rows, uint64_t nnz,
+cudaError_t launch_csr_inspect(fmb200_ctx* c, cudaStream_t st, const uint64_t* rp, uint64_t n_rows, uint64_t nnz,
                                unsigned int* out8) {
-  csr_inspect_kernel<<<grid_for(c, n_rows ? n_rows : 1), 256, 0, c->stream>>>(rp, n_rows, nnz, out8);
+  csr_inspect_kernel<<<grid_for(c, n_rows ? n_rows : 1), 256, 0, st>>>(rp, n_rows, nnz, out8);
   c->launches++;
   return cudaGetLastError();
 }
 
-cudaError_t launch_feature_counts(fmb200_ctx* c, const uint32_t* col, uint64_t nnz, float* cnt,
+cudaError_t launch_feature_counts(fmb200_ctx* c, cudaStream_t st, const uint32_t* col, uint64_t nnz, float* cnt,
                                   unsigned int* out_max_id, unsigned int* out_max) {
   unsigned int* u = reinterpret_cast<unsigned int*>(cnt);
-  cudaError_t e = cudaMemsetAsync(u, 0, sizeof(unsigned int) * (size_t)c->n, c->stream);
+  cudaError_t e = cudaMemsetAsync(u, 0, sizeof(unsigned int) * (size_t)c->n, st);
   if (e != cudaSuccess) return e;
   if (nnz > 0) {
     constexpr int BINS = 12288;  // 48 KB of static shared memory
     if (c->n <= (uint32_t)BINS) {
       const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((nnz + 16383) / 16384, (uint64_t)c->sm_count));
-      hist_kernel<BINS><<<grid, 1024, 0, c->stream>>>(col, nnz, c->n, u, out_max_id);
+      hist_kernel<BINS><<<grid, 1024, 0, st>>>(col, nnz, c->n, u, out_max_id);
     } else {
-      hist_kernel<0><<<grid_for(c, nnz), 256, 0, c->stream>>>(col, nnz, c->n, u, out_max_id);
+      hist_kernel<0><<<grid_for(c, nnz), 256, 0, st>>>(col, nnz, c->n, u, out_max_id);
     }
     c->launches++;
   }
   if (c->n > 0) {
-    cnt_to_float_kernel<<<grid_for(c, c->n), 256, 0, c->stream>>>(u, c->n, out_max);
+    cnt_to_float_kernel<<<grid_for(c, c->n), 256, 0, st>>>(u, c->n, out_max);
     c->launches++;
   }
   return cudaGetLastError();

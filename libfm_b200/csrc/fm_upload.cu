@@ -142,39 +142,33 @@ __global__ void onehot_fill_kernel(uint64_t n_rows, uint32_t z, uint64_t* __rest
   }
 }
 
-int grid_for(const fmb200_ctx* c, uint64_t work) {
-  const uint64_t blocks = (work + 255) / 256;
-  const uint64_t cap = (uint64_t)c->sm_count * 8;
-  return (int)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap));
-}
-
 }  // namespace
 
 // d_rows: device copy of the sparse_row array; scratch: aos_scan_tiles(n_rows)+1 u64.
 // Writes row_ptr[0..n_rows]; flag[0] bit 0 = rows are not one contiguous block.
 // (d_entries / nnz / col / val: when given, the split runs in the same call.)
-cudaError_t launch_aos_to_csr(fmb200_ctx* c, const void* d_rows, const void* d_entries, uint64_t n_rows,
+cudaError_t launch_aos_to_csr(fmb200_ctx* c, cudaStream_t st, const void* d_rows, const void* d_entries, uint64_t n_rows,
                               uint64_t nnz, unsigned long long host_base_ptr, unsigned long long* scratch,
                               uint64_t* row_ptr, uint32_t* col, float* val, unsigned int* flag) {
   const uint64_t n_tiles = (n_rows + SCAN_TILE - 1) / SCAN_TILE;
   const AosRow* rows = static_cast<const AosRow*>(d_rows);
   if (n_tiles > 0) {
-    aos_tile_sums_kernel<<<(unsigned)n_tiles, SCAN_THREADS, 0, c->stream>>>(rows, n_rows, scratch);
-    scan_tile_sums_kernel<<<1, SCAN_THREADS, 0, c->stream>>>(scratch, n_tiles);
-    aos_row_ptr_kernel<<<(unsigned)n_tiles, SCAN_THREADS, 0, c->stream>>>(rows, n_rows, scratch, host_base_ptr,
+    aos_tile_sums_kernel<<<(unsigned)n_tiles, SCAN_THREADS, 0, st>>>(rows, n_rows, scratch);
+    scan_tile_sums_kernel<<<1, SCAN_THREADS, 0, st>>>(scratch, n_tiles);
+    aos_row_ptr_kernel<<<(unsigned)n_tiles, SCAN_THREADS, 0, st>>>(rows, n_rows, scratch, host_base_ptr,
                                                                          row_ptr, flag);
     c->launches += 3;
   } else {
-    aos_row_ptr_kernel<<<1, SCAN_THREADS, 0, c->stream>>>(rows, 0, scratch, host_base_ptr, row_ptr, flag);
+    aos_row_ptr_kernel<<<1, SCAN_THREADS, 0, st>>>(rows, 0, scratch, host_base_ptr, row_ptr, flag);
     c->launches++;
   }
-  if (nnz > 0 && d_entries != nullptr) return launch_aos_split(c, d_entries, nnz, col, val);
+  if (nnz > 0 && d_entries != nullptr) return launch_aos_split(c, st, d_entries, nnz, col, val);
   return cudaGetLastError();
 }
 
-cudaError_t launch_aos_split(fmb200_ctx* c, const void* d_entries, uint64_t nnz, uint32_t* col, float* val) {
+cudaError_t launch_aos_split(fmb200_ctx* c, cudaStream_t st, const void* d_entries, uint64_t nnz, uint32_t* col, float* val) {
   if (nnz > 0) {
-    aos_split_kernel<<<grid_for(c, nnz), 256, 0, c->stream>>>(static_cast<const uint2*>(d_entries), nnz, col, val);
+    aos_split_kernel<<<grid_for(c, nnz), 256, 0, st>>>(static_cast<const uint2*>(d_entries), nnz, col, val);
     c->launches++;
   }
   return cudaGetLastError();
@@ -182,8 +176,8 @@ cudaError_t launch_aos_split(fmb200_ctx* c, const void* d_entries, uint64_t nnz,
 
 uint64_t aos_scan_tiles(uint64_t n_rows) { return (n_rows + SCAN_TILE - 1) / SCAN_TILE; }
 
-cudaError_t launch_onehot_fill(fmb200_ctx* c, uint64_t n_rows, uint32_t z, uint64_t* row_ptr, float* val) {
-  onehot_fill_kernel<<<grid_for(c, n_rows * z + n_rows + 1), 256, 0, c->stream>>>(n_rows, z, row_ptr, val);
+cudaError_t launch_onehot_fill(fmb200_ctx* c, cudaStream_t st, uint64_t n_rows, uint32_t z, uint64_t* row_ptr, float* val) {
+  onehot_fill_kernel<<<grid_for(c, n_rows * z + n_rows + 1), 256, 0, st>>>(n_rows, z, row_ptr, val);
   c->launches++;
   return cudaGetLastError();
 }

@@ -4,11 +4,72 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <memory>
 #include <string>
+#include <type_traits>
 
 #include "../../include/fmb200.h"
 
 namespace fmb {
+
+// Owning handles: every device buffer, pinned host buffer and event of a context is released by
+// its owner's destructor.  Kernel argument structs keep raw pointers (they are copied to the device).
+struct CudaFree {
+  void operator()(void* p) const { cudaFree(p); }
+};
+struct CudaFreeHost {
+  void operator()(void* p) const { cudaFreeHost(p); }
+};
+struct CudaEventDestroy {
+  void operator()(cudaEvent_t e) const { cudaEventDestroy(e); }
+};
+template <class T>
+using DevPtr = std::unique_ptr<T, CudaFree>;
+template <class T>
+using HostPtr = std::unique_ptr<T, CudaFreeHost>;
+using EventPtr = std::unique_ptr<std::remove_pointer_t<cudaEvent_t>, CudaEventDestroy>;
+
+// p := a fresh device buffer of n elements (at least one); what p held is released first
+template <class T>
+cudaError_t alloc(DevPtr<T>& p, uint64_t n) {
+  p.reset();
+  T* raw = nullptr;
+  const cudaError_t e = cudaMalloc(&raw, (n ? n : 1) * sizeof(T));
+  p.reset(raw);
+  return e;
+}
+
+// p := a fresh pinned host buffer of n elements
+template <class T>
+cudaError_t host_alloc(HostPtr<T>& p, size_t n) {
+  p.reset();
+  T* raw = nullptr;
+  const cudaError_t e = cudaHostAlloc((void**)&raw, n * sizeof(T), cudaHostAllocDefault);
+  p.reset(raw);
+  return e;
+}
+
+inline cudaError_t event_create(EventPtr& p, unsigned int flags) {
+  cudaEvent_t raw = nullptr;
+  const cudaError_t e = cudaEventCreateWithFlags(&raw, flags);
+  p.reset(raw);
+  return e;
+}
+
+// Grow-on-demand scratch: make p hold at least n elements, cap = what it holds.  Contents are not kept.
+template <class T, class Cap>
+cudaError_t grow(DevPtr<T>& p, Cap& cap, uint64_t n) {
+  if (p && cap >= n) return cudaSuccess;
+  cap = 0;
+  const cudaError_t e = alloc(p, n);
+  if (e == cudaSuccess) cap = (Cap)n;
+  return e;
+}
+
+// slack (in elements) behind every per-row and per-entry array of a slot (the CSR arrays and the
+// ORDERED index) so that whole-tile TMA bulk copies of the last tile stay inside the allocation
+constexpr uint64_t kRowSlack = 512 + 8;
+constexpr uint64_t kEntrySlack = 16;
 
 // One uploaded data set, SoA CSR in HBM.  Arrays are over-allocated so that
 // 16-byte-granular TMA bulk copies may read past the logical end.
@@ -16,16 +77,16 @@ struct DataSlot {
   bool present = false;
   uint64_t n_rows = 0;
   uint64_t nnz = 0;
-  uint64_t* row_ptr = nullptr;  // [n_rows + 1] (+ padding)
-  uint32_t* col = nullptr;      // [nnz] (+ padding)
-  float* val = nullptr;         // [nnz] (+ padding)
-  float* target = nullptr;      // [n_rows] (+ padding)
+  DevPtr<uint64_t> row_ptr;  // [cap_rows + 1 + kRowSlack]
+  DevPtr<uint32_t> col;      // [cap_nnz + kEntrySlack]
+  DevPtr<float> val;         // [cap_nnz + kEntrySlack]
+  DevPtr<float> target;      // [cap_rows + kRowSlack]
   uint32_t max_row_nnz = 0;
   uint64_t cap_rows = 0, cap_nnz = 0;  // allocated capacity (re-uploads reuse the buffers)
-  float* feat_cnt = nullptr;    // [n_attr] occurrences of each feature in this data set
-  unsigned int* d_flag = nullptr;  // 16 words: inspection results of the last upload
-  unsigned int* h_flag = nullptr;  // pinned mirror
-  cudaEvent_t ready = nullptr;     // recorded behind the upload's last operation
+  DevPtr<float> feat_cnt;    // [n_attr] occurrences of each feature in this data set
+  DevPtr<unsigned int> d_flag;   // 16 words: inspection results of the last upload
+  HostPtr<unsigned int> h_flag;  // pinned mirror
+  EventPtr ready;                // recorded behind the upload's last operation
   bool pending = false;            // an upload is enqueued and not yet collected
   uint64_t upload_gen = 0;         // unique per upload of a context (fmb200_ctx::upload_counter)
   uint32_t max_feat_cnt = 0;
@@ -34,12 +95,51 @@ struct DataSlot {
   uint32_t tile_span[5] = {0, 0, 0, 0, 0};
   // ORDERED mode (fm_ordered.cu): per-entry distance to the previous entry of the same
   // feature, per-row distance to the nearest earlier row sharing a feature; built lazily
-  uint32_t* link = nullptr;
-  uint32_t* rowdep = nullptr;
+  DevPtr<uint32_t> link;
+  DevPtr<uint32_t> rowdep;
+  uint64_t link_cap = 0, rowdep_cap = 0;
   uint32_t* ord_shape = nullptr;  // behind rowdep: bit 0 = all values 1, bit 1 = all rows max_row_nnz long
   bool links_ready = false;
-  void* ord_scratch = nullptr;  // scratch of the index build (kept for re-uploads of moderate size)
+  DevPtr<unsigned char> ord_scratch;  // scratch of the index build (kept for re-uploads of moderate size)
   size_t ord_scratch_bytes = 0;
+};
+
+// Layout of the peer comm block (fm_peer.cu), one per context, mapped by its peers:
+//   header | state buffer 0 | state buffer 1 | theta0 | counts, parity 0 | |V|^2 partials x 2 |
+//   mean counts | counts, parity 1
+// The published counts and row-count words are double-buffered by the parity of the exchange that
+// will read them: a slow peer may still be reading exchange e's table while this rank prepares e+1.
+// Header words (u32):
+constexpr int COMM_SEQ_WORD = 0;                 // [rank]: sequence number of the averaging kernels
+constexpr int COMM_BAR_WORD = FMB200_MAX_PEERS;  // [rank]: sequence number of the barrier kernel
+constexpr int COMM_ROWS_WORD = 64;               // [COMM_ROWS_PARITY_STRIDE parity + rank]: rows of a shard
+constexpr int COMM_ROWS_PARITY_STRIDE = 16;
+constexpr int COMM_MEAN_ROWS_WORD = 100;         // [parity]: mean rows per shard, as a float
+
+// per-block |V|^2 partials of the mean-field exchange: two tables of this many floats in the comm block
+// (the sliced exchange needs world x grid entries)
+constexpr int FMB_PEER_PART = 4096;
+
+struct CommLayout {
+  static constexpr size_t hdr_bytes = 1024;
+  size_t buf_bytes = 0;   // one state buffer (the packed fp32 state, rounded up to 256 bytes)
+  size_t cnt_floats = 0;  // one count table (n_attr, rounded up to 64)
+  CommLayout() = default;
+  CommLayout(uint64_t n_floats, uint32_t n_attr)
+      : buf_bytes((n_floats * sizeof(float) + 255) & ~(size_t)255), cnt_floats(((size_t)n_attr + 63) & ~(size_t)63) {}
+  size_t total_bytes() const { return hdr_bytes + 3 * buf_bytes + (3 * cnt_floats + 2 * (size_t)FMB_PEER_PART) * sizeof(float); }
+  static unsigned int* words(unsigned char* b) { return reinterpret_cast<unsigned int*>(b); }
+  unsigned int* rows_word(unsigned char* b, unsigned parity, int rank) const {
+    return words(b) + COMM_ROWS_WORD + COMM_ROWS_PARITY_STRIDE * parity + rank;
+  }
+  float* buf(unsigned char* b, int i) const { return reinterpret_cast<float*>(b + hdr_bytes + (size_t)i * buf_bytes); }
+  float* theta0(unsigned char* b) const { return buf(b, 2); }
+  float* counts(unsigned char* b, unsigned parity) const {
+    float* cnt0 = buf(b, 3);
+    return parity ? cnt0 + 2 * cnt_floats + 2 * (size_t)FMB_PEER_PART : cnt0;
+  }
+  float* partials(unsigned char* b, int j) const { return counts(b, 0) + cnt_floats + (size_t)j * FMB_PEER_PART; }
+  float* mean_counts(unsigned char* b) const { return partials(b, 2); }
 };
 
 // Packed fp32 state: [w0, 0, 0, 0 | w[n*ws] padded to a multiple of 4 | V[n][kp]].
@@ -74,11 +174,10 @@ struct HParams {
   double min_target = 0, max_target = 0;
 };
 
-// per-block |V|^2 partials of the mean-field exchange: two tables of this many floats in the comm block
-// (the sliced exchange needs world x grid entries)
-constexpr int FMB_PEER_PART = 4096;
-
 struct McmcState;  // fm_mcmc.cu
+struct McmcDelete {
+  void operator()(McmcState* s) const;
+};
 
 struct EpochConfig {
   int lanes_per_row = 0, slots = 0, rows_per_tile = 0, grid = 0, block = 0, smem = 0, damp = 0;
@@ -92,34 +191,32 @@ struct fmb200_ctx {
   int max_smem_optin = 0;
   cudaStream_t stream = nullptr;
   cudaStream_t copy_stream = nullptr;  // asynchronous uploads (fmb200_upload_data_async)
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  fmb::EventPtr ev0, ev1;
   uint32_t n = 0;
   int k = 0, kp = 0;
   bool k0 = true, k1 = true;
   int mode = FMB200_MODE_HOGWILD;
   fmb::HParams hp;
-  fmb::Params32 p32;
-  fmb::Params64 p64;
+  fmb::Params32 p32;  // base points into the comm block
+  fmb::Params64 p64;  // base = p64_buf
+  fmb::DevPtr<double> p64_buf;
   fmb::DataSlot slots[FMB200_MAX_SLOTS];
   // scratch
-  double* d_partials = nullptr;  // evaluate: per-block partial sums
-  int n_partials = 0;
-  double* d_pred = nullptr;  // predict output staging
+  fmb::DevPtr<double> d_partials;  // evaluate: per-block partial sums (3 per block)
+  uint64_t n_partials = 0;
+  fmb::DevPtr<double> d_pred;  // predict output staging
   uint64_t pred_cap = 0;
-  unsigned int* d_sched = nullptr;   // hogwild tile scheduler: [next tile, CTAs run dry]
-  unsigned long long* d_acc = nullptr;  // fixed-point steps of one row-lane launch, beside p32 (zero between launches)
-  unsigned int* d_flag = nullptr;    // 16 device words: upload-time inspection results
-  unsigned int* h_flag = nullptr;    // pinned host mirror of d_flag
-  void* h_stage = nullptr;           // pinned staging for set/get_params (small models)
-  size_t h_stage_bytes = 0;
+  fmb::DevPtr<unsigned int> d_sched;   // hogwild tile scheduler: [next tile, CTAs run dry]
+  fmb::DevPtr<unsigned long long> d_acc;  // fixed-point accumulator of the row-lane epoch (fm_hogwild.cu)
+  fmb::DevPtr<unsigned int> d_flag;    // 16 device words: upload-time inspection results
+  fmb::HostPtr<unsigned int> h_flag;   // pinned host mirror of d_flag
+  fmb::HostPtr<unsigned char> h_stage;  // pinned staging for set/get_params (small models)
   uint64_t launches = 0;
   fmb::EpochConfig last_cfg;
   int tune_ctas_per_sm = 0, tune_rows_per_tile = 0, tune_threads = 0;
-  // peer-memory parameter averaging (fm_peer.cu).  comm block = [flags | buf0 | buf1]
-  unsigned char* comm_base = nullptr;
-  size_t comm_hdr = 1024, comm_buf_bytes = 0;
-  // behind the two state buffers: theta0 (comm_buf_bytes) | counts (comm_cnt_floats) | |V|^2 partials (2 x FMB_PEER_PART) | mean counts | counts of the other parity
-  size_t comm_cnt_floats = 0;
+  // peer-memory parameter averaging (fm_peer.cu)
+  fmb::DevPtr<unsigned char> comm_base;
+  fmb::CommLayout comm;
   bool peer_base_valid = false;  // theta0 holds the state the running epoch started from
   bool hogwild_fresh = true;     // no HOGWILD epoch has run since the state was last set (bias ramp)
   int peer_part_cur = 0, peer_n_part = 0;
@@ -131,15 +228,21 @@ struct fmb200_ctx {
   uint64_t peer_cnt_stamp[2] = {0, 0};  // upload generation held by the table of each parity (0 = none)
   uint64_t upload_counter = 0;          // generations handed out to uploads
   // SGDA state (fm_learn_sgd_element_adapt_reg.h): stored gradients, per-group regularisation
-  double *sgda_grad_w = nullptr, *sgda_grad_v = nullptr, *sgda_reg_w = nullptr, *sgda_reg_v = nullptr;
-  uint32_t* sgda_group = nullptr;
+  fmb::DevPtr<double> sgda_grad_w, sgda_grad_v, sgda_reg_w, sgda_reg_v;
+  fmb::DevPtr<uint32_t> sgda_group;
   uint32_t sgda_groups = 0;
   int tune_damp = 0;  // 0 auto, 1 force on, -1 force off
   int tune_variant = 0;  // 0 auto, 1 row-group kernel, 2 row-lane kernel when eligible
-  fmb::McmcState* mcmc = nullptr;  // MCMC / ALS learner state (fm_mcmc.cu)
+  std::unique_ptr<fmb::McmcState, fmb::McmcDelete> mcmc;  // MCMC / ALS learner state (fm_mcmc.cu)
 };
 
 namespace fmb {
+
+// launch size of the grid-stride helper kernels: blocks of 256 threads, at least 1, at most 8 per SM
+inline int grid_for(const fmb200_ctx* c, uint64_t work) {
+  const uint64_t blocks = (work + 255) / 256, cap = (uint64_t)c->sm_count * 8;
+  return (int)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap));
+}
 
 // fm_inorder.cu: sequential-equivalent fp64 epoch (one warp, rows in order)
 cudaError_t launch_sgd_inorder(fmb200_ctx* c, const DataSlot& d);
@@ -150,8 +253,15 @@ cudaError_t launch_predict64(fmb200_ctx* c, const DataSlot& d, int transform, do
 // fm_ordered.cu: sequentially consistent fp64 epoch (runs of independent rows in parallel, bias by
 // affine scan).  *handled = false: shape not eligible, nothing launched (caller uses launch_sgd_inorder)
 cudaError_t launch_sgd_ordered(fmb200_ctx* c, DataSlot& d, bool* handled);
-// keep_scratch: keep the (id, entry) sort in d.ord_scratch whatever the data set's size
-cudaError_t build_ordered_links(fmb200_ctx* c, DataSlot& d, bool keep_scratch = false);
+// The training entries stably sorted by feature id (each feature's occurrences in file order):
+// ids[i] = the id, ent[i] = the entry's position in col[] / val[]
+struct SortedEntries {
+  const uint32_t* ids = nullptr;
+  const uint32_t* ent = nullptr;
+};
+// Build link[] / rowdep[] of a data set on c->stream (no host sync).  sorted != null: also keep the
+// (id, entry) sort behind the index whatever the data set's size, and return a view of it.
+cudaError_t build_ordered_links(fmb200_ctx* c, DataSlot& d, SortedEntries* sorted = nullptr);
 // fm_inorder.cu: the MCMC / ALS e-term pass (fm_learn_mcmc.h:148-378), bit-identical accumulation
 cudaError_t launch_mcmc_eterms(fmb200_ctx* c, const DataSlot& d, double* e_out);
 // fm_mcmc.cu: MCMC / ALS learning (fm_learn_mcmc_simultaneous); "" on success, else the error
@@ -161,11 +271,12 @@ std::string mcmc_begin(fmb200_ctx* c, int train, int test, int do_sample, int do
 std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counters);
 bool mcmc_get(const fmb200_ctx* c, double* alpha, double* w_mu, double* w_lambda, double* v_mu, double* v_lambda,
               double* pred_this, double* pred_sum_all, double* pred_sum_all_but5, uint32_t* n_runs);
-void mcmc_free(fmb200_ctx* c);
 // fm_inorder.cu: one SGDA epoch (theta-step per training row, lambda-step per validation row)
 cudaError_t launch_sgda_epoch(fmb200_ctx* c, const DataSlot& tr, const DataSlot& va, int lambda_steps);
 // fm_hogwild.cu: throughput epoch
 cudaError_t launch_sgd_hogwild(fmb200_ctx* c, const DataSlot& d);
+// fm_hogwild.cu: a fresh state clears the divergence flag of the row-lane epoch's accumulator
+cudaError_t clear_acc_flag(fmb200_ctx* c);
 // fm_predict.cu: fp32 scores / metrics with sub-warp row groups
 cudaError_t launch_predict32(fmb200_ctx* c, const DataSlot& d, int transform, double* out_pred,
                              double* partials, int n_blocks);
@@ -181,19 +292,19 @@ cudaError_t peer_preload_kernels();  // defeat lazy loading before any exchange 
 cudaError_t launch_peer_meanfield(fmb200_ctx* c);
 cudaError_t peer_before_epoch(fmb200_ctx* c, const DataSlot& d);
 // device-side structural check of row offsets (see fm_predict.cu)
-cudaError_t launch_csr_inspect(fmb200_ctx* c, const uint64_t* rp, uint64_t n_rows, uint64_t nnz,
+cudaError_t launch_csr_inspect(fmb200_ctx* c, cudaStream_t st, const uint64_t* rp, uint64_t n_rows, uint64_t nnz,
                                unsigned int* out8);
 // histogram of column ids -> float counts in cnt[n]; *out_max = largest count
-cudaError_t launch_feature_counts(fmb200_ctx* c, const uint32_t* col, uint64_t nnz, float* cnt,
+cudaError_t launch_feature_counts(fmb200_ctx* c, cudaStream_t st, const uint32_t* col, uint64_t nnz, float* cnt,
                                   unsigned int* out_max_id, unsigned int* out_max);
 
 // fm_upload.cu: the reference's AoS containers -> SoA CSR on the device; one-hot materialisation
-cudaError_t launch_aos_to_csr(fmb200_ctx* c, const void* d_rows, const void* d_entries, uint64_t n_rows,
+cudaError_t launch_aos_to_csr(fmb200_ctx* c, cudaStream_t st, const void* d_rows, const void* d_entries, uint64_t n_rows,
                               uint64_t nnz, unsigned long long host_base_ptr, unsigned long long* scratch,
                               uint64_t* row_ptr, uint32_t* col, float* val, unsigned int* flag);
-cudaError_t launch_aos_split(fmb200_ctx* c, const void* d_entries, uint64_t nnz, uint32_t* col, float* val);
+cudaError_t launch_aos_split(fmb200_ctx* c, cudaStream_t st, const void* d_entries, uint64_t nnz, uint32_t* col, float* val);
 uint64_t aos_scan_tiles(uint64_t n_rows);
-cudaError_t launch_onehot_fill(fmb200_ctx* c, uint64_t n_rows, uint32_t z, uint64_t* row_ptr, float* val);
+cudaError_t launch_onehot_fill(fmb200_ctx* c, cudaStream_t st, uint64_t n_rows, uint32_t z, uint64_t* row_ptr, float* val);
 
 // pick the sub-warp geometry for a data set: G lanes per V row (power of two
 // covering kp/4 float4 chunks), S entry slots per row group, and the row-group
