@@ -63,28 +63,23 @@ __global__ void ord_shape_kernel(const float* __restrict__ val, uint64_t nnz, co
   if (clear) atomicAnd(shape, ~clear);
 }
 
-// blockDim <= ORD_SMAX * GL (one group of GL lanes per example of a run): small k leaves the
-// register file to few threads (k <= 8: 128 threads)
-template <int GL, int KF, int TASK, int ZF = 0>
-__global__ void __launch_bounds__((ORD_SMAX * GL < 256 ? 256 : (ORD_SMAX * GL < ORD_MAX_THREADS ? ORD_SMAX * GL : ORD_MAX_THREADS)), 1)
-    fm_sgd_ordered_kernel(const OrderedArgs a) {
-  extern __shared__ __align__(128) unsigned char ord_smem[];
-  ordered_epoch_body<GL, KF, TASK, ZF>(a, ord_smem);
-}
-
-// warp-specialised form: ORD_SMAX * GL compute threads, ORD_PARKED threads that leave after the set-up and
-// ORD_HELPERS helper threads (write-back, fetch).  ONE helper warp: every further helper warp slowed the epoch
-// by ~5% although the helpers idle most of the time -- their bursts of shared-memory / LSU traffic delay the
-// compute warps' loads (r02 calls M, N, the same build on one box, C2-shaped 200 000 rows: 1 / 2 / 3 / 4 helper
-// warps = 6.30 / 6.64-6.74 / 6.92 / 7.33 ms; which schedulers the helpers sit on matters little).  The parked
-// threads keep the helper warp's index a multiple of 4 apart from compute warp 3.
+// One CTA, one group of GL lanes per example of a run: ORD_SMAX * GL compute threads (at most 1 024; small k
+// leaves the register file to few threads, k <= 8: 128).  HELPERS (k <= 32 only, where they fit): then
+// ORD_PARKED threads that leave after the set-up and ORD_HELPERS helper threads (write-back, fetch); without
+// them the compute threads do that work themselves (ordered_epoch).  ONE helper warp: every further helper
+// warp slowed the epoch by ~5% although the helpers idle most of the time -- their bursts of shared-memory / LSU
+// traffic delay the compute warps' loads (r02 calls M, N, the same build on one box, C2-shaped 200 000 rows:
+// 1 / 2 / 3 / 4 helper warps = 6.30 / 6.64-6.74 / 6.92 / 7.33 ms; which schedulers the helpers sit on matters
+// little).  The parked threads keep the helper warp's index a multiple of 4 apart from compute warp 3.
 constexpr int ORD_PARKED = 96;
 constexpr int ORD_HELPERS = 32;
-template <int GL, int KF, int TASK, int ZF = 0>
-__global__ void __launch_bounds__(ORD_SMAX * GL + ORD_PARKED + ORD_HELPERS, 1)
-    fm_sgd_ordered_ws_kernel(const OrderedArgs a) {
+template <int GL, int KF, int TASK, int ZF, bool HELPERS>
+__global__ void __launch_bounds__(HELPERS ? ORD_SMAX * GL + ORD_PARKED + ORD_HELPERS
+                                          : (ORD_SMAX * GL < 256 ? 256 : (ORD_SMAX * GL < ORD_MAX_THREADS ? ORD_SMAX * GL : ORD_MAX_THREADS)), 1)
+    fm_sgd_ordered_kernel(const OrderedArgs a) {
   extern __shared__ __align__(128) unsigned char ord_smem[];
-  ordered_epoch_body_ws<GL, KF, TASK, ZF>(a, ord_smem, ORD_SMAX * GL, ORD_PARKED);
+  if constexpr (HELPERS) ordered_epoch_body_ws<GL, KF, TASK, ZF>(a, ord_smem, ORD_SMAX * GL, ORD_PARKED);
+  else ordered_epoch_body<GL, KF, TASK, ZF>(a, ord_smem);
 }
 
 using OrdFn = void (*)(const OrderedArgs);
@@ -102,53 +97,25 @@ inline void ordered_shape(int k, int* GL, int* KF) {
   *GL = g;
 }
 
-// register-resident fast path: k in {2,4,8} exactly, rows of at most 2 / 4 entries
-template <int TASK>
-OrdFn pick_fast_kernel(int k, uint32_t max_row_nnz) {
-  if (max_row_nnz < 1 || max_row_nnz > 4) return nullptr;
-  const bool z2 = max_row_nnz <= 2;
-  if (k == 2) return z2 ? fm_sgd_ordered_kernel<1, 2, TASK, 2> : fm_sgd_ordered_kernel<1, 2, TASK, 4>;
-  if (k == 4) return z2 ? fm_sgd_ordered_kernel<1, 4, TASK, 2> : fm_sgd_ordered_kernel<1, 4, TASK, 4>;
-  if (k == 8) return z2 ? fm_sgd_ordered_kernel<1, 8, TASK, 2> : fm_sgd_ordered_kernel<1, 8, TASK, 4>;
-  return nullptr;
-}
-
-// warp-specialised kernels: k <= 32 (GL <= 4: 128 GL compute threads + 128 helpers fit one CTA)
-template <int TASK>
-OrdFn pick_ws_kernel(int k, uint32_t max_row_nnz, int* ncompute) {
-  *ncompute = ORD_SMAX;
-  if (max_row_nnz >= 1 && max_row_nnz <= 4 && (k == 2 || k == 4 || k == 8)) {
+// the register-resident fast path where `fast` allows it (k in {2,4,8} exactly, rows of at most 2 / 4
+// entries), else the general kernel of ordered_shape's (GL, KF); with helpers where H asks for them (k <= 32)
+template <int TASK, bool H>
+OrdFn pick_kernel(int k, uint32_t max_row_nnz, bool fast) {
+  if (fast && max_row_nnz >= 1 && max_row_nnz <= 4) {
     const bool z2 = max_row_nnz <= 2;
-    if (k == 2) return z2 ? fm_sgd_ordered_ws_kernel<1, 2, TASK, 2> : fm_sgd_ordered_ws_kernel<1, 2, TASK, 4>;
-    if (k == 4) return z2 ? fm_sgd_ordered_ws_kernel<1, 4, TASK, 2> : fm_sgd_ordered_ws_kernel<1, 4, TASK, 4>;
-    return z2 ? fm_sgd_ordered_ws_kernel<1, 8, TASK, 2> : fm_sgd_ordered_ws_kernel<1, 8, TASK, 4>;
+    if (k == 2) return z2 ? fm_sgd_ordered_kernel<1, 2, TASK, 2, H> : fm_sgd_ordered_kernel<1, 2, TASK, 4, H>;
+    if (k == 4) return z2 ? fm_sgd_ordered_kernel<1, 4, TASK, 2, H> : fm_sgd_ordered_kernel<1, 4, TASK, 4, H>;
+    if (k == 8) return z2 ? fm_sgd_ordered_kernel<1, 8, TASK, 2, H> : fm_sgd_ordered_kernel<1, 8, TASK, 4, H>;
   }
-  if (k <= 1) return fm_sgd_ordered_ws_kernel<1, 1, TASK>;
-  if (k <= 2) return fm_sgd_ordered_ws_kernel<1, 2, TASK>;
-  if (k <= 4) return fm_sgd_ordered_ws_kernel<1, 4, TASK>;
-  if (k <= 8) return fm_sgd_ordered_ws_kernel<1, 8, TASK>;
-  if (k <= 16) {
-    *ncompute = 2 * ORD_SMAX;
-    return fm_sgd_ordered_ws_kernel<2, 8, TASK>;
-  }
-  if (k <= 32) {
-    *ncompute = 4 * ORD_SMAX;
-    return fm_sgd_ordered_ws_kernel<4, 8, TASK>;
-  }
-  return nullptr;
-}
-
-template <int TASK>
-OrdFn pick_kernel(int k) {
-  if (k <= 1) return fm_sgd_ordered_kernel<1, 1, TASK>;
-  if (k <= 2) return fm_sgd_ordered_kernel<1, 2, TASK>;
-  if (k <= 4) return fm_sgd_ordered_kernel<1, 4, TASK>;
-  if (k <= 8) return fm_sgd_ordered_kernel<1, 8, TASK>;
-  if (k <= 16) return fm_sgd_ordered_kernel<2, 8, TASK>;
-  if (k <= 32) return fm_sgd_ordered_kernel<4, 8, TASK>;
-  if (k <= 64) return fm_sgd_ordered_kernel<8, 8, TASK>;
-  if (k <= 128) return fm_sgd_ordered_kernel<16, 8, TASK>;
-  return fm_sgd_ordered_kernel<32, 8, TASK>;
+  if (k <= 1) return fm_sgd_ordered_kernel<1, 1, TASK, 0, H>;
+  if (k <= 2) return fm_sgd_ordered_kernel<1, 2, TASK, 0, H>;
+  if (k <= 4) return fm_sgd_ordered_kernel<1, 4, TASK, 0, H>;
+  if (k <= 8) return fm_sgd_ordered_kernel<1, 8, TASK, 0, H>;
+  if (k <= 16) return fm_sgd_ordered_kernel<2, 8, TASK, 0, H>;
+  if (k <= 32) return fm_sgd_ordered_kernel<4, 8, TASK, 0, H>;
+  if (k <= 64) return fm_sgd_ordered_kernel<8, 8, TASK, 0, false>;
+  if (k <= 128) return fm_sgd_ordered_kernel<16, 8, TASK, 0, false>;
+  return fm_sgd_ordered_kernel<32, 8, TASK, 0, false>;
 }
 
 // the stable (id, entry) sort in the scratch of the index build, [ids | ent_in | ent | sort temp]
@@ -305,31 +272,23 @@ cudaError_t launch_sgd_ordered(fmb200_ctx* c, DataSlot& d, bool* handled) {
   ordered_shape(c->k, &GL, &KF);
   // one group of GL lanes per example of a run: min(ORD_SMAX, 1024 / GL) examples
   int threads = std::min(ORD_SMAX * GL, ORD_MAX_THREADS);
-  const int bound = std::max(threads, 256);  // the kernel's launch bound
-  if (c->tune_threads)  // fewer threads = shorter runs; more = helper warps for the fetch issue / write-back
+  const int bound = std::max(threads, 256);  // the launch bound without helpers
+  if (c->tune_threads)  // fewer threads = shorter runs; more = threads that only share the fetch issue / write-back
     threads = std::min(bound, std::max(32, (c->tune_threads / (32 > GL ? 32 : GL)) * (32 > GL ? 32 : GL)));
-  OrdFn fn = c->hp.task == FMB200_TASK_REGRESSION ? pick_kernel<0>(c->k) : pick_kernel<1>(c->k);
-  if (c->tune_variant != 1) {  // variant 1 forces the general path
-    OrdFn fast = c->hp.task == FMB200_TASK_REGRESSION ? pick_fast_kernel<0>(c->k, d.max_row_nnz)
-                                                      : pick_fast_kernel<1>(c->k, d.max_row_nnz);
-    if (fast != nullptr) fn = fast;
-  }
-  // the warp-specialised form is the default where it exists (variant 1 / 2 and explicit thread counts keep
-  // the single-role kernels: comparisons, tests)
-  if (c->tune_variant != 1 && c->tune_variant != 2 && !c->tune_threads) {
-    int ncompute = 0;
-    OrdFn ws = c->hp.task == FMB200_TASK_REGRESSION ? pick_ws_kernel<0>(c->k, d.max_row_nnz, &ncompute)
-                                                    : pick_ws_kernel<1>(c->k, d.max_row_nnz, &ncompute);
-    if (ws != nullptr) {
-      fn = ws;
-      threads = ncompute + ORD_PARKED + ORD_HELPERS;
-    }
-  }
+  const bool fast = c->tune_variant != 1;  // variant 1 forces the general path
+  // the helper warp is the default where it fits (variant 1 / 2 and explicit thread counts keep every thread a
+  // compute thread: comparisons, tests)
+  const bool helpers = GL <= 4 && c->tune_variant != 1 && c->tune_variant != 2 && !c->tune_threads;
+  const bool reg = c->hp.task == FMB200_TASK_REGRESSION;
+  OrdFn fn = (helpers ? (reg ? pick_kernel<0, true> : pick_kernel<1, true>)
+                      : (reg ? pick_kernel<0, false> : pick_kernel<1, false>))(c->k, d.max_row_nnz, fast);
+  const int ncompute = threads;
+  if (helpers) threads += ORD_PARKED + ORD_HELPERS;
   e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
   fn<<<1, threads, smem, c->stream>>>(a);
   c->launches++;
-  c->last_cfg = EpochConfig{GL, std::min(ORD_SMAX, (threads >= ORD_SMAX * GL ? ORD_SMAX * GL : threads) / GL), TR, 1, threads, (int)smem, 0};
+  c->last_cfg = EpochConfig{GL, std::min(ORD_SMAX, ncompute / GL), TR, 1, threads, (int)smem, 0};
   *handled = true;
   if (want_prof) {
     unsigned long long h[16];

@@ -25,10 +25,11 @@
 //       the chain is re-walked behind the first contradicted one -- a consistent assignment
 //       IS the sequential answer (induction over t).  Classification (logistic multiplier)
 //       walks the chain serially from shared memory.
-//   (3) memory: one CTA owns the epoch (there is ONE chain), warp-specialised where the
-//       thread budget allows (ordered_epoch_body_ws): compute warps walk the runs of tile T
-//       while a helper warp writes tile T-1's final records back to global memory and
-//       fetches tile T+1's records (cp.async, L2 -> shared, 16 B) into a 3-deep ring; the CSR
+//   (3) memory: one CTA owns the epoch (there is ONE chain).  Compute warps walk the runs of
+//       tile T; tile T-1's final records are written back to global memory and tile T+1's
+//       records fetched (cp.async, L2 -> shared, 16 B) into a 3-deep ring by a helper warp
+//       beside the runs where the thread budget allows (k <= 32), else by the compute warps
+//       before them (ordered_epoch: one driver, two configurations); the CSR
 //       of tile T+2 arrives by TMA bulk copies (cp.async.bulk + mbarrier).  A record fetched
 //       that early is stale if its feature is written by tile T or T+1 itself; exactly those
 //       entries (known from `link`) skip the fetch and read the record FORWARDED in shared
@@ -876,12 +877,34 @@ __device__ __forceinline__ void ord_writeback(const OrderedArgs& a, unsigned cha
   }
 }
 
-// ---- driver 1: every thread does everything, phases separated by CTA barriers ------------------------
-template <int GL, int KF, int TASK, int ZF = 0>
-__device__ __forceinline__ void ordered_epoch_body(const OrderedArgs& a, unsigned char* smem) {
+// ---- the epoch driver --------------------------------------------------------------------------------
+// Threads [0, ncompute) are the compute threads: they walk the runs of tile T.  Threads [ncompute, ncompute +
+// nparked) leave after the set-up (warp w runs on scheduler w % 4: they choose which compute warps the helpers
+// share a scheduler with; measured to matter little, see fm_ordered.cu).  The rest, if any, are helpers.
+// The helper steps of tile T: write tile T-1's final records back to global memory, stage the CSR of tile T+2
+// (TMA into the stage tile T-1 held, which that write-back has just read), fetch tile T+1's records.
+//   - With helpers, they run these steps while the compute threads walk tile T.  The write-back and the fetch
+//     issue are LSU work a single SM issues at about one 16-byte request per cycle and neither is on the
+//     dependency chain; done by the compute threads they take a share of the stall samples.  One CTA barrier
+//     per tile joins the two roles.
+//   - Without helpers (k > 32, where the compute threads fill the CTA), the compute threads run the same
+//     steps themselves before the runs of tile T and leave tile T+1's fetches in flight during those runs.
+// Either way the fetch of tile T+1 is issued behind tile T-1's write-back (a barrier over the threads of the
+// helper steps in between), so what it may miss is what tiles T and T+1 write -- exactly the entries ord_prep
+// forwards from the ring.
+// HELPERS says at compile time whether there are helpers: one kernel that chose the configuration at run time
+// ran the C2-shaped epoch 5% slower (H100 80GB HBM3, 400 W).  Without helpers every barrier is a CTA barrier;
+// with them the compute threads (1) and the helpers (2) meet at named barriers.
+template <int GL, int KF, int TASK, int ZF, bool HELPERS>
+__device__ __forceinline__ void ordered_epoch(const OrderedArgs& a, unsigned char* smem, int ncompute,
+                                              int nparked) {
   constexpr int KC = ZF > 0 ? KF : 0;  // the fast kernels run with k == KF (even): fetch and write-back unroll
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nthreads = blockDim.x;
-  const int smax = min(ORD_SMAX, nthreads / GL);
+  const int hstart = ncompute + nparked;
+  // the threads of the helper steps: the helpers, or all compute threads (htid < 0: not one of them)
+  const int nhelp = HELPERS ? nthreads - hstart : ncompute, htid = HELPERS ? tid - hstart : tid;
+  const int nlive = nthreads - nparked, ltid = tid >= hstart ? tid - nparked : tid;
+  const int smax = min(ORD_SMAX, ncompute / GL);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem);
   int* sP = reinterpret_cast<int*>(smem + 32);
 
@@ -906,101 +929,7 @@ __device__ __forceinline__ void ordered_epoch_body(const OrderedArgs& a, unsigne
   const uint32_t NT = a.n_tiles;
   const int TR = a.tile_rows;
 
-  // producer state (thread 0): entry range of the next tile to stage, fetched a tile ahead
-  uint64_t policy = 0, nb = 0, ne = 0;
-  if (tid == 0) {
-    policy = policy_evict_first();
-    for (uint32_t t = 0; t < 2 && t < NT; t++) {
-      const uint64_t r0 = (uint64_t)t * TR, r1 = min(r0 + TR, a.n_rows);
-      ord_issue_csr(a, smem, bars, t, a.row_ptr[r0], a.row_ptr[r1], policy);
-    }
-    if (2 < NT) {
-      const uint64_t r0 = 2ull * TR, r1 = min(r0 + TR, a.n_rows);
-      nb = a.row_ptr[r0];
-      ne = a.row_ptr[r1];
-    }
-  }
-  mbar_wait(bars + 0, 0);
-  ord_prep<KC>(a, smem, 0, tid, nthreads);
-  cp_async_commit();
-
-  for (uint32_t T = 0; T < NT; T++) {
-    if (tid == 0 && T + 2 < NT) {  // stage (T+2)%3 held tile T-1: closed by the last barrier
-      ord_issue_csr(a, smem, bars, T + 2, nb, ne, policy);
-      if (T + 3 < NT) {
-        const uint64_t r0 = (uint64_t)(T + 3) * TR, r1 = min(r0 + TR, a.n_rows);
-        nb = a.row_ptr[r0];
-        ne = a.row_ptr[r1];
-      }
-    }
-    if (T + 1 < NT) {
-      mbar_wait(bars + (T + 1) % ORD_NBUF, ((T + 1) / ORD_NBUF) & 1);
-      ord_prep<KC>(a, smem, T + 1, tid, nthreads);
-    }
-    cp_async_commit();
-    cp_async_wait_1();  // this thread's fetches for tile T have landed
-    if (warp == 0) {    // length of the tile's first run (reads the CSR stage only: complete since the mbarrier)
-      const OrdStage s = ord_stage(a, smem, T);
-      const int nrows = (int)min((uint64_t)TR, a.n_rows - (uint64_t)T * TR);
-      const int P0 = ord_detect(s, 0, nrows, smax, lane);
-      if (lane == 0) sP[0] = P0;
-    }
-    __syncthreads();  // ... everyone's fetches; src[] of tile T; the first run length
-    ord_tile_runs<GL, KF, TASK, ZF, false>(a, smem, cc, T, tid, nthreads, w0, it, onehot);
-    ord_writeback<false, KC>(a, smem, cc, T, tid, nthreads);
-    __syncthreads();  // stage T%3 is read above and refilled by the TMA issue at the top of tile T+1
-  }
-  if (tid == 0 && cc.k0) *a.w0 = w0;
-  if (a.prof != nullptr && tid < 16) a.prof[tid] = reinterpret_cast<unsigned long long*>(smem + ORD_PROF_OFF)[tid];
-}
-
-// ---- driver 2: warp-specialised.  The first `ncompute` threads walk the runs of tile T; the remaining
-// (helper) threads meanwhile write tile T-1's final records back to global memory and then fetch tile T+1's
-// records.  With every thread doing everything in sequence, the write-back loop and the fetch issue take a
-// share of the stall samples; both are LSU work a
-// single SM issues at about one 16-byte request per cycle, and neither is on the dependency chain.
-//
-// Order of the global traffic is the single-role driver's: the fetch of tile T+1 is issued behind tile T-1's
-// write-back (same helper threads, a helper barrier in between), so what it may miss is what tiles T and T+1
-// write -- exactly the entries ord_prep forwards from the ring.  Tile T-1's CSR stage is read by its
-// write-back, so the TMA refill of that stage (tile T+2) is issued behind it.
-template <int GL, int KF, int TASK, int ZF = 0>
-__device__ __forceinline__ void ordered_epoch_body_ws(const OrderedArgs& a, unsigned char* smem, int ncompute,
-                                                      int nparked) {
-  constexpr int KC = ZF > 0 ? KF : 0;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nthreads = blockDim.x;
-  // Threads [ncompute, ncompute + nparked) leave after the set-up (warp w runs on scheduler w % 4: they choose
-  // which compute warps the helpers share a scheduler with; measured to matter little, see fm_ordered.cu).
-  const int hstart = ncompute + nparked;
-  const int nhelp = nthreads - hstart, htid = tid - hstart;
-  const bool helper = tid >= hstart;
-  const int nlive = nthreads - nparked, ltid = helper ? tid - nparked : tid;
-  const int smax = min(ORD_SMAX, ncompute / GL);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem);
-  int* sP = reinterpret_cast<int*>(smem + 32);
-
-  if (tid == 0) {
-    for (int i = 0; i < ORD_NBUF; i++) mbar_init(bars + i, 1);
-    fence_mbar_init();
-    reinterpret_cast<int*>(smem + 40)[0] = 0x7fffffff;
-    reinterpret_cast<int*>(smem + 40)[1] = 0x7fffffff;
-  }
-  if (tid < 16) reinterpret_cast<unsigned long long*>(smem + ORD_PROF_OFF)[tid] = 0ull;
-  for (int g = tid; g < ORD_SMAX; g += nthreads) reinterpret_cast<double2*>(smem + 64)[g] = make_double2(1.0, 0.0);
-  for (uint32_t t = 0; t < (uint32_t)ORD_NBUF; t++) {
-    unsigned char* sup = ord_stage(a, smem, t).sup;
-    for (uint32_t j = tid; j < a.tile_cap; j += nthreads) sup[j] = 0;
-  }
-  __syncthreads();
-
-  const OrdConsts cc = ord_consts(a);
-  double w0 = cc.k0 ? *a.w0 : 0.0;
-  uint32_t it = 0;
-  const bool onehot = (ZF == 2) && ((*a.shape & 3u) == 3u);
-  const uint32_t NT = a.n_tiles;
-  const int TR = a.tile_rows;
-
-  // producer state (helper thread 0): entry range of the next tile to stage, fetched a tile ahead
+  // producer state (htid 0): entry range of the next tile to stage, fetched a tile ahead
   uint64_t policy = 0, nb = 0, ne = 0;
   if (htid == 0) {
     policy = policy_evict_first();
@@ -1018,18 +947,21 @@ __device__ __forceinline__ void ordered_epoch_body_ws(const OrderedArgs& a, unsi
   mbar_wait(bars + 0, 0);
   ord_prep<KC>(a, smem, 0, ltid, nlive);  // the first tile's records: everybody fetches
   cp_async_commit();
-  cp_async_wait_0();
-  __syncthreads();
+  if (HELPERS) {  // (without helpers, the wait of tile 0 below covers these fetches)
+    cp_async_wait_0();
+    __syncthreads();
+  }
 
   long long tprof = 0;
-  ORD_PROF(tid == 0 || htid == 0, 15);
+  const bool cprof = HELPERS && tid == 0, hprof = HELPERS && htid == 0;  // the driver's phase timers: with helpers only
+  ORD_PROF(cprof || hprof, 15);
   for (uint32_t T = 0; T < NT; T++) {
-    if (helper) {
+    if (htid >= 0) {
       if (T > 0) {
-        ord_writeback<true, KC>(a, smem, cc, T - 1, htid, nhelp);
-        named_bar_sync(2, nhelp);  // the stores are issued (and sup[] is clear) before anything below
+        ord_writeback<HELPERS, KC>(a, smem, cc, T - 1, htid, nhelp);
+        ord_group_sync<HELPERS>(2, nhelp);  // the stores are issued (and sup[] is clear) before anything below
       }
-      ORD_PROF(htid == 0, 8);  // write-back
+      ORD_PROF(hprof, 8);  // write-back
       if (htid == 0 && T + 2 < NT) {  // stage (T+2)%3 held tile T-1, whose write-back just read it
         ord_issue_csr(a, smem, bars, T + 2, nb, ne, policy);
         if (T + 3 < NT) {
@@ -1040,33 +972,49 @@ __device__ __forceinline__ void ordered_epoch_body_ws(const OrderedArgs& a, unsi
       }
       if (T + 1 < NT) {
         mbar_wait(bars + (T + 1) % ORD_NBUF, ((T + 1) / ORD_NBUF) & 1);
-        ORD_PROF(htid == 0, 9);  // CSR issue + wait
+        ORD_PROF(hprof, 9);  // CSR issue + wait
         ord_prep<KC>(a, smem, T + 1, htid, nhelp);
       }
-      ORD_PROF(htid == 0, 10);  // fetch issue
+      ORD_PROF(hprof, 10);  // fetch issue
       cp_async_commit();
-      cp_async_wait_0();
-      ORD_PROF(htid == 0, 11);  // fetch landing
-    } else {
-      mbar_wait(bars + T % ORD_NBUF, (T / ORD_NBUF) & 1);  // (complete since a tile ago; acquires the TMA's writes)
-      if (warp == 0) {
+      if (HELPERS) cp_async_wait_0();  // tile T+1's records have landed
+      else cp_async_wait_1();     // this thread's fetches for tile T have landed, tile T+1's stay in flight
+      ORD_PROF(hprof, 11);  // fetch landing
+    }
+    if (tid < ncompute) {
+      // (complete since a tile ago; acquires the TMA's writes.  Without helpers every thread waited before ord_prep)
+      if (HELPERS) mbar_wait(bars + T % ORD_NBUF, (T / ORD_NBUF) & 1);
+      if (warp == 0) {  // length of the tile's first run (reads the CSR stage only)
         const OrdStage s = ord_stage(a, smem, T);
         const int nrows = (int)min((uint64_t)TR, a.n_rows - (uint64_t)T * TR);
         const int P0 = ord_detect(s, 0, nrows, smax, lane);
         if (lane == 0) sP[0] = P0;
       }
-      named_bar_sync(1, ncompute);
-      ORD_PROF(tid == 0, 6);  // tile prologue (CSR acquire, first run length)
-      ord_tile_runs<GL, KF, TASK, ZF, true>(a, smem, cc, T, tid, ncompute, w0, it, onehot);
-      ORD_PROF(tid == 0, 15);
+      ord_group_sync<HELPERS>(1, ncompute);  // the first run length (without helpers: also everyone's fetches, src[])
+      ORD_PROF(cprof, 6);  // tile prologue (CSR acquire, first run length)
+      ord_tile_runs<GL, KF, TASK, ZF, HELPERS>(a, smem, cc, T, tid, ncompute, w0, it, onehot);
+      ORD_PROF(cprof, 15);
     }
-    __syncthreads();  // tile T's slots are final, tile T+1's records have landed, tile T-1 is written back
-    ORD_PROF(tid == 0, 7);     // compute side: waiting for the helpers
-    ORD_PROF(htid == 0, 12);   // helper side: waiting for the compute warps
+    if (HELPERS) {  // (without helpers, the runs' last barrier and the one behind the next write-back do this)
+      __syncthreads();  // tile T's slots are final, tile T+1's records have landed, tile T-1 is written back
+      ORD_PROF(cprof, 7);   // compute side: waiting for the helpers
+      ORD_PROF(hprof, 12);  // helper side: waiting for the compute warps
+    }
   }
-  if (NT > 0) ord_writeback<false, KC>(a, smem, cc, NT - 1, ltid, nlive);
+  if (NT > 0) ord_writeback<false, KC>(a, smem, cc, NT - 1, ltid, nlive);  // every thread still running
   if (tid == 0 && cc.k0) *a.w0 = w0;
   if (a.prof != nullptr && tid < 16) a.prof[tid] = reinterpret_cast<unsigned long long*>(smem + ORD_PROF_OFF)[tid];
+}
+
+// The two configurations.  Without helpers every thread of the CTA is a compute thread.
+template <int GL, int KF, int TASK, int ZF = 0>
+__device__ __forceinline__ void ordered_epoch_body(const OrderedArgs& a, unsigned char* smem) {
+  ordered_epoch<GL, KF, TASK, ZF, false>(a, smem, blockDim.x, 0);
+}
+template <int GL, int KF, int TASK, int ZF = 0>
+__device__ __forceinline__ void ordered_epoch_body_ws(const OrderedArgs& a, unsigned char* smem, int ncompute,
+                                                      int nparked) {
+  ordered_epoch<GL, KF, TASK, ZF, true>(a, smem, ncompute, nparked);
 }
 
 }  // namespace fmb
