@@ -199,6 +199,8 @@ static int create_resources(fmb200_ctx* c, int device, const cudaDeviceProp& pro
   CK(cudaMemsetAsync(c->p64.base, 0, c->p64.n_doubles * sizeof(double), c->stream));
   CK(alloc(c->d_sched, 2));
   CK(cudaMemsetAsync(c->d_sched.get(), 0, 2 * sizeof(unsigned int), c->stream));
+  CK(alloc(c->d_gbar, 1));
+  CK(cudaMemsetAsync(c->d_gbar.get(), 0, sizeof(unsigned int), c->stream));
   CK(alloc(c->d_flag, 16));
   CK(host_alloc(c->h_flag, 16));
   {

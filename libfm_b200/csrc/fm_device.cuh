@@ -125,6 +125,17 @@ __device__ __forceinline__ void red_add_u64(unsigned long long* p, unsigned long
   asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(p), "l"(a) : "memory");
 }
 
+// ---- grid-scope release / acquire on a counter word (GridBarrier, fm_hogwild_common.cuh) -------------
+// release: this thread's earlier writes, and those it has observed, become visible before the add does
+__device__ __forceinline__ void red_release_add_u32(unsigned int* p, unsigned int a) {
+  asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(a) : "memory");
+}
+__device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int* p) {
+  unsigned int v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+
 // named barrier 1: producer warp arrives (non-blocking), consumer warps sync
 __device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");

@@ -50,6 +50,7 @@
 // Algorithmic HBM traffic per example (roofline numerator, BASELINE.json):
 // 2*k*nnz*4 bytes (V rows read + written back).
 #include <algorithm>
+#include <cstdio>
 
 #include "fm_hogwild_common.cuh"
 #include "fm_rowgroup.cuh"
@@ -390,6 +391,9 @@ static HogwildArgs make_args(fmb200_ctx* c, const DataSlot& d, uint64_t n_tiles,
   a.n_acc = 0;
   a.ramp_tiles = 0;
   a.ramp_conc_scale = a.ramp_w0_conc = 1.f;
+  a.gbar = nullptr;
+  a.gbar_base = 0;
+  a.prof = nullptr;
   a.sched = c->d_sched.get();
   a.global_entries = 0;
   return a;
@@ -422,8 +426,10 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, const DataSlot& d, bool* handle
   const bool combine = (double)d.max_feat_cnt * 32.0 / (double)d.n_rows > 0.5;
   // variant 3 = warp-specialised (producer warp + mbarrier hand-offs, no block barrier)
   const bool ws = c->tune_variant == 3;
+  // variant 132 = the window kernel with phase timers, printed per window (development aid)
+  const bool want_prof = c->tune_variant == 132;
   HogwildKernelFn fn = ws ? pick_rowlane_ws_kernel(gp, (int)d.max_row_nnz, damp, combine)
-                          : pick_rowlane_kernel(gp, (int)d.max_row_nnz, damp, combine);
+                          : pick_rowlane_kernel(gp, (int)d.max_row_nnz, damp, combine, want_prof);
   if (fn == nullptr) return cudaSuccess;
   const int smem = (ws ? HW_WS_HDR_BYTES : HW_HDR_BYTES) + HW_NSTAGE * (int)sbytes;
   const int launch_threads = ws ? threads + 32 : threads;
@@ -466,6 +472,7 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, const DataSlot& d, bool* handle
     // in flight), in one cooperative launch; each window reads the state the previous one left and
     // its steps are folded in after it: the same result on every run.  A ramp window is one tile.
     const uint64_t n_acc = c->p32.n_floats;
+    if (n_acc % 4 != 0) return cudaErrorInvalidValue;  // the fold takes float4s (Params32: blocks of 4 floats)
     if (!c->d_acc) {
       if ((e = alloc(c->d_acc, n_acc + 1)) != cudaSuccess) return e;
       e = cudaMemsetAsync(c->d_acc.get(), 0, (n_acc + 1) * sizeof(unsigned long long), c->stream);
@@ -485,13 +492,37 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, const DataSlot& d, bool* handle
       a.ramp_conc_scale = (float)((double)TR / (double)d.n_rows);
       a.ramp_w0_conc = (float)TR;
     }
+    a.gbar = c->d_gbar.get();
+    a.gbar_base = c->gbar_count;
+    if (want_prof) {
+      if ((e = cudaMalloc(&a.prof, RL_PROF_SLOTS * sizeof(unsigned long long))) != cudaSuccess) return e;
+      if ((e = cudaMemsetAsync(a.prof, 0, RL_PROF_SLOTS * sizeof(unsigned long long), c->stream)) != cudaSuccess)
+        return e;
+    }
     // cooperative: the grid barriers between windows need every CTA resident; a grid that cannot be
     // fails to launch instead of hanging (grid <= occ * SMs holds by construction)
     void* args[] = {&a};
     e = cudaLaunchCooperativeKernel((const void*)fn, dim3(grid), dim3(launch_threads), args, (size_t)smem,
                                     c->stream);
-    if (e != cudaSuccess) return e;
+    if (e != cudaSuccess) {
+      cudaFree(a.prof);
+      return e;
+    }
     c->launches++;
+    // every CTA arrives once at each grid barrier of the launch (wraps modulo 2^32, as the counter does)
+    const uint32_t n_win = rowlane_windows(a.n_tiles, a.ramp_tiles, (uint32_t)grid);
+    c->gbar_count += (uint32_t)grid * rowlane_barriers(a.n_tiles, a.ramp_tiles, (uint32_t)grid);
+    if (want_prof) {
+      unsigned long long h[RL_PROF_SLOTS];
+      if ((e = cudaMemcpyAsync(h, a.prof, sizeof(h), cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess) return e;
+      if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) return e;
+      cudaFree(a.prof);
+      static const char* name[RL_PROF_SLOTS] = {"bias+gather", "score+issue", "bulk_wait", "barrier1", "fold",
+                                                "barrier2"};
+      fprintf(stderr, "[rowlane phases, cycles per window of CTA thread 0 (%u windows x %d CTAs)]", n_win, grid);
+      for (int i = 0; i < RL_PROF_SLOTS; i++) fprintf(stderr, " %s=%.1f", name[i], (double)h[i] / n_win / grid);
+      fprintf(stderr, "\n");
+    }
   }
   c->last_cfg = EpochConfig{1, (int)std::max<uint32_t>(1, d.max_row_nnz), TR, grid, launch_threads, smem, damp ? 1 : 0};
   *handled = true;

@@ -64,6 +64,42 @@ struct HogwildArgs {
   // fm_sgd_rowlane_kernel: the first ramp_tiles windows are one tile each, with these concurrencies
   uint32_t ramp_tiles;
   float ramp_conc_scale, ramp_w0_conc;
+  // fm_sgd_rowlane_kernel: the grid barriers' arrival counter and its value when the launch starts (GridBarrier)
+  unsigned int* gbar;
+  uint32_t gbar_base;
+  unsigned long long* prof;  // phase timers (development aid): RL_PROF_SLOTS clock64 sums over the CTAs, or null
+};
+
+// Windows of the row-lane epoch over n_tiles tiles: `ramp` windows of one tile, then windows of G tiles
+// (the grid), the last one what is left
+__host__ __device__ inline uint32_t rowlane_windows(uint32_t n_tiles, uint32_t ramp, uint32_t G) {
+  return ramp + (n_tiles - ramp + G - 1) / G;
+}
+// The row-lane epoch separates its windows by 2 * windows - 1 grid barriers (none behind the last fold)
+__host__ __device__ inline uint32_t rowlane_barriers(uint32_t n_tiles, uint32_t ramp, uint32_t G) {
+  return 2u * rowlane_windows(n_tiles, ramp, G) - 1u;
+}
+
+// Split-phase grid barrier of a cooperative launch (every CTA resident).  Each CTA adds 1 to a counter
+// with release semantics when it arrives, and its thread 0 polls the counter with acquire loads until
+// all gridDim.x CTAs have arrived; bar.sync on both sides extends both orderings to the whole CTA.
+// The counter only grows: barrier k of a launch is complete at base + (k+1)·gridDim.x, compared modulo
+// 2^32, so it is never reset and the host passes each launch the value its predecessors left.
+// Work placed between arrive() and wait() overlaps the other CTAs' arrival.
+struct GridBarrier {
+  unsigned int* count;
+  uint32_t target;  // the counter's value once the latest barrier arrived at is complete
+  __device__ __forceinline__ void arrive(int tid) {
+    __syncthreads();
+    if (tid == 0) red_release_add_u32(count, 1u);
+    target += gridDim.x;
+  }
+  __device__ __forceinline__ void wait(int tid) {
+    if (tid == 0)
+      while ((int32_t)(ld_acquire_u32(count) - target) < 0) {
+      }
+    __syncthreads();
+  }
 };
 
 // Fixed point of the accumulated steps: integer sums do not depend on the order in which the
@@ -240,8 +276,10 @@ struct TileSched {
 using HogwildKernelFn = void (*)(const HogwildArgs);
 
 // fm_rowlane.cu: kernel for (float4 chunks per row gp in {1,2}, rows of at most Z entries); a
-// cooperative launch whose grid size is the window size
-HogwildKernelFn pick_rowlane_kernel(int gp, int max_row_nnz, bool damp, bool combine);
+// cooperative launch whose grid size is the window size.  prof: the instantiation with phase timers.
+HogwildKernelFn pick_rowlane_kernel(int gp, int max_row_nnz, bool damp, bool combine, bool prof);
+// its phase timers: cycles of CTA thread 0 per window, summed over the CTAs
+constexpr int RL_PROF_SLOTS = 6;  // bias+gather, score+issue, bulk wait, barrier 1, fold, barrier 2
 // warp-specialised variant: blockDim = rows_per_tile + 32, smem header HW_WS_HDR_BYTES
 HogwildKernelFn pick_rowlane_ws_kernel(int gp, int max_row_nnz, bool damp, bool combine);
 

@@ -25,11 +25,7 @@
 //  * GP == 1 (k <= 4): a factor row is a single float4; every lane fetches its own.
 #include <algorithm>
 
-#include <cooperative_groups.h>
-
 #include "fm_hogwild_common.cuh"
-
-namespace cg = cooperative_groups;
 
 namespace fmb {
 
@@ -262,18 +258,33 @@ __device__ __forceinline__ void rowlane_tile(const HogwildArgs& a, const uint64_
 // the next window starts.  So every row of a window sees the state as the previous window left it,
 // whichever CTA runs it and whenever, and the epoch computes the same state on every run.
 // Every CTA runs every window's barriers and fold, with or without a tile in it.
-template <int GP, int Z, bool DAMP, bool COMBINE>
+// PROF: phase timers (development aid, launch_rowlane: tuning variant 132).  Thread 0 adds the cycles of
+// each phase of a window to a shared-memory slot; the sums go to a.prof once, at the end.
+constexpr int RL_PROF_OFF = 200;  // RL_PROF_SLOTS u64 in the spare bytes of the HW_HDR_BYTES header
+
+template <int GP, int Z, bool DAMP, bool COMBINE, bool PROF>
 __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const HogwildArgs a) {
   extern __shared__ __align__(128) unsigned char smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem);
   float* s_acc = reinterpret_cast<float*>(smem + 64);
-  cg::grid_group grid = cg::this_grid();
+  unsigned long long* s_prof = reinterpret_cast<unsigned long long*>(smem + RL_PROF_OFF);
 
   const int tid = threadIdx.x;
   const int TR = a.tile_rows;  // == blockDim.x
   const uint32_t G = gridDim.x;
   const uint32_t R = a.ramp_tiles;
-  const uint32_t n_win = R + (a.n_tiles - R + G - 1) / G;
+  const uint32_t n_win = rowlane_windows(a.n_tiles, R, G);
+  long long tprof = 0;
+  auto prof_mark = [&](int slot) {  // the cycles since the previous mark go to `slot`
+    if constexpr (PROF) {
+      if (tid == 0) {
+        const long long now = clock64();
+        s_prof[slot] += (unsigned long long)(now - tprof);
+        tprof = now;
+      }
+    }
+  };
+  if (PROF && tid < RL_PROF_SLOTS) s_prof[tid] = 0ull;  // ordered before any mark by ring_init's barrier
   // this CTA's tile of window j, or HW_NO_TILE
   auto tile_of = [&](uint32_t j) -> uint32_t {
     const uint32_t t = j < R ? (blockIdx.x == 0 ? j : HW_NO_TILE) : R + (j - R) * G + blockIdx.x;
@@ -305,7 +316,15 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const
 
   const bool use_w0 = a.use_w0 != 0;
   const float lr = a.lr;
+  GridBarrier gbar{a.gbar, a.gbar_base};
+  // This thread's slice of the fold: the four elements [4q, 4q+4) for every q ≡ q0 (mod fold_stride) below
+  // n_acc / 4 (the launcher checks that n_acc is a multiple of 4; the flag word acc[n_acc] lies behind).
+  const uint64_t q0 = blockIdx.x * (uint64_t)blockDim.x + tid;
   const uint64_t fold_stride = (uint64_t)G * blockDim.x;
+  const uint64_t n_vec = a.n_acc / 4;
+  float4* state4 = reinterpret_cast<float4*>(a.state);
+  ulonglong2* acc2 = reinterpret_cast<ulonglong2*>(a.acc);  // two u64 steps per 16-byte access
+  if (PROF && tid == 0) tprof = clock64();
 
   int it = 0;  // tiles this CTA has run
   for (uint32_t j = 0; j < n_win; ++j) {
@@ -346,7 +365,12 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const
       float mult, hj, w0 = 0.f;
       rowlane_tile<GP, Z, DAMP, COMBINE, true>(
           w, rp, ys, ids, xs, rows_here, tid,
-          [&]() { return w0 = bias.get(use_w0, tid, it, (int)blockDim.x); }, mult, hj);
+          [&]() {
+            w0 = bias.get(use_w0, tid, it, (int)blockDim.x);
+            prof_mark(0);  // bias fetch and gathers: the scores need both
+            return w0;
+          },
+          mult, hj);
       // ---- bias: one damped reduction into the global w0 per tile ----
       float2* s_part = reinterpret_cast<float2*>(s_acc) + (it & 1) * 8;  // [2 slots][8 warps]
       if (use_w0) bias_partial(s_part, mult, hj, tid);
@@ -367,22 +391,50 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const
       }
       ++it;
     }
+    prof_mark(1);  // scores, quantisation, reductions issued, bias partials
     // every step of the window is in the accumulator: the bulk reductions' writes are complete and,
     // through the proxy fence, ordered before the barrier's release like the generic reductions
     bulk_wait_all();
     fence_proxy_async_global();
-    grid.sync();
+    gbar.arrive(tid);
+    prof_mark(2);
+    // Only the fold writes the state, and this slice only this thread's fold: its first state vector can be
+    // read while the other CTAs arrive.  acc and state through L2 (ld.global.cg): an L1 line from an
+    // earlier window would be stale.
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (q0 < n_vec) s = __ldcg(state4 + q0);
+    gbar.wait(tid);
+    prof_mark(3);
     // ---- fold: state[i] += acc[i] (fixed point), acc[i] = 0; all NaN once a step overflowed ----
-    // acc and state through L2 (ld.global.cg): an L1 line from an earlier window would be stale
     const bool bad = __ldcg(a.acc + a.n_acc) != 0ull;
-    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + tid; i < a.n_acc; i += fold_stride) {
-      const long long q = (long long)__ldcg(a.acc + i);
-      if (bad) a.state[i] = __int_as_float(0x7fffffff);
-      else if (q != 0) a.state[i] = __ldcg(a.state + i) + (float)((double)q * (1.0 / (double)kAccScale));
-      if (q != 0) a.acc[i] = 0ull;
+    for (uint64_t q = q0; q < n_vec; q += fold_stride) {
+      const ulonglong2 lo = __ldcg(acc2 + 2 * q), hi = __ldcg(acc2 + 2 * q + 1);
+      if (q != q0) s = __ldcg(state4 + q);
+      auto fold = [&](float& x, unsigned long long u) {
+        if (bad) x = __int_as_float(0x7fffffff);
+        else if (u != 0ull) x = x + (float)((double)(long long)u * (1.0 / (double)kAccScale));
+      };
+      fold(s.x, lo.x);
+      fold(s.y, lo.y);
+      fold(s.z, hi.x);
+      fold(s.w, hi.y);
+      // elements without a step keep their value, so a whole-vector store rewrites them unchanged; likewise
+      // a pair of accumulator words is cleared whole when either holds a step
+      if (bad || (lo.x | lo.y | hi.x | hi.y) != 0ull) state4[q] = s;
+      if ((lo.x | lo.y) != 0ull) acc2[2 * q] = make_ulonglong2(0ull, 0ull);
+      if ((hi.x | hi.y) != 0ull) acc2[2 * q + 1] = make_ulonglong2(0ull, 0ull);
     }
-    if (j + 1 < n_win) grid.sync();  // the next window reads the folded state into a zero accumulator
-    fence_proxy_async_global();      // ... and its bulk reductions add to the fold's zeros
+    prof_mark(4);
+    if (j + 1 < n_win) {  // the next window reads the folded state into a zero accumulator
+      gbar.arrive(tid);
+      gbar.wait(tid);
+    }
+    fence_proxy_async_global();  // ... and its bulk reductions add to the fold's zeros
+    prof_mark(5);
+  }
+  if constexpr (PROF) {
+    __syncthreads();
+    if (tid < RL_PROF_SLOTS) atomicAdd(a.prof + tid, s_prof[tid]);
   }
 }
 
@@ -490,18 +542,23 @@ __global__ void __launch_bounds__(HW_MAX_THREADS + 32, 3) fm_sgd_rowlane_ws_kern
   }
 }
 
-template <int GP, int Z>
+template <int GP, int Z, bool PROF>
 static HogwildKernelFn pick_d(bool damp, bool combine) {
   if (combine)
-    return damp ? fm_sgd_rowlane_kernel<GP, Z, true, true> : fm_sgd_rowlane_kernel<GP, Z, false, true>;
-  return damp ? fm_sgd_rowlane_kernel<GP, Z, true, false> : fm_sgd_rowlane_kernel<GP, Z, false, false>;
+    return damp ? fm_sgd_rowlane_kernel<GP, Z, true, true, PROF> : fm_sgd_rowlane_kernel<GP, Z, false, true, PROF>;
+  return damp ? fm_sgd_rowlane_kernel<GP, Z, true, false, PROF> : fm_sgd_rowlane_kernel<GP, Z, false, false, PROF>;
+}
+
+template <int GP, int Z>
+static HogwildKernelFn pick_p(bool damp, bool combine, bool prof) {
+  return prof ? pick_d<GP, Z, true>(damp, combine) : pick_d<GP, Z, false>(damp, combine);
 }
 
 template <int GP>
-static HogwildKernelFn pick_z(int z, bool damp, bool combine) {
-  if (z <= 1) return pick_d<GP, 1>(damp, combine);
-  if (z <= 2) return pick_d<GP, 2>(damp, combine);
-  if (z <= 4) return pick_d<GP, 4>(damp, combine);
+static HogwildKernelFn pick_z(int z, bool damp, bool combine, bool prof) {
+  if (z <= 1) return pick_p<GP, 1>(damp, combine, prof);
+  if (z <= 2) return pick_p<GP, 2>(damp, combine, prof);
+  if (z <= 4) return pick_p<GP, 4>(damp, combine, prof);
   return nullptr;
 }
 
@@ -526,9 +583,9 @@ HogwildKernelFn pick_rowlane_ws_kernel(int gp, int max_row_nnz, bool damp, bool 
   return nullptr;
 }
 
-HogwildKernelFn pick_rowlane_kernel(int gp, int max_row_nnz, bool damp, bool combine) {
-  if (gp == 1) return pick_z<1>(max_row_nnz, damp, combine);
-  if (gp == 2) return pick_z<2>(max_row_nnz, damp, combine);
+HogwildKernelFn pick_rowlane_kernel(int gp, int max_row_nnz, bool damp, bool combine, bool prof) {
+  if (gp == 1) return pick_z<1>(max_row_nnz, damp, combine, prof);
+  if (gp == 2) return pick_z<2>(max_row_nnz, damp, combine, prof);
   return nullptr;
 }
 

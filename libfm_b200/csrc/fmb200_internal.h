@@ -208,6 +208,8 @@ struct fmb200_ctx {
   uint64_t pred_cap = 0;
   fmb::DevPtr<unsigned int> d_sched;   // hogwild tile scheduler: [next tile, CTAs run dry]
   fmb::DevPtr<unsigned long long> d_acc;  // fixed-point accumulator of the row-lane epoch (fm_hogwild.cu)
+  fmb::DevPtr<unsigned int> d_gbar;    // row-lane epoch: arrival counter of its grid barriers (never reset) ...
+  uint32_t gbar_count = 0;             // ... and its value once every launch enqueued so far has run
   fmb::DevPtr<unsigned int> d_flag;    // 16 device words: upload-time inspection results
   fmb::HostPtr<unsigned int> h_flag;   // pinned host mirror of d_flag
   fmb::HostPtr<unsigned char> h_stage;  // pinned staging for set/get_params (small models)
