@@ -39,7 +39,7 @@ CU_SOURCES = {
     "fm_mcmc.cu": ["--fmad=false"],
 }
 CU_HEADERS = ["fm_device.cuh", "fm_rowgroup.cuh", "fm_hogwild_common.cuh", "fmb200_internal.h",
-              "fm_inorder_wavefront.cuh", "fm_ordered.cuh", "fm_roworder.cuh"]
+              "fm_inorder_wavefront.cuh", "fm_ordered.cuh", "fm_roworder.cuh", "ref_random.h"]
 
 
 def _newer(target: str, deps: list[str]) -> bool:
@@ -96,6 +96,7 @@ def build_cli(force: bool = False) -> str | None:
         return None
     os.makedirs(BINDIR, exist_ok=True)
     hdrs = [os.path.join(HOST, f) for f in os.listdir(HOST) if f.endswith(".h")]
+    hdrs.append(os.path.join(CSRC, "ref_random.h"))  # fm_host.h includes it
     out = cli_path()
     if force or _newer(out, [main] + hdrs + [lib_path()]):
         cmd = ["g++", "-O2", "-std=c++17", "-Wall", "-I", os.path.join(ROOT, "include"), main,

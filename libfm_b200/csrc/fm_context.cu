@@ -163,6 +163,27 @@ int need_slot(fmb200_ctx* c, int slot) {
   return 0;
 }
 
+// the fp64 learners need an fp64 mode (INORDER or ORDERED) to be live; `what` says which needs it
+int need_fp64(const fmb200_ctx* c, const char* what) {
+  if (c->mode == FMB200_MODE_HOGWILD) return fail("%s", what);
+  return 0;
+}
+
+// body() between the context's two events; *device_seconds (may be null) := the time between them
+template <class F>
+int timed(fmb200_ctx* c, double* device_seconds, F&& body) {
+  CK(cudaEventRecord(c->ev0.get(), c->stream));
+  if (body()) return 1;
+  CK(cudaEventRecord(c->ev1.get(), c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  if (device_seconds) {
+    float ms = 0.f;
+    CK(cudaEventElapsedTime(&ms, c->ev0.get(), c->ev1.get()));
+    *device_seconds = (double)ms * 1e-3;
+  }
+  return 0;
+}
+
 }  // namespace
 
 // Everything of fmb200_create that can fail after the context object exists; the caller
@@ -521,13 +542,11 @@ int fmb200_sgd_epoch_async(fmb200_ctx* c, int slot) {
   if (bind(c)) return 1;
   DataSlot& d = c->slots[slot];
   if (c->mode == FMB200_MODE_ORDERED) {
-    if (c->k > 256) return fail("num_factor > 256 is not supported in the fp64 modes");
     bool handled = false;
     CK(launch_sgd_ordered(c, d, &handled));
     // shapes the ring cannot hold run row-at-a-time: the same order, just slower
     if (!handled) CK(launch_sgd_inorder(c, d));
   } else if (c->mode == FMB200_MODE_INORDER) {
-    if (c->k > 256) return fail("num_factor > 256 is not supported in the fp64 modes");
     CK(launch_sgd_inorder(c, d));
   } else {
     if (c->kp > 128) return fail("num_factor > 128 is not supported in HOGWILD mode");
@@ -547,16 +566,7 @@ int fmb200_sync(fmb200_ctx* c) {
 int fmb200_sgd_epoch(fmb200_ctx* c, int slot, double* device_seconds) {
   NEED_CTX(c);
   if (bind(c)) return 1;
-  CK(cudaEventRecord(c->ev0.get(), c->stream));
-  if (fmb200_sgd_epoch_async(c, slot)) return 1;
-  CK(cudaEventRecord(c->ev1.get(), c->stream));
-  CK(cudaStreamSynchronize(c->stream));
-  if (device_seconds) {
-    float ms = 0.f;
-    CK(cudaEventElapsedTime(&ms, c->ev0.get(), c->ev1.get()));
-    *device_seconds = (double)ms * 1e-3;
-  }
-  return 0;
+  return timed(c, device_seconds, [&] { return fmb200_sgd_epoch_async(c, slot); });
 }
 
 int fmb200_evaluate(fmb200_ctx* c, int slot, double* sum_sq_err, double* sum_abs_err,
@@ -636,7 +646,7 @@ int fmb200_predict(fmb200_ctx* c, int slot, int transform, double* out) {
 int fmb200_sgda_begin(fmb200_ctx* c, uint32_t n_groups, const uint32_t* attr_group) {
   NEED_CTX(c);
   if (bind(c)) return 1;
-  if (c->mode == FMB200_MODE_HOGWILD) return fail("SGDA runs on the fp64 state: set INORDER or ORDERED mode first");
+  if (need_fp64(c, "SGDA runs on the fp64 state: set INORDER or ORDERED mode first")) return 1;
   if (n_groups == 0 || n_groups > 1024) return fail("n_groups must be in [1,1024]");
   if (n_groups > 1 && !attr_group) return fail("attr_group is required for more than one group");
   if (attr_group)
@@ -671,19 +681,12 @@ int fmb200_sgda_epoch(fmb200_ctx* c, int train_slot, int val_slot, int lambda_st
   NEED_CTX(c);
   if (need_slot(c, train_slot) || need_slot(c, val_slot)) return 1;
   if (bind(c)) return 1;
-  if (c->mode == FMB200_MODE_HOGWILD) return fail("SGDA runs on the fp64 state: set INORDER or ORDERED mode first");
+  if (need_fp64(c, "SGDA runs on the fp64 state: set INORDER or ORDERED mode first")) return 1;
   if (c->sgda_groups == 0) return fail("call fmb200_sgda_begin first");
-  if (c->k > 256) return fail("num_factor > 256 is not supported in the fp64 modes");
-  CK(cudaEventRecord(c->ev0.get(), c->stream));
-  CK(launch_sgda_epoch(c, c->slots[train_slot], c->slots[val_slot], lambda_steps));
-  CK(cudaEventRecord(c->ev1.get(), c->stream));
-  CK(cudaStreamSynchronize(c->stream));
-  if (device_seconds) {
-    float ms = 0.f;
-    CK(cudaEventElapsedTime(&ms, c->ev0.get(), c->ev1.get()));
-    *device_seconds = (double)ms * 1e-3;
-  }
-  return 0;
+  return timed(c, device_seconds, [&]() -> int {
+    CK(launch_sgda_epoch(c, c->slots[train_slot], c->slots[val_slot], lambda_steps));
+    return 0;
+  });
 }
 
 int fmb200_sgda_get_reg(fmb200_ctx* c, double* reg_w, double* reg_v) {
@@ -701,8 +704,7 @@ int fmb200_mcmc_eterms(fmb200_ctx* c, int slot, double* e_out) {
   NEED_CTX(c);
   if (need_slot(c, slot)) return 1;
   if (bind(c)) return 1;
-  if (c->mode == FMB200_MODE_HOGWILD)
-    return fail("e-terms are computed from the fp64 state: set INORDER or ORDERED mode first");
+  if (need_fp64(c, "e-terms are computed from the fp64 state: set INORDER or ORDERED mode first")) return 1;
   const DataSlot& d = c->slots[slot];
   if (d.n_rows == 0) return 0;
   if (!e_out) return fail("null output pointer");
@@ -719,8 +721,7 @@ int fmb200_mcmc_begin(fmb200_ctx* c, int train_slot, int test_slot, int do_sampl
   NEED_CTX(c);
   if (need_slot(c, train_slot) || need_slot(c, test_slot)) return 1;
   if (bind(c)) return 1;
-  if (c->mode == FMB200_MODE_HOGWILD)
-    return fail("MCMC / ALS run on the fp64 state: set INORDER or ORDERED mode first");
+  if (need_fp64(c, "MCMC / ALS run on the fp64 state: set INORDER or ORDERED mode first")) return 1;
   if (!w_lambda || (!v_lambda && c->k > 0)) return fail("null w_lambda / v_lambda");
   if (c->peer_world > 1) return fail("MCMC / ALS run on one GPU: this context is attached to a multi-GPU peer world");
   return guarded([&]() {
@@ -737,8 +738,7 @@ int fmb200_mcmc_begin(fmb200_ctx* c, int train_slot, int test_slot, int do_sampl
 int fmb200_mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counters) {
   NEED_CTX(c);
   if (!c->mcmc) return fail("call fmb200_mcmc_begin first");
-  if (c->mode == FMB200_MODE_HOGWILD)
-    return fail("MCMC / ALS run on the fp64 state: set INORDER or ORDERED mode first");
+  if (need_fp64(c, "MCMC / ALS run on the fp64 state: set INORDER or ORDERED mode first")) return 1;
   if (bind(c)) return 1;
   return guarded([&]() {
     double m = 0.0;

@@ -23,15 +23,17 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 #include <vector>
 
 #include "fm_roworder.cuh"
 #include "fmb200_internal.h"
+#include "ref_random.h"
 
 namespace cg = cooperative_groups;
 
 namespace fmb {
+
+using namespace ref_random;
 
 // hyperpriors, fm_learn_mcmc.h:1107-1114
 constexpr double kAlpha0 = 1.0, kGamma0 = 1.0, kBeta0 = 1.0, kMu0 = 0.0, kW0Mean0 = 0.0;
@@ -66,103 +68,7 @@ void McmcDelete::operator()(McmcState* s) const { delete s; }
 
 namespace {
 
-// ---- the reference's samplers (util/random.h), restated: same algorithms, same operations ----
-// Leva's ratio-of-uniforms normal; Marsaglia-Tsang gamma; Robert's exponential-proposal
-// truncated normal; the Abramowitz-Stegun 7.1.26 erf.
-double ran_uniform() { return rand() / ((double)RAND_MAX + 1); }
-
-double ran_gaussian() {
-  double u, v, x, y, Q;
-  do {
-    do {
-      u = ran_uniform();
-    } while (u == 0.0);
-    v = 1.7156 * (ran_uniform() - 0.5);
-    x = u - 0.449871;
-    y = std::abs(v) + 0.386595;
-    Q = x * x + y * (0.19600 * y - 0.25472 * x);
-    if (Q < 0.27597) break;
-  } while ((Q > 0.27846) || ((v * v) > (-4.0 * u * u * std::log(u))));
-  return v / u;
-}
-
-double ran_gaussian(double mean, double stdev) {
-  if ((stdev == 0.0) || std::isnan(stdev)) return mean;
-  return mean + stdev * ran_gaussian();
-}
-
-double ran_gamma(double a) {
-  if (a < 1.0) {
-    double u;
-    do {
-      u = ran_uniform();
-    } while (u == 0.0);
-    return ran_gamma(a + 1.0) * std::pow(u, 1.0 / a);
-  }
-  const double d = a - 1.0 / 3.0;
-  const double c = 1.0 / std::sqrt(9.0 * d);
-  double x, v, u;
-  do {
-    do {
-      x = ran_gaussian();
-      v = 1.0 + c * x;
-    } while (v <= 0.0);
-    v = v * v * v;
-    u = ran_uniform();
-  } while ((u >= (1.0 - 0.0331 * (x * x) * (x * x))) && (std::log(u) >= (0.5 * x * x + d * (1.0 - v + std::log(v)))));
-  return d * v;
-}
-
-double ran_gamma(double a, double b) { return ran_gamma(a) / b; }
-
-double ran_exp() { return -std::log(1 - ran_uniform()); }
-
-double ran_left_tgaussian(double left) {
-  if (left <= 0.0) {
-    double r;
-    do {
-      r = ran_gaussian();
-    } while (r < left);
-    return r;
-  }
-  const double alpha_star = 0.5 * (left + std::sqrt(left * left + 4.0));
-  for (;;) {
-    const double z = ran_exp() / alpha_star + left;
-    double d = z - alpha_star;
-    d = std::exp(-(d * d) / 2);
-    const double u = ran_uniform();
-    if (u < d) return z;
-  }
-}
-
-double ran_left_tgaussian(double left, double mean, double stdev) {
-  return mean + stdev * ran_left_tgaussian((left - mean) / stdev);
-}
-
-double ran_right_tgaussian(double right, double mean, double stdev) {
-  return mean + stdev * -ran_left_tgaussian(-((right - mean) / stdev));
-}
-
-double as_erf(double x) {
-  const double t = x >= 0 ? 1.0 / (1.0 + 0.3275911 * x) : 1.0 / (1.0 - 0.3275911 * x);
-  const double r = 1.0 - (t * (0.254829592 + t * (-0.284496736 + t * (1.421413741 + t * (-1.453152027 + t * 1.061405429))))) *
-                             std::exp(-x * x);
-  return x >= 0 ? r : -r;
-}
-
-double cdf_gaussian(double x) { return 0.5 + 0.5 * as_erf(0.707106781 * x); }
-
 // ---- device: index build -------------------------------------------------------------------
-__device__ __forceinline__ uint32_t row_of(const uint64_t* rp, uint64_t n_rows, uint64_t e) {
-  uint64_t lo = 0, hi = n_rows;  // largest r with rp[r] <= e
-  while (hi - lo > 1) {
-    const uint64_t mid = (lo + hi) >> 1;
-    if (rp[mid] <= e) lo = mid;
-    else hi = mid;
-  }
-  return (uint32_t)lo;
-}
-
 // prev[j] = 1 + the largest id below j that shares a case with j (0: none); one thread per case
 __global__ void mcmc_prev_kernel(const uint64_t* __restrict__ rp, const uint32_t* __restrict__ col, uint64_t n_rows,
                                  unsigned int* prev) {
@@ -184,10 +90,10 @@ __global__ void mcmc_csc_kernel(const uint32_t* __restrict__ ids, const uint32_t
                                 const uint64_t* __restrict__ rp, uint64_t n_rows, const float* __restrict__ val,
                                 uint32_t* cs_case, float* cs_x, uint32_t* dup) {
   for (uint64_t p = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; p < nnz; p += (uint64_t)gridDim.x * blockDim.x) {
-    const uint32_t r = row_of(rp, n_rows, ent[p]);
+    const uint32_t r = (uint32_t)row_of(rp, n_rows, ent[p]);
     cs_case[p] = r;
     cs_x[p] = val[ent[p]];
-    if (p > 0 && ids[p - 1] == ids[p] && row_of(rp, n_rows, ent[p - 1]) == r) dup[ids[p]] = 1u;
+    if (p > 0 && ids[p - 1] == ids[p] && (uint32_t)row_of(rp, n_rows, ent[p - 1]) == r) dup[ids[p]] = 1u;
   }
 }
 
@@ -341,19 +247,11 @@ __global__ void __launch_bounds__(256) mcmc_sweep_kernel(const SweepArgs a) {
   }
   if (a.use_w) sweep_runs<false>(a, grid, 0, warp, nwarp, lane);
   for (int f = 0; f < a.k; f++) {
-    // q_c = 0 + sum v_jf x over the case's entries in (id, entry) order (add_main_q, :406-428)
-    for (uint64_t c = tid; c < a.n_rows; c += nth) {
+    for (uint64_t c = tid; c < a.n_rows; c += nth) {  // the q rebuild (add_main_q, :406-428)
       const uint64_t beg = a.row_ptr[c];
-      const uint32_t size = (uint32_t)(a.row_ptr[c + 1] - beg);
       RowOrder o;
-      o.init(a.col + beg, size);
-      double q = 0.0;
-      uint32_t pos = 0;
-      for (uint32_t i = 0; i < size; i++) {
-        pos = o.at(i, pos);
-        q += a.v[(size_t)a.col[beg + pos] * a.k + f] * (double)a.val[beg + pos];
-      }
-      a.q[c] = q;
+      o.init(a.col + beg, (uint32_t)(a.row_ptr[c + 1] - beg));
+      a.q[c] = row_q(o, a.v, a.k, f, a.val + beg);
     }
     grid.sync();
     sweep_runs<true>(a, grid, f, warp, nwarp, lane);
@@ -380,6 +278,52 @@ std::string repredict(fmb200_ctx* c, McmcState& s) {
   if (te.n_rows) MK(cudaMemcpyAsync(s.e_test.data(), s.e_test_d.get(), te.n_rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   MK(cudaStreamSynchronize(c->stream));
   return "";
+}
+
+// x := draw when it is finite.  Otherwise x keeps its value, counter a (NaN) or a + 1 (Inf) grows and the
+// result is true: the reference restores the old value and, in its per-group loops, stops drawing.
+bool reject_nonfinite(double& x, double draw, uint32_t* cnt, int a) {
+  if (std::isnan(draw)) { cnt[a]++; return true; }
+  if (std::isinf(draw)) { cnt[a + 1]++; return true; }
+  x = draw;
+  return false;
+}
+
+// draw_w_lambda (fm_learn_mcmc.h:980-1017) / one factor of draw_v_lambda (:1059-1097) over one column:
+// feature i's parameter is par[i * stride], group g's mean and precision mu[g * stride] and lambda[g * stride].
+// True when a draw was not finite (the reference stops there).
+bool draw_lambda(const McmcState& s, const double* par, const double* mu, double* lambda, size_t stride,
+                 uint32_t* cnt, int a) {
+  std::vector<double> gam(s.G);
+  for (uint32_t g = 0; g < s.G; g++) {
+    const double m = mu[g * stride];
+    gam[g] = kBeta0 * (m - kMu0) * (m - kMu0) + kGamma0;
+  }
+  for (size_t i = 0; i < s.group.size(); i++) {
+    const uint32_t g = s.group[i];
+    const double m = mu[g * stride];
+    gam[g] += (par[i * stride] - m) * (par[i * stride] - m);
+  }
+  for (uint32_t g = 0; g < s.G; g++) {
+    const double al = kAlpha0 + s.per_group[g] + 1;
+    if (reject_nonfinite(lambda[g * stride], s.sample ? ran_gamma(al / 2.0, gam[g] / 2.0) : al / gam[g], cnt, a))
+      return true;
+  }
+  return false;
+}
+
+// draw_w_mu (:941-978) / one factor of draw_v_mu (:1019-1057), same column layout as draw_lambda
+bool draw_mu(const McmcState& s, const double* par, double* mu, const double* lambda, size_t stride, uint32_t* cnt,
+             int a) {
+  std::vector<double> mean(s.G, 0.0);
+  for (size_t i = 0; i < s.group.size(); i++) mean[s.group[i]] += par[i * stride];
+  for (uint32_t g = 0; g < s.G; g++) {
+    mean[g] = (mean[g] + kBeta0 * kMu0) / (s.per_group[g] + kBeta0);
+    const double sig = (double)1.0 / ((s.per_group[g] + kBeta0) * lambda[g * stride]);
+    if (reject_nonfinite(mu[g * stride], s.sample ? ran_gaussian(mean[g], std::sqrt(sig)) : mean[g], cnt, a))
+      return true;
+  }
+  return false;
 }
 
 }  // namespace
@@ -515,10 +459,7 @@ std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counte
     const double alpha_n = kAlpha0 + N;
     double gamma_n = kGamma0;
     for (uint64_t i = 0; i < N; i++) gamma_n += s.e[i] * s.e[i];
-    const double old = s.alpha;
-    s.alpha = ran_gamma(alpha_n / 2.0, gamma_n / 2.0);
-    if (std::isnan(s.alpha)) { cnt[0]++; s.alpha = old; }
-    else if (std::isinf(s.alpha)) { cnt[1]++; s.alpha = old; }
+    reject_nonfinite(s.alpha, ran_gamma(alpha_n / 2.0, gamma_n / 2.0), cnt, 0);
   }
   const double alpha = s.alpha;
   // draw_w0, :643-683
@@ -530,86 +471,29 @@ std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counte
     const double sig = (double)1.0 / (s.reg0 + alpha * N);
     mean = -sig * (alpha * mean - kW0Mean0 * s.reg0);
     const double old = w0;
-    w0 = sample ? ran_gaussian(mean, std::sqrt(sig)) : mean;
-    if (std::isnan(w0)) { cnt[2]++; w0 = old; }
-    else if (std::isinf(w0)) { cnt[3]++; w0 = old; }
-    else { shift = true; e_shift = old - w0; }
+    if (!reject_nonfinite(w0, sample ? ran_gaussian(mean, std::sqrt(sig)) : mean, cnt, 2)) {
+      shift = true;
+      e_shift = old - w0;
+    }
   }
   if (c->k1) {
-    if (ml) {  // draw_w_lambda, :980-1017
-      std::vector<double> gam(G);
-      for (uint32_t g = 0; g < G; g++) gam[g] = kBeta0 * (s.w_mu[g] - kMu0) * (s.w_mu[g] - kMu0) + kGamma0;
-      for (uint32_t i = 0; i < n; i++) {
-        const uint32_t g = s.group[i];
-        gam[g] += (w[i] - s.w_mu[g]) * (w[i] - s.w_mu[g]);
-      }
-      for (uint32_t g = 0; g < G; g++) {
-        const double a = kAlpha0 + s.per_group[g] + 1;
-        const double old = s.w_lambda[g];
-        s.w_lambda[g] = sample ? ran_gamma(a / 2.0, gam[g] / 2.0) : a / gam[g];
-        if (std::isnan(s.w_lambda[g])) { cnt[10]++; s.w_lambda[g] = old; break; }
-        if (std::isinf(s.w_lambda[g])) { cnt[11]++; s.w_lambda[g] = old; break; }
-      }
-    }
-    if (!ml) {  // draw_w_mu, :941-978
-      std::fill(s.w_mu.begin(), s.w_mu.end(), kMu0);
+    if (ml) {
+      draw_lambda(s, w, s.w_mu.data(), s.w_lambda.data(), 1, cnt, 10);
+      draw_mu(s, w, s.w_mu.data(), s.w_lambda.data(), 1, cnt, 8);
     } else {
-      std::vector<double> mean(G, 0.0);
-      for (uint32_t i = 0; i < n; i++) mean[s.group[i]] += w[i];
-      for (uint32_t g = 0; g < G; g++) {
-        mean[g] = (mean[g] + kBeta0 * kMu0) / (s.per_group[g] + kBeta0);
-        const double sig = (double)1.0 / ((s.per_group[g] + kBeta0) * s.w_lambda[g]);
-        const double old = s.w_mu[g];
-        s.w_mu[g] = sample ? ran_gaussian(mean[g], std::sqrt(sig)) : mean[g];
-        if (std::isnan(s.w_mu[g])) { cnt[8]++; s.w_mu[g] = old; break; }
-        if (std::isinf(s.w_mu[g])) { cnt[9]++; s.w_mu[g] = old; break; }
-      }
+      std::fill(s.w_mu.begin(), s.w_mu.end(), kMu0);
     }
     if (sample)
       for (uint32_t j = 0; j < n; j++) s.z[j] = ran_gaussian();
   }
   if (k > 0) {
-    if (ml) {  // draw_v_lambda, :1059-1097
-      std::vector<double> gam(G);
-      bool stop = false;
-      for (int f = 0; f < k && !stop; f++) {
-        for (uint32_t g = 0; g < G; g++) {
-          const double m = s.v_mu[(size_t)g * k + f];
-          gam[g] = kBeta0 * (m - kMu0) * (m - kMu0) + kGamma0;
-        }
-        for (uint32_t i = 0; i < n; i++) {
-          const uint32_t g = s.group[i];
-          const double m = s.v_mu[(size_t)g * k + f];
-          gam[g] += (v[(size_t)i * k + f] - m) * (v[(size_t)i * k + f] - m);
-        }
-        for (uint32_t g = 0; g < G && !stop; g++) {
-          double& lam = s.v_lambda[(size_t)g * k + f];
-          const double a = kAlpha0 + s.per_group[g] + 1;
-          const double old = lam;
-          lam = sample ? ran_gamma(a / 2.0, gam[g] / 2.0) : a / gam[g];
-          if (std::isnan(lam)) { cnt[14]++; lam = old; stop = true; }
-          else if (std::isinf(lam)) { cnt[15]++; lam = old; stop = true; }
-        }
-      }
-    }
-    if (!ml) {  // draw_v_mu, :1019-1057
-      std::fill(s.v_mu.begin(), s.v_mu.end(), kMu0);
+    if (ml) {  // a non-finite draw stops the factors that follow too
+      for (int f = 0; f < k; f++)
+        if (draw_lambda(s, v + f, s.v_mu.data() + f, s.v_lambda.data() + f, k, cnt, 14)) break;
+      for (int f = 0; f < k; f++)
+        if (draw_mu(s, v + f, s.v_mu.data() + f, s.v_lambda.data() + f, k, cnt, 12)) break;
     } else {
-      std::vector<double> mean(G);
-      bool stop = false;
-      for (int f = 0; f < k && !stop; f++) {
-        std::fill(mean.begin(), mean.end(), 0.0);
-        for (uint32_t i = 0; i < n; i++) mean[s.group[i]] += v[(size_t)i * k + f];
-        for (uint32_t g = 0; g < G && !stop; g++) {
-          mean[g] = (mean[g] + kBeta0 * kMu0) / (s.per_group[g] + kBeta0);
-          double& mu = s.v_mu[(size_t)g * k + f];
-          const double sig = (double)1.0 / ((s.per_group[g] + kBeta0) * s.v_lambda[(size_t)g * k + f]);
-          const double old = mu;
-          mu = sample ? ran_gaussian(mean[g], std::sqrt(sig)) : mean[g];
-          if (std::isnan(mu)) { cnt[12]++; mu = old; stop = true; }
-          else if (std::isinf(mu)) { cnt[13]++; mu = old; stop = true; }
-        }
-      }
+      std::fill(s.v_mu.begin(), s.v_mu.end(), kMu0);
     }
     if (sample)
       for (size_t i = n; i < (size_t)(k + 1) * n; i++) s.z[i] = ran_gaussian();

@@ -9,6 +9,7 @@
 #include <cub/device/device_radix_sort.cuh>
 
 #include "fm_ordered.cuh"
+#include "fm_roworder.cuh"
 #include "fmb200_internal.h"
 
 namespace fmb {
@@ -18,17 +19,6 @@ namespace {
 __global__ void ord_iota_kernel(uint32_t* p, uint64_t n) {
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
     p[i] = (uint32_t)i;
-}
-
-// row containing entry e: the last r with row_ptr[r] <= e (empty rows skipped by construction)
-__device__ __forceinline__ uint64_t row_of(const uint64_t* __restrict__ rp, uint64_t n_rows, uint64_t e) {
-  uint64_t lo = 0, hi = n_rows;  // invariant: rp[lo] <= e < rp[hi]
-  while (hi - lo > 1) {
-    const uint64_t mid = (lo + hi) >> 1;
-    if (rp[mid] <= e) lo = mid;
-    else hi = mid;
-  }
-  return lo;
 }
 
 // `ids` / `ent`: the entries stably sorted by feature id, i.e. each feature's occurrences in

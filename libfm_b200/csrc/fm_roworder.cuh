@@ -1,6 +1,7 @@
 // fm_roworder.cuh -- a case's entries in (feature id, position) order, the order in which the
 // MCMC / ALS learner reaches them through the transposed data (reference Data.h:292-341).
-// Shared by the e-term pass (fm_inorder.cu) and the q rebuild of the Gibbs sweep (fm_mcmc.cu).
+// Shared by the e-term pass (fm_inorder.cu) and the q rebuild of the Gibbs sweep (fm_mcmc.cu), with
+// row_of, the entry -> case lookup of the index builds (fm_ordered.cu, fm_mcmc.cu).
 #pragma once
 #include <stdint.h>
 
@@ -47,6 +48,34 @@ struct RowOrder {
     }
     return best;
   }
+  // fn(pos) for every entry, in (id, position) order
+  template <class F>
+  __device__ __forceinline__ void for_each(F&& fn) const {
+    uint32_t pos = 0;
+    for (uint32_t i = 0; i < size; i++) {
+      pos = at(i, pos);
+      fn(pos);
+    }
+  }
 };
+
+// q_f of a case: 0 + sum of v[id][f] * x over its entries in (id, position) order (fm_learn_mcmc.h:172-252,
+// add_main_q :406-428); v is attribute-major [n][k], x the case's values
+__device__ __forceinline__ double row_q(const RowOrder& o, const double* v, int k, int f, const float* x) {
+  double q = 0.0;
+  o.for_each([&](uint32_t pos) { q += v[(size_t)o.c[pos] * k + f] * (double)x[pos]; });
+  return q;
+}
+
+// row containing entry e: the last r with row_ptr[r] <= e (empty rows skipped by construction)
+__device__ __forceinline__ uint64_t row_of(const uint64_t* __restrict__ rp, uint64_t n_rows, uint64_t e) {
+  uint64_t lo = 0, hi = n_rows;  // invariant: rp[lo] <= e < rp[hi]
+  while (hi - lo > 1) {
+    const uint64_t mid = (lo + hi) >> 1;
+    if (rp[mid] <= e) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
 
 }  // namespace fmb
