@@ -37,7 +37,6 @@ class CmdLine {
 
   bool has(const std::string& name) const { return values_.count(name) != 0; }
   void set(const std::string& name, const std::string& value) { values_[name] = value; }
-  void remove(const std::string& name) { values_.erase(name); }
 
   // cmdline.h:150-157
   void check() const {
