@@ -222,13 +222,17 @@ int fmb200_download_data(fmb200_ctx* ctx, int slot, uint64_t* n_rows, uint64_t* 
 int fmb200_kernel_launches(fmb200_ctx* ctx, uint64_t* count); /* kernels launched so far */
 int fmb200_last_epoch_config(fmb200_ctx* ctx, int* lanes_per_row, int* slots, int* rows_per_tile,
                              int* grid, int* block, int* smem_bytes, int* damp);
+/* 1 when the last epoch was the row-lane epoch's dealt schedule: each window's rows dealt to the CTAs
+ * sorted by the id of their last entry (bit-identical to the file-order schedule, fewer L2 requests) */
+int fmb200_last_epoch_dealt(fmb200_ctx* ctx, int* dealt);
 /* hogwild tuning knobs; 0 keeps the default.  ctas_per_sm bounds the number of
  * rows in flight (the Hogwild staleness window).  damp: 0 = automatic hot-feature
  * damping (on when the hottest feature's expected concurrency matters), 1 = force
  * on, -1 = force off (plain summed Hogwild on w/V).  variant: 0 = automatic choice
  * of the epoch kernel, 1 = sub-warp row-group kernel, 2 = one-lane-per-row kernel
  * (k <= 8, rows of <= 4 entries; ignored when not applicable), 3 = its warp-specialised
- * form (producer warp + mbarrier hand-offs; bias read three tiles ahead).
+ * form (producer warp + mbarrier hand-offs; bias read three tiles ahead), 5 = the one-lane-per-row
+ * kernel on rows in file order (no deal; see fmb200_last_epoch_dealt).
  * INORDER mode runs the wavefront schedule of the sequential epoch for k <= 8 and rows of <= 4
  * entries (conflict-free runs of examples gather and scatter in parallel, only the bias chain
  * stays serial; bit-identical to the row-at-a-time kernel, verified on the device); variant 1

@@ -65,6 +65,7 @@ SYMBOLS = {
     "fmb200_download_data": (C.c_int, [_ctx, C.c_int, _u64p, _u64p, _u64p, _u32p, _f32p, _f32p]),
     "fmb200_kernel_launches": (C.c_int, [_ctx, _u64p]),
     "fmb200_last_epoch_config": (C.c_int, [_ctx] + [_intp] * 7),
+    "fmb200_last_epoch_dealt": (C.c_int, [_ctx, _intp]),
     "fmb200_set_tuning": (C.c_int, [_ctx, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "fmb200_ordered_index": (C.c_int, [_ctx, C.c_int, _u32p, _u32p]),
 }

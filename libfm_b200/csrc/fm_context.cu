@@ -84,6 +84,7 @@ int upload_begin(fmb200_ctx* c, int slot, uint64_t n_rows, uint64_t nnz, cudaStr
   s.present = false;
   s.links_ready = false;
   s.upload_gen = ++c->upload_counter;
+  s.hogwild_epochs = 0;
   s.n_rows = n_rows;
   s.nnz = nnz;
   return 0;
@@ -130,8 +131,10 @@ int upload_onehot_enqueue(fmb200_ctx* c, int slot, uint64_t n_rows, uint32_t z, 
   return upload_inspect(c, slot, st);
 }
 
-// The one host sync of an upload: wait for the slot's event and read the verdict.
-int upload_finish(fmb200_ctx* c, int slot) {
+// The one host sync of an upload: wait for the slot's event and read the verdict.  deal: build the
+// row-lane epoch's dealt copy now (a synchronous upload: a data set loaded to be trained on; one streamed
+// in asynchronously is dealt at its second epoch, see launch_rowlane).
+int upload_finish(fmb200_ctx* c, int slot, bool deal = false) {
   DataSlot& s = c->slots[slot];
   if (!s.pending) return 0;
   CK(cudaEventSynchronize(s.ready.get()));
@@ -147,13 +150,14 @@ int upload_finish(fmb200_ctx* c, int slot) {
   for (int i = 0; i < 5; i++) s.tile_span[i] = h[2 + i];
   s.max_feat_cnt = h[9];
   s.present = true;
+  if (deal) CK(prepare_rowlane_deal(c, s));
   return 0;
 }
 
 int upload_common(fmb200_ctx* c, int slot, uint64_t n_rows, uint64_t nnz, const uint64_t* row_ptr,
                   const uint32_t* col, const float* val, const float* target) {
   if (upload_enqueue(c, slot, n_rows, nnz, row_ptr, col, val, target, c->stream)) return 1;
-  return upload_finish(c, slot);
+  return upload_finish(c, slot, true);
 }
 
 int need_slot(fmb200_ctx* c, int slot) {
@@ -418,7 +422,7 @@ int fmb200_upload_data_aos(fmb200_ctx* c, int slot, uint64_t n_rows, const void*
   CK(cudaMemcpyAsync(s.target.get(), target, n_rows * sizeof(float), cudaMemcpyHostToDevice, st));
   CK(launch_aos_split(c, st, d_ent.get(), nnz, s.col.get(), s.val.get()));
   if (upload_inspect(c, slot, st)) return 1;
-  return upload_finish(c, slot);  // syncs: the temporaries may be released
+  return upload_finish(c, slot, true);  // syncs: the temporaries may be released
 }
 
 int fmb200_upload_onehot(fmb200_ctx* c, int slot, uint64_t n_rows, uint32_t nnz_per_row,
@@ -429,7 +433,7 @@ int fmb200_upload_onehot(fmb200_ctx* c, int slot, uint64_t n_rows, uint32_t nnz_
   if (n_rows > 0xffffffffull) return fail("row count exceeds the reference's uint range");
   if (bind(c)) return 1;
   if (upload_onehot_enqueue(c, slot, n_rows, nnz_per_row, ids, target, c->stream)) return 1;
-  return upload_finish(c, slot);
+  return upload_finish(c, slot, true);
 }
 
 int fmb200_upload_onehot_async(fmb200_ctx* c, int slot, uint64_t n_rows, uint32_t nnz_per_row,
@@ -913,6 +917,12 @@ int fmb200_last_epoch_config(fmb200_ctx* c, int* lanes_per_row, int* slots, int*
   if (block) *block = c->last_cfg.block;
   if (smem_bytes) *smem_bytes = c->last_cfg.smem;
   if (damp) *damp = c->last_cfg.damp;
+  return 0;
+}
+
+int fmb200_last_epoch_dealt(fmb200_ctx* c, int* dealt) {
+  NEED_CTX(c);
+  if (dealt) *dealt = c->last_cfg.dealt;
   return 0;
 }
 

@@ -394,6 +394,9 @@ static HogwildArgs make_args(fmb200_ctx* c, const DataSlot& d, uint64_t n_tiles,
   a.gbar = nullptr;
   a.gbar_base = 0;
   a.prof = nullptr;
+  a.deal_pos = nullptr;
+  a.bias_rows = nullptr;
+  a.acc_w0x = nullptr;
   a.sched = c->d_sched.get();
   a.global_entries = 0;
   return a;
@@ -408,48 +411,99 @@ cudaError_t clear_acc_flag(fmb200_ctx* c) {
   return c->d_acc ? cudaMemsetAsync(acc_flag(c), 0, sizeof(unsigned long long), c->stream) : cudaSuccess;
 }
 
-// one-lane-per-row variant (fm_rowlane.cu) for k <= 8 and rows of at most 4 entries
-static cudaError_t launch_rowlane(fmb200_ctx* c, const DataSlot& d, bool* handled) {
-  *handled = false;
+// How the one-lane-per-row variant (fm_rowlane.cu, k <= 8, rows of at most 4 entries) runs a data set.
+// dealable: the reproducible epoch may run the dealt schedule (fm_deal.cu), whose windows are those of the
+// file-order schedule (the same grid).  It is left out where the rows of a warp decide the result (COMBINE's
+// fp32 merge of same-feature steps) and for the warp-specialised variant.  Tuning variant 5 forces the
+// file-order schedule (133: with phase timers), to compare the two on one build.
+struct RowlanePlan {
+  int threads = 0, TR = 0, launch_threads = 0, grid = 0;
+  uint32_t cap = 0, sbytes = 0, cap_dealt = 0, sbytes_dealt = 0;
+  int smem = 0, smem_dealt = 0;
+  bool damp = false, combine = false, ws = false, prof = false, dealable = false;
+  HogwildKernelFn fn = nullptr, fn_dealt = nullptr;
+};
+
+static cudaError_t plan_rowlane(fmb200_ctx* c, const DataSlot& d, RowlanePlan* p, bool* ok) {
+  *ok = false;
   const int gp = c->kp / 4;
-  if (gp < 1 || gp > 2 || d.max_row_nnz > 4 || c->tune_variant == 1) return cudaSuccess;
+  if (gp < 1 || gp > 2 || d.max_row_nnz > 4 || c->tune_variant == 1 || d.n_rows == 0) return cudaSuccess;
   int threads = c->tune_threads > 0 ? std::min(c->tune_threads, HW_MAX_THREADS) : 256;
   int tr_idx = 0;
   while ((32 << (tr_idx + 1)) <= threads) tr_idx++;
-  threads = 32 << tr_idx;  // rows_per_tile == threads: lane t owns row t of the tile
-  const int TR = threads;
-  const uint32_t cap = (d.tile_span[tr_idx] + 3u) & ~3u;
-  const uint32_t sbytes = (uint32_t)hw_stage_bytes(TR, cap);
-  const bool damp = want_damp(c, d, 3.0 * TR);
+  p->threads = 32 << tr_idx;  // rows_per_tile == threads: lane t owns row t of the tile
+  p->TR = p->threads;
+  p->cap = (d.tile_span[tr_idx] + 3u) & ~3u;
+  p->sbytes = (uint32_t)hw_stage_bytes(p->TR, p->cap);
+  p->damp = want_damp(c, d, 3.0 * p->TR);
   // in-warp merging of same-feature steps pays once a warp of 32 rows is likely to hold
   // the hottest feature more than once
-  const bool combine = (double)d.max_feat_cnt * 32.0 / (double)d.n_rows > 0.5;
+  p->combine = (double)d.max_feat_cnt * 32.0 / (double)d.n_rows > 0.5;
   // variant 3 = warp-specialised (producer warp + mbarrier hand-offs, no block barrier)
-  const bool ws = c->tune_variant == 3;
-  // variant 132 = the window kernel with phase timers, printed per window (development aid)
-  const bool want_prof = c->tune_variant == 132;
-  HogwildKernelFn fn = ws ? pick_rowlane_ws_kernel(gp, (int)d.max_row_nnz, damp, combine)
-                          : pick_rowlane_kernel(gp, (int)d.max_row_nnz, damp, combine, want_prof);
-  if (fn == nullptr) return cudaSuccess;
-  const int smem = (ws ? HW_WS_HDR_BYTES : HW_HDR_BYTES) + HW_NSTAGE * (int)sbytes;
-  const int launch_threads = ws ? threads + 32 : threads;
-  const uint64_t n_tiles = (d.n_rows + TR - 1) / TR;
-  int grid = 0;
-  cudaError_t e = fit_grid(c, fn, launch_threads, smem, n_tiles, &grid);
+  p->ws = c->tune_variant == 3;
+  // variant 132 / 133 = the window kernel with phase timers, printed per window (development aid)
+  p->prof = c->tune_variant == 132 || c->tune_variant == 133;
+  p->fn = p->ws ? pick_rowlane_ws_kernel(gp, (int)d.max_row_nnz, p->damp, p->combine)
+                : pick_rowlane_kernel(gp, (int)d.max_row_nnz, p->damp, p->combine, p->prof, false);
+  if (p->fn == nullptr) return cudaSuccess;
+  p->smem = (p->ws ? HW_WS_HDR_BYTES : HW_HDR_BYTES) + HW_NSTAGE * (int)p->sbytes;
+  p->launch_threads = p->ws ? p->threads + 32 : p->threads;
+  const uint64_t n_tiles = (d.n_rows + p->TR - 1) / p->TR;
+  cudaError_t e = fit_grid(c, p->fn, p->launch_threads, p->smem, n_tiles, &p->grid);
   if (e != cudaSuccess) return e;
-  HogwildArgs a = make_args(c, d, n_tiles, TR, cap, sbytes);
-  a.conc_scale = (float)(std::min<double>((double)d.n_rows, (double)grid * TR) / (double)d.n_rows);
-  // the warp-specialised kernel reads the bias when a stage is filled: HW_NSTAGE tiles ahead
-  a.w0_conc = (float)std::min<double>((double)d.n_rows, (double)grid * TR * (ws ? HW_NSTAGE : 1));
+  *ok = true;
+  if (p->ws || p->combine || c->tune_variant == 5 || c->tune_variant == 133) return cudaSuccess;
+  p->fn_dealt = pick_rowlane_kernel(gp, (int)d.max_row_nnz, p->damp, false, p->prof, true);
+  // a dealt tile gathers rows from all over its window: stage the longest rows' worth of entries
+  p->cap_dealt = std::max<uint32_t>(p->cap, (uint32_t)p->TR * d.max_row_nnz + 4u);
+  p->sbytes_dealt = (uint32_t)hw_stage_bytes(p->TR, p->cap_dealt);
+  p->smem_dealt = HW_HDR_BYTES + HW_NSTAGE * (int)p->sbytes_dealt;
+  int grid_dealt = 0;
+  if ((e = fit_grid(c, p->fn_dealt, p->threads, p->smem_dealt, n_tiles, &grid_dealt)) != cudaSuccess) return e;
+  p->dealable = grid_dealt == p->grid;
+  return cudaSuccess;
+}
+
+cudaError_t prepare_rowlane_deal(fmb200_ctx* c, DataSlot& d) {
+  if (c->mode != FMB200_MODE_HOGWILD || c->kp == 0) return cudaSuccess;
+  RowlanePlan p;
+  bool ok = false;
+  cudaError_t e = plan_rowlane(c, d, &p, &ok);
+  if (e != cudaSuccess || !ok || !p.dealable) return e;
+  return build_rowlane_deal(c, d, p.TR, (uint32_t)p.grid);
+}
+
+static cudaError_t launch_rowlane(fmb200_ctx* c, DataSlot& d, bool* handled) {
+  *handled = false;
+  RowlanePlan p;
+  bool ok = false;
+  cudaError_t e = plan_rowlane(c, d, &p, &ok);
+  if (e != cudaSuccess || !ok) return e;
+  const int TR = p.TR;
+  const int grid = p.grid;
+  const uint64_t n_tiles = (d.n_rows + TR - 1) / TR;
+  const bool ws = p.ws, want_prof = p.prof;
   // First epoch after the state was (re)set: the bias starts far from its equilibrium (w0 = 0 against a
   // target mean of ~3.5 on ratings) and a window of grid*TR rows would all be scored with that bias -- the
   // sequential loop corrects it within its first few hundred rows (fm_sgd.h:34-37: 1 - lr per row).  So
   // the first kRampTiles tiles run on ONE CTA (window = one tile: the bias contracts as in the sequential
   // loop), the rest on the full grid.  Costs ~40 us once; the epoch-0 RMSE gap to the oracle drops by an
-  // order of magnitude (DESIGN.md section 3.3).
+  // order of magnitude (DESIGN.md section 3.3).  That epoch runs the file-order schedule.
   constexpr uint64_t kRampTiles = 4;
   const bool ramp = c->hogwild_fresh && c->k0 && c->tune_damp >= 0 && n_tiles > 8 * kRampTiles;
   c->hogwild_fresh = false;
+  // A deal pays over repeated epochs on one data set; streaming a fresh data set in for every epoch and
+  // dealing each cost more than it saved (DESIGN.md section 3.3).  So a data set uploaded synchronously is
+  // dealt by the upload, one uploaded asynchronously from its second epoch on.
+  const bool dealt = p.dealable && !ramp && (d.deal.matches(d.upload_gen, TR, (uint32_t)grid) || d.hogwild_epochs > 0);
+  d.hogwild_epochs++;
+  HogwildKernelFn fn = dealt ? p.fn_dealt : p.fn;
+  const int smem = dealt ? p.smem_dealt : p.smem;
+  const int launch_threads = p.launch_threads;
+  HogwildArgs a = make_args(c, d, n_tiles, TR, dealt ? p.cap_dealt : p.cap, dealt ? p.sbytes_dealt : p.sbytes);
+  a.conc_scale = (float)(std::min<double>((double)d.n_rows, (double)grid * TR) / (double)d.n_rows);
+  // the warp-specialised kernel reads the bias when a stage is filled: HW_NSTAGE tiles ahead
+  a.w0_conc = (float)std::min<double>((double)d.n_rows, (double)grid * TR * (ws ? HW_NSTAGE : 1));
   if (ws) {
     if (ramp) {
       HogwildArgs r = a;
@@ -492,6 +546,23 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, const DataSlot& d, bool* handle
       a.ramp_conc_scale = (float)((double)TR / (double)d.n_rows);
       a.ramp_w0_conc = (float)TR;
     }
+    if (dealt) {
+      if ((e = build_rowlane_deal(c, d, TR, (uint32_t)grid)) != cudaSuccess) return e;
+      a.row_ptr = d.deal.row_ptr.get();
+      a.col = d.deal.col.get();
+      a.val = d.deal.val.get();
+      a.target = d.deal.target.get();
+      a.deal_pos = d.deal.pos.get();
+      // [2] bias steps (zero between launches), then a window's (mult, hjoint) pairs
+      const uint64_t words = 2 + (uint64_t)grid * TR;
+      if (c->deal_bias_cap < words) {
+        if ((e = grow(c->d_deal_bias, c->deal_bias_cap, words)) != cudaSuccess) return e;
+        if ((e = cudaMemsetAsync(c->d_deal_bias.get(), 0, 2 * sizeof(unsigned long long), c->stream)) != cudaSuccess)
+          return e;
+      }
+      a.acc_w0x = c->d_deal_bias.get();
+      a.bias_rows = reinterpret_cast<float2*>(c->d_deal_bias.get() + 2);
+    }
     a.gbar = c->d_gbar.get();
     a.gbar_base = c->gbar_count;
     if (want_prof) {
@@ -511,7 +582,7 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, const DataSlot& d, bool* handle
     c->launches++;
     // every CTA arrives once at each grid barrier of the launch (wraps modulo 2^32, as the counter does)
     const uint32_t n_win = rowlane_windows(a.n_tiles, a.ramp_tiles, (uint32_t)grid);
-    c->gbar_count += (uint32_t)grid * rowlane_barriers(a.n_tiles, a.ramp_tiles, (uint32_t)grid);
+    c->gbar_count += (uint32_t)grid * rowlane_barriers(a.n_tiles, a.ramp_tiles, (uint32_t)grid, dealt);
     if (want_prof) {
       unsigned long long h[RL_PROF_SLOTS];
       if ((e = cudaMemcpyAsync(h, a.prof, sizeof(h), cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess) return e;
@@ -524,12 +595,13 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, const DataSlot& d, bool* handle
       fprintf(stderr, "\n");
     }
   }
-  c->last_cfg = EpochConfig{1, (int)std::max<uint32_t>(1, d.max_row_nnz), TR, grid, launch_threads, smem, damp ? 1 : 0};
+  c->last_cfg = EpochConfig{1, (int)std::max<uint32_t>(1, d.max_row_nnz), TR, grid, launch_threads, smem,
+                            p.damp ? 1 : 0, dealt ? 1 : 0};
   *handled = true;
   return cudaGetLastError();
 }
 
-cudaError_t launch_sgd_hogwild(fmb200_ctx* c, const DataSlot& d) {
+cudaError_t launch_sgd_hogwild(fmb200_ctx* c, DataSlot& d) {
   if (c->kp / 4 > 32) return cudaErrorInvalidValue;  // num_factor <= 128 in this mode
   if (d.n_rows == 0) return cudaSuccess;
   {

@@ -68,6 +68,12 @@ struct HogwildArgs {
   unsigned int* gbar;
   uint32_t gbar_base;
   unsigned long long* prof;  // phase timers (development aid): RL_PROF_SLOTS clock64 sums over the CTAs, or null
+  // fm_sgd_rowlane_kernel<DEALT>: the CSR arrays above hold the dealt copy (fm_deal.cu); deal_pos[i] is
+  // dealt row i's position inside its window in file order, bias_rows [gridDim.x * tile_rows] takes every
+  // row's (mult, hjoint) at that position, and acc_w0x [2] the bias step of a window, by window parity
+  const uint32_t* deal_pos;
+  float2* bias_rows;
+  unsigned long long* acc_w0x;
 };
 
 // Windows of the row-lane epoch over n_tiles tiles: `ramp` windows of one tile, then windows of G tiles
@@ -75,9 +81,10 @@ struct HogwildArgs {
 __host__ __device__ inline uint32_t rowlane_windows(uint32_t n_tiles, uint32_t ramp, uint32_t G) {
   return ramp + (n_tiles - ramp + G - 1) / G;
 }
-// The row-lane epoch separates its windows by 2 * windows - 1 grid barriers (none behind the last fold)
-__host__ __device__ inline uint32_t rowlane_barriers(uint32_t n_tiles, uint32_t ramp, uint32_t G) {
-  return 2u * rowlane_windows(n_tiles, ramp, G) - 1u;
+// The row-lane epoch separates its windows by 2 * windows - 1 grid barriers (none behind the last fold);
+// the dealt schedule also publishes the last window's bias step by one
+__host__ __device__ inline uint32_t rowlane_barriers(uint32_t n_tiles, uint32_t ramp, uint32_t G, bool dealt) {
+  return 2u * rowlane_windows(n_tiles, ramp, G) - (dealt ? 0u : 1u);
 }
 
 // Split-phase grid barrier of a cooperative launch (every CTA resident).  Each CTA adds 1 to a counter
@@ -120,6 +127,12 @@ __device__ __forceinline__ unsigned long long acc_quantise(float d, unsigned lon
   if (fabsf(d) < kAccStepMax) return (unsigned long long)__float2ll_rn(d * kAccScale);
   atomicOr(bad, 1ull);
   return 0ull;
+}
+
+// the fold of one accumulated element into the state: NaN once a step overflowed
+__device__ __forceinline__ float acc_fold(float x, unsigned long long u, bool bad) {
+  if (bad) return __int_as_float(0x7fffffff);
+  return u != 0ull ? x + (float)((double)(long long)u * (1.0 / (double)kAccScale)) : x;
 }
 
 // stage `stage` of the ring, which follows a shared-memory header of `hdr` bytes
@@ -277,7 +290,8 @@ using HogwildKernelFn = void (*)(const HogwildArgs);
 
 // fm_rowlane.cu: kernel for (float4 chunks per row gp in {1,2}, rows of at most Z entries); a
 // cooperative launch whose grid size is the window size.  prof: the instantiation with phase timers.
-HogwildKernelFn pick_rowlane_kernel(int gp, int max_row_nnz, bool damp, bool combine, bool prof);
+// dealt: the schedule over the dealt CSR (no COMBINE, no bias ramp).
+HogwildKernelFn pick_rowlane_kernel(int gp, int max_row_nnz, bool damp, bool combine, bool prof, bool dealt);
 // its phase timers: cycles of CTA thread 0 per window, summed over the CTAs
 constexpr int RL_PROF_SLOTS = 6;  // bias+gather, score+issue, bulk wait, barrier 1, fold, barrier 2
 // warp-specialised variant: blockDim = rows_per_tile + 32, smem header HW_WS_HDR_BYTES

@@ -42,28 +42,66 @@ struct FactorRow {
 // Each lane owns two slots of s_wb and alternates them over the row's entries; a slot is rewritten only
 // once the bulk read of its previous contents is done.  The kernel waits for the writes before the
 // window's grid barrier.
-template <int GP, int Z>
-__device__ __forceinline__ void acc_add_row(unsigned long long* acc_v, uint32_t id, bool live,
-                                            const float (&d)[4 * GP], int e, int tid, unsigned long long* bad) {
+// q(f) gives the quantised element f.
+template <int GP>
+__device__ __forceinline__ unsigned long long* wb_slot(int e, int tid) {  // one array for every caller
+  __shared__ __align__(128) unsigned long long s_wb[2][HW_MAX_THREADS][4 * GP];
+  return s_wb[e & 1][tid];
+}
+template <int GP, int Z, typename Q>
+__device__ __forceinline__ void acc_add_row_q(unsigned long long* acc_v, uint32_t id, bool live, int e, int tid, Q q) {
   constexpr int K = 4 * GP;
-  __shared__ __align__(128) unsigned long long s_wb[2][HW_MAX_THREADS][K];
-  unsigned long long* slot = s_wb[e & 1][tid];
+  unsigned long long* slot = wb_slot<GP>(e, tid);
   bulk_wait_read<Z == 1 ? 0 : 1>();  // Z == 1 reuses slot 0 for every row
   if (live) {
 #pragma unroll
-    for (int f = 0; f < K; f += 2)
-      *reinterpret_cast<ulonglong2*>(slot + f) = make_ulonglong2(acc_quantise(d[f], bad), acc_quantise(d[f + 1], bad));
+    for (int f = 0; f < K; f += 2) *reinterpret_cast<ulonglong2*>(slot + f) = make_ulonglong2(q(f), q(f + 1));
     fence_proxy_async_shared();  // the generic-proxy stores above, before the bulk read of the slot
     bulk_red_add_u64(acc_v + (size_t)id * K, slot, K * 8);
   }
   bulk_commit();
+}
+template <int GP, int Z>
+__device__ __forceinline__ void acc_add_row(unsigned long long* acc_v, uint32_t id, bool live,
+                                            const float (&d)[4 * GP], int e, int tid, unsigned long long* bad) {
+  acc_add_row_q<GP, Z>(acc_v, id, live, e, tid, [&](int f) { return acc_quantise(d[f], bad); });
+}
+
+// This lane's factor row of feature gid (none: 0xffffffff, fetches nothing).  GP == 2: lane pairs fetch
+// each other's halves so that one instruction covers a whole sector per row (see the file comment).
+template <int GP>
+__device__ __forceinline__ FactorRow<GP> gather_row(const float4* V4, uint32_t gid, int odd) {
+  FactorRow<GP> r;
+  const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
+  if constexpr (GP == 2) {
+    const uint32_t pid = __shfl_xor_sync(0xffffffffu, gid, 1);
+    const uint32_t idA = odd ? pid : gid;  // row of the even lane
+    const uint32_t idB = odd ? gid : pid;  // row of the odd lane
+    const float4 la = idA != 0xffffffffu ? ld_cg_f4(V4 + (size_t)idA * 2 + odd) : zero4;
+    const float4 lb = idB != 0xffffffffu ? ld_cg_f4(V4 + (size_t)idB * 2 + odd) : zero4;
+    const float4 send = odd ? la : lb;
+    float4 recv;
+    recv.x = __shfl_xor_sync(0xffffffffu, send.x, 1);
+    recv.y = __shfl_xor_sync(0xffffffffu, send.y, 1);
+    recv.z = __shfl_xor_sync(0xffffffffu, send.z, 1);
+    recv.w = __shfl_xor_sync(0xffffffffu, send.w, 1);
+    const float4 lo = odd ? recv : la;
+    const float4 hi = odd ? lb : recv;
+    r.v[0] = lo.x; r.v[1] = lo.y; r.v[2] = lo.z; r.v[3] = lo.w;
+    r.v[4] = hi.x; r.v[5] = hi.y; r.v[6] = hi.z; r.v[7] = hi.w;
+  } else {
+    const float4 l = gid != 0xffffffffu ? ld_cg_f4(V4 + (size_t)gid) : zero4;
+    r.v[0] = l.x; r.v[1] = l.y; r.v[2] = l.z; r.v[3] = l.w;
+  }
+  return r;
 }
 
 // One tile, one lane per row: gather, score, multiplier, write-back.  `get_w0` is called
 // once the gathers are in flight and returns the tile's bias.  Returns this lane's loss
 // multiplier and joint curvature (zero for lanes without a row) for the bias step.
 // ACC: the steps go to the fixed-point accumulator (a.acc_*) instead of the state.
-template <int GP, int Z, bool DAMP, bool COMBINE, bool ACC, typename W0F>
+// DEALT (with ACC, without COMBINE): rows sharing the key entry's feature merge its gather and its steps.
+template <int GP, int Z, bool DAMP, bool COMBINE, bool ACC, bool DEALT, typename W0F>
 __device__ __forceinline__ void rowlane_tile(const HogwildArgs& a, const uint64_t* rp,
                                              const float* ys, const uint32_t* ids,
                                              const float* xs, int rows_here, int tid, W0F get_w0,
@@ -95,33 +133,41 @@ __device__ __forceinline__ void rowlane_tile(const HogwildArgs& a, const uint64_
     id[e] = on ? ids[beg + e] : 0u;
     x[e] = on ? xs[beg + e] : 0.f;
   }
+  // DEALT: the row's last entry is its key entry.  The deal sorts a window's rows by its id, so the lanes of
+  // a warp whose rows share the key form a run; `seg` is the run's first lane.  That lane alone gathers the
+  // key's parameters and hands them to the run, and it issues the run's summed steps after the scores.
+  const int kq = DEALT ? cnt - 1 : -1;  // the key entry (-1: none)
+  uint32_t kid = 0xffffffffu;
+#pragma unroll
+  for (int e = 0; e < Z; ++e)
+    if (e == kq) kid = id[e];
+  int seg = lane;
+  if (DEALT) {
+    const uint32_t prev = __shfl_up_sync(0xffffffffu, kid, 1);
+    const bool head = lane == 0 || kid == 0xffffffffu || prev != kid;
+    seg = 31 - __clz(__ballot_sync(0xffffffffu, head) & (0xffffffffu >> (31 - lane)));
+  }
 #pragma unroll
   for (int e = 0; e < Z; ++e) {
-    if (GP == 2) {
-      // a missing entry (ragged rows) fetches nothing: an unconditional gather of feature 0's sector would add
-      // L2 loads on a line the rows that really contain feature 0 are reducing into
-      const uint32_t gid = (e < cnt) ? id[e] : 0xffffffffu;
-      const uint32_t pid = __shfl_xor_sync(0xffffffffu, gid, 1);
-      const uint32_t idA = odd ? pid : gid;  // row of the even lane
-      const uint32_t idB = odd ? gid : pid;  // row of the odd lane
-      const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-      const float4 la = idA != 0xffffffffu ? ld_cg_f4(V4 + (size_t)idA * 2 + odd) : zero4;
-      const float4 lb = idB != 0xffffffffu ? ld_cg_f4(V4 + (size_t)idB * 2 + odd) : zero4;
-      const float4 send = odd ? la : lb;
-      float4 recv;
-      recv.x = __shfl_xor_sync(0xffffffffu, send.x, 1);
-      recv.y = __shfl_xor_sync(0xffffffffu, send.y, 1);
-      recv.z = __shfl_xor_sync(0xffffffffu, send.z, 1);
-      recv.w = __shfl_xor_sync(0xffffffffu, send.w, 1);
-      const float4 lo = odd ? recv : la;
-      const float4 hi = odd ? lb : recv;
-      vr[e].v[0] = lo.x; vr[e].v[1] = lo.y; vr[e].v[2] = lo.z; vr[e].v[3] = lo.w;
-      vr[e].v[4] = hi.x; vr[e].v[5] = hi.y; vr[e].v[6] = hi.z; vr[e].v[7] = hi.w;
-    } else {
-      const float4 l = (e < cnt) ? ld_cg_f4(V4 + (size_t)id[e]) : make_float4(0.f, 0.f, 0.f, 0.f);
-      vr[e].v[0] = l.x; vr[e].v[1] = l.y; vr[e].v[2] = l.z; vr[e].v[3] = l.w;
-    }
-    wv[e] = (use_w && e < cnt) ? ld_cg_f(a.w + (size_t)id[e] * a.ws) : 0.f;
+    // a missing entry (ragged rows) fetches nothing: an unconditional gather of feature 0's sector would add
+    // L2 loads on a line the rows that really contain feature 0 are reducing into
+    const bool fetch = e < cnt && e != kq;
+    vr[e] = gather_row<GP>(V4, fetch ? id[e] : 0xffffffffu, odd);
+    wv[e] = (use_w && fetch) ? ld_cg_f(a.w + (size_t)id[e] * a.ws) : 0.f;
+  }
+  if (DEALT) {
+    const bool fetch = lane == seg && kid != 0xffffffffu;
+    FactorRow<GP> kv = gather_row<GP>(V4, fetch ? kid : 0xffffffffu, odd);
+    float kw = (use_w && fetch) ? ld_cg_f(a.w + (size_t)kid * a.ws) : 0.f;
+#pragma unroll
+    for (int f = 0; f < K; ++f) kv.v[f] = __shfl_sync(0xffffffffu, kv.v[f], seg);
+    kw = __shfl_sync(0xffffffffu, kw, seg);
+#pragma unroll
+    for (int e = 0; e < Z; ++e)
+      if (e == kq) {
+        vr[e] = kv;
+        wv[e] = kw;
+      }
   }
 
   // ---- fm_model::predict in registers (fm_model.h:105-127) ----
@@ -157,6 +203,16 @@ __device__ __forceinline__ void rowlane_tile(const HogwildArgs& a, const uint64_
   const float hjoint = DAMP ? curv * ((use_w0 ? 1.f : 0.f) + hrow) : curv;
 
   // ---- fm_SGD write-back (fm_sgd.h:38-50) ----
+  struct KeyStep {
+    float v[K], w;
+  } kd{};  // DEALT: the key entry's steps
+  auto make_kd = [](const float (&d)[K], float dw) {
+    KeyStep k;
+#pragma unroll
+    for (int f = 0; f < K; ++f) k.v[f] = d[f];
+    k.w = dw;
+    return k;
+  };
   const float nlr_mult = -lr * mult;
   const float nlr_regv = -lr * a.regv;
   const float nlr_regw = -lr * a.regw;
@@ -178,6 +234,10 @@ __device__ __forceinline__ void rowlane_tile(const HogwildArgs& a, const uint64_
       d[f] = sv * (nlr_mult * (sum[f] * x[e] - vr[e].v[f] * x2) + nlr_regv * vr[e].v[f]);
     float dw = sw * (nlr_mult * x[e] + nlr_regw * wv[e]);
     bool on_c = on;  // this lane still owns a reduction for entry e
+    if (DEALT && e == kq) {  // the key entry's steps are summed over the run below
+      kd = make_kd(d, dw);
+      on_c = false;
+    }
     if (COMBINE) {
       // Skewed data: several rows of a warp hit the same feature.  Sum their steps
       // inside the warp (log-step segmented reduction over the lanes that share the
@@ -244,6 +304,29 @@ __device__ __forceinline__ void rowlane_tile(const HogwildArgs& a, const uint64_
       else red_add_f(a.w + (size_t)id[e] * a.ws, dw);
     }
   }
+  if constexpr (DEALT) {
+    // Quantise as acc_add does, then sum the run's integers (any order gives the same sums): after the
+    // segmented suffix sum, lane l holds the sum over [l, end of its run), so the run's first lane holds all
+    // of it and issues one bulk reduction and one w reduction.  Slot Z of acc_add_row_q follows the Z
+    // entries' alternation.
+    const bool has_key = kid != 0xffffffffu;
+    unsigned long long q[K + 1];
+#pragma unroll
+    for (int f = 0; f < K; ++f) q[f] = has_key ? acc_quantise(kd.v[f], a.acc_bad) : 0ull;
+    q[K] = (has_key && use_w) ? acc_quantise(kd.w, a.acc_bad) : 0ull;
+#pragma unroll
+    for (int s = 1; s < 32; s <<= 1) {
+      const bool take = __shfl_down_sync(0xffffffffu, seg, s) == seg && lane + s < 32;
+#pragma unroll
+      for (int f = 0; f <= K; ++f) {
+        const unsigned long long t = __shfl_down_sync(0xffffffffu, q[f], s);
+        if (take) q[f] += t;
+      }
+    }
+    const bool issue = has_key && lane == seg;
+    acc_add_row_q<GP, Z>(a.acc_v, kid, issue, Z, tid, [&](int f) { return q[f]; });
+    if (issue && use_w) red_add_u64(a.acc_w + (size_t)kid * a.ws, q[K]);
+  }
 
   mult_out = mult;
   hjoint_out = valid ? hjoint : 0.f;
@@ -262,7 +345,17 @@ __device__ __forceinline__ void rowlane_tile(const HogwildArgs& a, const uint64_
 // each phase of a window to a shared-memory slot; the sums go to a.prof once, at the end.
 constexpr int RL_PROF_OFF = 200;  // RL_PROF_SLOTS u64 in the spare bytes of the HW_HDR_BYTES header
 
-template <int GP, int Z, bool DAMP, bool COMBINE, bool PROF>
+//
+// DEALT: the CSR is the dealt copy (fm_deal.cu), no bias ramp.  CTA b runs chunk b of each window's rows in
+// key order; the rows' steps and the state they read are those of the file-order schedule, so only the bias
+// step needs care: it is formed per file-order tile from its rows' (mult, hjoint) in lane order, the
+// expression and summation order of the file-order schedule.  Every row stores its pair at its file-order
+// position in a.bias_rows; after barrier 1, CTA b forms the step of file-order tile b from it and reduces
+// it into a.acc_w0x[j & 1]; after barrier 2 thread 0 of every CTA folds that into its running w0, with
+// the fold's expression, so the bias each window reads is the state's bias of the file-order schedule.
+// One thread zeroes the slot again after the next window's barrier 1, and the epoch ends with one more
+// grid barrier, behind which CTA 0 writes the bias into the state.
+template <int GP, int Z, bool DAMP, bool COMBINE, bool PROF, bool DEALT>
 __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const HogwildArgs a) {
   extern __shared__ __align__(128) unsigned char smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem);
@@ -326,9 +419,13 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const
   ulonglong2* acc2 = reinterpret_cast<ulonglong2*>(a.acc);  // two u64 steps per 16-byte access
   if (PROF && tid == 0) tprof = clock64();
 
+  // DEALT, thread 0: the bias of the current window, and the previous window's bias step
+  float w0_run = (DEALT && use_w0 && tid == 0) ? ld_cg_f(a.w0) : 0.f;
+  bool bad = false;  // the accumulator's overflow flag as the latest fold saw it
   int it = 0;  // tiles this CTA has run
   for (uint32_t j = 0; j < n_win; ++j) {
     const uint32_t tile = tile_of(j);
+    if (DEALT && use_w0 && tid == 0 && j > 0) w0_run = acc_fold(w0_run, __ldcg(a.acc_w0x + ((j - 1) & 1)), bad);
     if (tile != HW_NO_TILE) {
       const int stage = it % HW_NSTAGE;
       const uint32_t parity = (uint32_t)(it / HW_NSTAGE) & 1u;
@@ -351,7 +448,12 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const
       }
       BiasFetch bias;
       bias.slot = reinterpret_cast<float*>(smem + 192);
-      bias.issue(a, use_w0, tid);
+      if (DEALT) bias.pending = w0_run;
+      else bias.issue(a, use_w0, tid);
+      // DEALT: this lane's row's position in file order, for its bias pair
+      const uint32_t pos = DEALT && tid < (int)min((uint64_t)TR, a.n_rows - (uint64_t)tile * TR)
+                               ? __ldg(a.deal_pos + (uint64_t)tile * TR + tid)
+                               : 0xffffffffu;
       mbar_wait(bars + stage, parity);
 
       unsigned char* sb = stage_base(smem, a, stage);
@@ -363,7 +465,7 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const
       const int rows_here = (int)min((uint64_t)TR, a.n_rows - row0);
 
       float mult, hj, w0 = 0.f;
-      rowlane_tile<GP, Z, DAMP, COMBINE, true>(
+      rowlane_tile<GP, Z, DAMP, COMBINE, true, DEALT>(
           w, rp, ys, ids, xs, rows_here, tid,
           [&]() {
             w0 = bias.get(use_w0, tid, it, (int)blockDim.x);
@@ -373,11 +475,15 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const
           mult, hj);
       // ---- bias: one damped reduction into the global w0 per tile ----
       float2* s_part = reinterpret_cast<float2*>(s_acc) + (it & 1) * 8;  // [2 slots][8 warps]
-      if (use_w0) bias_partial(s_part, mult, hj, tid);
+      if (DEALT) {
+        if (use_w0 && pos != 0xffffffffu) a.bias_rows[pos] = make_float2(mult, hj);
+      } else if (use_w0) {
+        bias_partial(s_part, mult, hj, tid);
+      }
       __syncthreads();
       if (tid == ptid) {
         if (nt != HW_NO_TILE) issue_tile(a, smem, bars, nt, stage, policy, nt_nb, nt_ne);
-        if (use_w0) {
+        if (!DEALT && use_w0) {
           float M = 0.f, H = 0.f;
           for (int i = 0; i < (int)(blockDim.x >> 5); i++) {
             M += s_part[i].x;
@@ -405,32 +511,64 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, 3) fm_sgd_rowlane_kernel(const
     if (q0 < n_vec) s = __ldcg(state4 + q0);
     gbar.wait(tid);
     prof_mark(3);
+    // DEALT: the pair of row tid of this CTA's file-order tile (zero without a row, as in the tile)
+    float2 pr = make_float2(0.f, 0.f);
+    if (DEALT && use_w0 && tile != HW_NO_TILE && tid < (int)min((uint64_t)TR, a.n_rows - (uint64_t)tile * TR))
+      pr = __ldcg(a.bias_rows + blockIdx.x * TR + tid);
     // ---- fold: state[i] += acc[i] (fixed point), acc[i] = 0; all NaN once a step overflowed ----
-    const bool bad = __ldcg(a.acc + a.n_acc) != 0ull;
+    bad = __ldcg(a.acc + a.n_acc) != 0ull;
     for (uint64_t q = q0; q < n_vec; q += fold_stride) {
       const ulonglong2 lo = __ldcg(acc2 + 2 * q), hi = __ldcg(acc2 + 2 * q + 1);
       if (q != q0) s = __ldcg(state4 + q);
-      auto fold = [&](float& x, unsigned long long u) {
-        if (bad) x = __int_as_float(0x7fffffff);
-        else if (u != 0ull) x = x + (float)((double)(long long)u * (1.0 / (double)kAccScale));
-      };
-      fold(s.x, lo.x);
-      fold(s.y, lo.y);
-      fold(s.z, hi.x);
-      fold(s.w, hi.y);
+      s.x = acc_fold(s.x, lo.x, bad);
+      s.y = acc_fold(s.y, lo.y, bad);
+      s.z = acc_fold(s.z, hi.x, bad);
+      s.w = acc_fold(s.w, hi.y, bad);
       // elements without a step keep their value, so a whole-vector store rewrites them unchanged; likewise
       // a pair of accumulator words is cleared whole when either holds a step
       if (bad || (lo.x | lo.y | hi.x | hi.y) != 0ull) state4[q] = s;
       if ((lo.x | lo.y) != 0ull) acc2[2 * q] = make_ulonglong2(0ull, 0ull);
       if ((hi.x | hi.y) != 0ull) acc2[2 * q + 1] = make_ulonglong2(0ull, 0ull);
     }
+    if (DEALT && use_w0) {
+      // the bias step of file-order tile b of this window, formed as the file-order schedule forms it
+      if (tile != HW_NO_TILE) {
+        float2* s_part = reinterpret_cast<float2*>(s_acc);
+        bias_partial(s_part, pr.x, pr.y, tid);
+        __syncthreads();
+        if (tid == 0) {
+          float M = 0.f, H = 0.f;
+          for (int i = 0; i < (int)(blockDim.x >> 5); i++) {
+            M += s_part[i].x;
+            H += s_part[i].y;
+          }
+          const float T = (float)min((uint64_t)TR, a.n_rows - (uint64_t)tile * TR);
+          M += T * a.reg0 * w0_run;
+          const float gsc = gamma_scale(fmaxf(a.w0_conc, 1.f), lr * (H / T + a.reg0));
+          acc_add(a.acc_w0x + (j & 1), -lr * gsc * M, a.acc_bad);
+        }
+      }
+      // every CTA has folded the previous window's step (before barrier 1): its slot is free again
+      if (blockIdx.x == 0 && tid == 0 && j > 0) a.acc_w0x[(j - 1) & 1] = 0ull;
+    }
     prof_mark(4);
-    if (j + 1 < n_win) {  // the next window reads the folded state into a zero accumulator
+    if (DEALT || j + 1 < n_win) {  // the next window reads the folded state into a zero accumulator
       gbar.arrive(tid);
       gbar.wait(tid);
     }
     fence_proxy_async_global();  // ... and its bulk reductions add to the fold's zeros
     prof_mark(5);
+  }
+  if (DEALT) {
+    // behind the last barrier: a step that overflowed after the last fold read the flag (the bias step of the
+    // last window) turns the state into NaN as the fold would have; CTA 0 writes the bias and frees its slot
+    const bool bad_end = __ldcg(a.acc + a.n_acc) != 0ull;
+    if (bad_end && !bad)
+      for (uint64_t q = q0; q < n_vec; q += fold_stride) state4[q] = make_float4(NAN, NAN, NAN, NAN);
+    if (use_w0 && blockIdx.x == 0 && tid == 0) {
+      *a.w0 = acc_fold(w0_run, __ldcg(a.acc_w0x + ((n_win - 1) & 1)), bad_end);
+      a.acc_w0x[(n_win - 1) & 1] = 0ull;
+    }
   }
   if constexpr (PROF) {
     __syncthreads();
@@ -535,7 +673,8 @@ __global__ void __launch_bounds__(HW_MAX_THREADS + 32, 3) fm_sgd_rowlane_ws_kern
     const int rows_here = (int)min((uint64_t)TR, a.n_rows - row0);
     const float w0 = s_w0[stage];
     float mult, hj;
-    rowlane_tile<GP, Z, DAMP, COMBINE, false>(a, rp, ys, ids, xs, rows_here, tid, [&]() { return w0; }, mult, hj);
+    rowlane_tile<GP, Z, DAMP, COMBINE, false, false>(a, rp, ys, ids, xs, rows_here, tid, [&]() { return w0; }, mult,
+                                                     hj);
     if (use_w0) bias_partial(s_part + stage * 8, mult, hj, tid);
     __syncwarp();
     if (lane == 0) mbar_arrive(empty + stage);  // release: partials + "done reading the stage"
@@ -543,22 +682,28 @@ __global__ void __launch_bounds__(HW_MAX_THREADS + 32, 3) fm_sgd_rowlane_ws_kern
 }
 
 template <int GP, int Z, bool PROF>
-static HogwildKernelFn pick_d(bool damp, bool combine) {
+static HogwildKernelFn pick_d(bool damp, bool combine, bool dealt) {
+  if (dealt)  // the dealt schedule never merges in fp32 (COMBINE): that merge depends on which rows share a warp
+    return combine ? nullptr
+                   : (damp ? fm_sgd_rowlane_kernel<GP, Z, true, false, PROF, true>
+                           : fm_sgd_rowlane_kernel<GP, Z, false, false, PROF, true>);
   if (combine)
-    return damp ? fm_sgd_rowlane_kernel<GP, Z, true, true, PROF> : fm_sgd_rowlane_kernel<GP, Z, false, true, PROF>;
-  return damp ? fm_sgd_rowlane_kernel<GP, Z, true, false, PROF> : fm_sgd_rowlane_kernel<GP, Z, false, false, PROF>;
+    return damp ? fm_sgd_rowlane_kernel<GP, Z, true, true, PROF, false>
+                : fm_sgd_rowlane_kernel<GP, Z, false, true, PROF, false>;
+  return damp ? fm_sgd_rowlane_kernel<GP, Z, true, false, PROF, false>
+              : fm_sgd_rowlane_kernel<GP, Z, false, false, PROF, false>;
 }
 
 template <int GP, int Z>
-static HogwildKernelFn pick_p(bool damp, bool combine, bool prof) {
-  return prof ? pick_d<GP, Z, true>(damp, combine) : pick_d<GP, Z, false>(damp, combine);
+static HogwildKernelFn pick_p(bool damp, bool combine, bool prof, bool dealt) {
+  return prof ? pick_d<GP, Z, true>(damp, combine, dealt) : pick_d<GP, Z, false>(damp, combine, dealt);
 }
 
 template <int GP>
-static HogwildKernelFn pick_z(int z, bool damp, bool combine, bool prof) {
-  if (z <= 1) return pick_p<GP, 1>(damp, combine, prof);
-  if (z <= 2) return pick_p<GP, 2>(damp, combine, prof);
-  if (z <= 4) return pick_p<GP, 4>(damp, combine, prof);
+static HogwildKernelFn pick_z(int z, bool damp, bool combine, bool prof, bool dealt) {
+  if (z <= 1) return pick_p<GP, 1>(damp, combine, prof, dealt);
+  if (z <= 2) return pick_p<GP, 2>(damp, combine, prof, dealt);
+  if (z <= 4) return pick_p<GP, 4>(damp, combine, prof, dealt);
   return nullptr;
 }
 
@@ -583,9 +728,9 @@ HogwildKernelFn pick_rowlane_ws_kernel(int gp, int max_row_nnz, bool damp, bool 
   return nullptr;
 }
 
-HogwildKernelFn pick_rowlane_kernel(int gp, int max_row_nnz, bool damp, bool combine, bool prof) {
-  if (gp == 1) return pick_z<1>(max_row_nnz, damp, combine, prof);
-  if (gp == 2) return pick_z<2>(max_row_nnz, damp, combine, prof);
+HogwildKernelFn pick_rowlane_kernel(int gp, int max_row_nnz, bool damp, bool combine, bool prof, bool dealt) {
+  if (gp == 1) return pick_z<1>(max_row_nnz, damp, combine, prof, dealt);
+  if (gp == 2) return pick_z<2>(max_row_nnz, damp, combine, prof, dealt);
   return nullptr;
 }
 

@@ -71,6 +71,22 @@ cudaError_t grow(DevPtr<T>& p, Cap& cap, uint64_t n) {
 constexpr uint64_t kRowSlack = 512 + 8;
 constexpr uint64_t kEntrySlack = 16;
 
+// The dealt copy of a data set for the row-lane epoch's dealt schedule (fm_deal.cu): the rows of every
+// window of grid x tr rows stably sorted by the id of their last entry; pos[i] = dealt row i's position
+// inside its window in file order.  Built for upload generation `gen`.
+struct RowlaneDeal {
+  DevPtr<uint64_t> row_ptr;  // [rows_cap + 1]
+  DevPtr<uint32_t> col, pos;
+  DevPtr<float> val, target;
+  uint64_t rows_cap = 0, nnz_cap = 0;
+  uint64_t gen = 0;
+  int tr = 0;
+  uint32_t grid = 0;
+  DevPtr<unsigned char> scratch;  // the sort's keys, values and temporary storage
+  size_t scratch_bytes = 0;
+  bool matches(uint64_t g, int t, uint32_t G) const { return gen == g && tr == t && grid == G; }
+};
+
 // One uploaded data set, SoA CSR in HBM.  Arrays are over-allocated so that
 // 16-byte-granular TMA bulk copies may read past the logical end.
 struct DataSlot {
@@ -102,6 +118,8 @@ struct DataSlot {
   bool links_ready = false;
   DevPtr<unsigned char> ord_scratch;  // scratch of the index build (kept for re-uploads of moderate size)
   size_t ord_scratch_bytes = 0;
+  RowlaneDeal deal;  // built by a synchronous upload, else at the second HOGWILD epoch (fm_hogwild.cu)
+  uint32_t hogwild_epochs = 0;  // HOGWILD epochs run on this upload
 };
 
 // Layout of the peer comm block (fm_peer.cu), one per context, mapped by its peers:
@@ -181,6 +199,7 @@ struct McmcDelete {
 
 struct EpochConfig {
   int lanes_per_row = 0, slots = 0, rows_per_tile = 0, grid = 0, block = 0, smem = 0, damp = 0;
+  int dealt = 0;  // the row-lane epoch ran the dealt schedule
 };
 
 }  // namespace fmb
@@ -208,6 +227,9 @@ struct fmb200_ctx {
   uint64_t pred_cap = 0;
   fmb::DevPtr<unsigned int> d_sched;   // hogwild tile scheduler: [next tile, CTAs run dry]
   fmb::DevPtr<unsigned long long> d_acc;  // fixed-point accumulator of the row-lane epoch (fm_hogwild.cu)
+  // its dealt schedule: the bias step of a window by window parity [2], then the rows' (mult, hjoint) pairs
+  fmb::DevPtr<unsigned long long> d_deal_bias;
+  uint64_t deal_bias_cap = 0;  // u64 words
   fmb::DevPtr<unsigned int> d_gbar;    // row-lane epoch: arrival counter of its grid barriers (never reset) ...
   uint32_t gbar_count = 0;             // ... and its value once every launch enqueued so far has run
   fmb::DevPtr<unsigned int> d_flag;    // 16 device words: upload-time inspection results
@@ -276,9 +298,13 @@ bool mcmc_get(const fmb200_ctx* c, double* alpha, double* w_mu, double* w_lambda
 // fm_inorder.cu: one SGDA epoch (theta-step per training row, lambda-step per validation row)
 cudaError_t launch_sgda_epoch(fmb200_ctx* c, const DataSlot& tr, const DataSlot& va, int lambda_steps);
 // fm_hogwild.cu: throughput epoch
-cudaError_t launch_sgd_hogwild(fmb200_ctx* c, const DataSlot& d);
+cudaError_t launch_sgd_hogwild(fmb200_ctx* c, DataSlot& d);
 // fm_hogwild.cu: a fresh state clears the divergence flag of the row-lane epoch's accumulator
 cudaError_t clear_acc_flag(fmb200_ctx* c);
+// fm_hogwild.cu: build the dealt copy the row-lane epoch would run on this data set, if it would deal
+cudaError_t prepare_rowlane_deal(fmb200_ctx* c, DataSlot& d);
+// fm_deal.cu: d.deal := the dealt copy of d for windows of G tiles of TR rows (kept while it matches)
+cudaError_t build_rowlane_deal(fmb200_ctx* c, DataSlot& d, int TR, uint32_t G);
 // fm_predict.cu: fp32 scores / metrics with sub-warp row groups
 cudaError_t launch_predict32(fmb200_ctx* c, const DataSlot& d, int transform, double* out_pred,
                              double* partials, int n_blocks);

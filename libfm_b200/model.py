@@ -475,3 +475,9 @@ class FmLearnSgdElement:
         self._check(self.lib.fmb200_last_epoch_config(self._ctx, *[C.byref(x) for x in v]))
         keys = ["lanes_per_row", "slots", "rows_per_tile", "grid", "block", "smem_bytes", "damp"]
         return dict(zip(keys, [x.value for x in v]))
+
+    def epoch_dealt(self) -> bool:
+        """Whether the last epoch ran the row-lane dealt schedule (rows dealt to CTAs by their last id)."""
+        v = C.c_int()
+        self._check(self.lib.fmb200_last_epoch_dealt(self._ctx, C.byref(v)))
+        return bool(v.value)

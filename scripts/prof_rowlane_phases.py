@@ -3,7 +3,8 @@
     python scripts/prof_rowlane_phases.py [c2|c2_zipf] [N] [OUT_DIR]
 
 Times N epochs by CUDA events with the default kernel (3 untimed epochs first, the first of them the
-bias-ramp epoch), then runs N epochs of the instantiation with phase timers (tuning variant 132), whose
+bias-ramp epoch), then runs N epochs of the instantiation with phase timers (tuning variant 132; 133 times
+the file-order schedule instead of the dealt one), whose
 thread 0 of every CTA adds the clock64 cycles of each phase of a window to a slot.  The library prints
 the sums of each epoch divided by windows x CTAs on stderr; this script collects those lines and writes
 OUT_DIR/phases_<workload>.txt: the mean cycles per window of each phase and the same in microseconds at
@@ -13,7 +14,7 @@ the card's maximum SM clock, beside the card's name and power limit.  The phases
   score+issue  scores, quantisation, the bulk reductions issued, bias partials, end-of-tile barrier
   bulk_wait    the bulk reductions' writes complete, proxy fence, the CTA's barrier before it arrives
   barrier1     arrival to the last CTA's arrival seen (the state loads of the fold are issued here)
-  fold         the fold of this thread's slice
+  fold         the fold of this thread's slice (dealt schedule: and the bias step of the file-order tile)
   barrier2     the grid barrier that publishes the fold
 """
 import os
