@@ -183,11 +183,13 @@ int fmb200_sgda_get_reg(fmb200_ctx* ctx, double* reg_w, double* reg_v);
 
 /* Multi-GPU plumbing (row sharding + one all-reduce of w0|w|V per epoch; the
  * reference has no equivalent).  The HOGWILD state is one packed fp32 device
- * buffer [w0, pad x3 | w (strided) | V[n][kp]]; the caller all-reduces it
+ * buffer [w0, pad | w (strided), pad | V[n][kp]], the pads zero; the caller all-reduces it
  * (NCCL) and calls fmb200_scale_params(1/G).  Both run on fmb200_stream(). */
 int fmb200_params_device(fmb200_ctx* ctx, void** device_ptr, uint64_t* n_floats);
 int fmb200_scale_params(fmb200_ctx* ctx, double factor);
-/* geometry of the packed fp32 state: w0 at [0], w[i] at [off_w + i*ws], V[i][f] at [off_v + i*kp + f] */
+/* geometry of the packed fp32 state: w0 at [0], w[i] at [off_w + i*ws], V[i][f] at [off_v + i*kp + f];
+ * off_w and off_v are multiples of 32 floats and the buffer is 256-byte aligned, so w and V start on
+ * 128-byte lines */
 int fmb200_params_layout(fmb200_ctx* ctx, uint64_t* off_w, int* ws, uint64_t* off_v, int* kp);
 int fmb200_stream(fmb200_ctx* ctx, void** cuda_stream);
 

@@ -207,10 +207,11 @@ static int create_resources(fmb200_ctx* c, int device, const cudaDeviceProp& pro
   CK(event_create(c->ev0, cudaEventDefault));
   CK(event_create(c->ev1, cudaEventDefault));
   c->p32.ws = (n_attr <= 131072u) ? 8 : 1;
-  const uint64_t n4 = ((uint64_t)n_attr * c->p32.ws + 3) & ~3ull;
-  c->p32.off_w = 4;
-  c->p32.off_v = 4 + n4;
-  c->p32.n_floats = 4 + n4 + (uint64_t)n_attr * c->kp;
+  // w and V start on 128-byte lines (Params32): a k = 8 factor row is then exactly one 32-byte sector
+  const uint64_t w_floats = ((uint64_t)n_attr * c->p32.ws + Params32::align - 1) & ~(Params32::align - 1);
+  c->p32.off_w = Params32::align;
+  c->p32.off_v = c->p32.off_w + w_floats;
+  c->p32.n_floats = c->p32.off_v + (uint64_t)n_attr * c->kp;
   c->p64.off_v = Params64::off_w + (((uint64_t)n_attr + 1) & ~1ull);
   c->p64.n_doubles = c->p64.off_v + (uint64_t)n_attr * num_factor + 2;
   c->comm = CommLayout(c->p32.n_floats, n_attr);

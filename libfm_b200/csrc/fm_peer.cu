@@ -209,8 +209,8 @@ __device__ __forceinline__ float4 mf_combine(const MeanFieldArgs& a, uint64_t i,
   }
   const uint64_t e0 = i * 4;
   float g[4];
-  if (e0 < a.off_w) {
-    g[0] = g0;
+  if (e0 < a.off_w) {  // the bias, then padding up to w: zero in every replica, and zero it stays
+    g[0] = e0 == 0 ? g0 : 0.f;
     g[1] = g[2] = g[3] = 0.f;
   } else if (e0 < a.off_v) {
 #pragma unroll

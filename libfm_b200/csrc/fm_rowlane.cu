@@ -12,7 +12,8 @@
 //  * lane t of a CTA owns row t of the staged tile (rows_per_tile == blockDim.x);
 //    all per-row math (fm_model::predict, reference fm_model.h:105-127; fm_SGD,
 //    fm_sgd.h:33-51) happens in that lane's registers: no shuffles for sums.
-//  * a factor row of k=8 floats is one 32-byte sector = two float4.  Letting every
+//  * a factor row of k=8 floats is one 32-byte sector = two float4 (V starts on a 128-byte
+//    line, Params32).  Letting every
 //    lane fetch its own two halves would cost two sector requests per row and
 //    instruction; instead lane PAIRS (2j, 2j+1) co-operate: instruction A fetches
 //    the row of lane 2j (even lane low half, odd lane high half), instruction B the

@@ -160,13 +160,18 @@ struct CommLayout {
   float* mean_counts(unsigned char* b) const { return partials(b, 2); }
 };
 
-// Packed fp32 state: [w0, 0, 0, 0 | w[n*ws] padded to a multiple of 4 | V[n][kp]].
+// Packed fp32 state: [w0, 0 ... | w[n*ws], 0 ... | V[n][kp]].  base is 256-byte aligned and w and V start
+// on multiples of `align` floats (one 128-byte line), so a factor row of kp = 8 floats is one 32-byte
+// sector and a longer row touches no sector or line it does not fill; the same holds for the records of the
+// row-lane epoch's accumulator, which mirrors the state element for element.  The padding words are zero
+// and stay zero: the kernels that walk the whole state (fold, scale, peer exchange) rely on it.
 // ws = stride of the linear weights in floats: 8 (one w per 32-byte sector) for small
 // tables, whose few lines otherwise serialise at L2 under load+reduction traffic, else 1.
 struct Params32 {
+  static constexpr uint64_t align = 32;  // floats
   float* base = nullptr;
   uint64_t n_floats = 0;
-  uint64_t off_w = 4;
+  uint64_t off_w = align;
   uint64_t off_v = 0;
   int ws = 1;
   __host__ __device__ float* w0() const { return base; }

@@ -1,5 +1,7 @@
-// Microbenchmark: cost model of fire-and-forget fp32 reductions (REDG), and of three write-back forms
-// of 64-byte records of 64-bit integers (REDG.E.ADD.64 scattered or sector-coalesced, UBLKRED).
+// Microbenchmark: cost model of fire-and-forget fp32 reductions (REDG), and of the write-back forms of a
+// k=8 fixed-point record: 64 bytes of 64-bit integers (REDG.E.ADD.64 scattered or sector-coalesced, UBLKRED,
+// on or off a 64-byte boundary) or 32 bytes of 32-bit integers (UBLKRED), and of a paired 32-byte row
+// gather on or off a sector boundary.
 // Each warp issues NITER reduction instructions (or record write-backs) to pseudo-random rows of a table.
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o red_bench red_bench.cu
 #include <cstdio>
@@ -37,6 +39,7 @@ __device__ __forceinline__ uint32_t hash(uint32_t x) {
 // mode 5: v4, 4 lanes cover 64B (8 half-lines / instr)
 // mode 6: v2, 4 lanes share a 32B row (8 sectors)
 // mode 7: loads instead (ld.cg v4 paired, 16 sectors) for comparison
+// mode 12: mode 7 with every 32-byte row 16 bytes into a sector (each row straddles two sectors)
 template <int MODE>
 __global__ void k(float* tab, uint32_t rows32 /*number of 32B rows*/, int niter, float* sink) {
   const int lane = threadIdx.x & 31;
@@ -55,6 +58,7 @@ __global__ void k(float* tab, uint32_t rows32 /*number of 32B rows*/, int niter,
     if (MODE == 9) { uint32_t r = hash(base + lane) % rows32; acc += __ldcg(tab + r); }
     if (MODE == 10) { uint32_t r = hash(base + lane) % rows32; acc += __ldcg(tab + r); red1(tab + r, 1e-9f); }
     if (MODE == 11) { uint32_t r = hash(base + lane) % rows32; acc += __ldcg(tab + (size_t)r * 8); red1(tab + (size_t)r * 8, 1e-9f); }
+    if (MODE == 12) { uint32_t r = hash(base + (lane >> 1)) % rows32; float4 v = __ldcg(reinterpret_cast<const float4*>(tab + 4 + (size_t)r * 8 + (lane & 1) * 4)); acc += v.x + v.w; }
     if (MODE == 7) { uint32_t r = hash(base + (lane >> 1)) % rows32; float4 v = __ldcg(reinterpret_cast<const float4*>(tab + (size_t)r * 8 + (lane & 1) * 4)); acc += v.x + v.w; }
   }
   if (acc == 123.456f) *sink = acc;
@@ -67,8 +71,14 @@ __global__ void k(float* tab, uint32_t rows32 /*number of 32B rows*/, int niter,
 // mode 1: sector-coalesced: the 4 lanes of a quad cover one 32-byte sector (4 x 8 B contiguous); the
 //         same 8 instructions per 32 records, each touching 8 full sectors
 // mode 2: bulk: one cp.reduce.async.bulk .add.u64 of the lane's 64-byte record from shared memory
+// mode 3: bulk, narrow: one cp.reduce.async.bulk .add.s32 of a 32-byte record (8 x s32), one sector
+// mode 4: mode 2 with every record 32 bytes off a 64-byte boundary (every other one straddles a line)
 __device__ __forceinline__ void red_u64(unsigned long long* p, unsigned long long a) {
   asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(p), "l"(a) : "memory");
+}
+__device__ __forceinline__ void bulk_red_s32(void* g, const void* s, uint32_t bytes) {
+  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.s32 [%0], [%1], %2;" ::"l"(g),
+               "r"((uint32_t)__cvta_generic_to_shared(s)), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void bulk_red_u64(unsigned long long* g, const void* s, uint32_t bytes) {
   asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.u64 [%0], [%1], %2;" ::"l"(g),
@@ -101,13 +111,16 @@ __global__ void __launch_bounds__(256) k64(unsigned long long* tab, uint32_t rec
         for (int h = 0; h < 2; h++) red_u64(tab + (size_t)rec * 8 + h * 4 + (lane & 3), 1ull);
       }
     }
-    if (MODE == 2) {
-      bulk_red_u64(tab + (size_t)(hash(base + lane) % recs) * 8, stage + tid * 8, 64);
+    if (MODE >= 2) {
+      const size_t rec = hash(base + lane) % recs;
+      if (MODE == 2) bulk_red_u64(tab + rec * 8, stage + tid * 8, 64);
+      if (MODE == 3) bulk_red_s32(tab + rec * 4, stage + tid * 8, 32);
+      if (MODE == 4) bulk_red_u64(tab + 4 + rec * 8, stage + tid * 8, 64);
       asm volatile("cp.async.bulk.commit_group;" ::: "memory");
       if ((i & 7) == 7) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
     }
   }
-  if (MODE == 2) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+  if (MODE >= 2) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 template <int MODE>
 void run64(const char* name, unsigned long long* tab, uint32_t recs, int grid, int block, int niter) {
@@ -150,6 +163,7 @@ int main() {
     run<11>("LD+RED same word, 32B stride", tab, rows32, grid, block, niter, sink);
     run<0>("v4 paired RED (16 sectors)", tab, rows32, grid, block, niter, sink);
     run<7>("v4 paired LD (16 sectors)", tab, rows32, grid, block, niter, sink);
+    run<12>("(f) v4 paired LD, rows 16 B into a sector", tab, rows32, grid, block, niter, sink);
   }
   // 64-byte u64 records of the k=8 accumulator; 9746 = the C2 feature count
   unsigned long long* tab64 = reinterpret_cast<unsigned long long*>(tab);
@@ -158,6 +172,8 @@ int main() {
     run64<0>("u64 (a) scattered, 8 REDs/record, 32 sectors", tab64, recs, grid, block, niter);
     run64<1>("u64 (b) quad per sector, 8 REDs/record, 8 sec", tab64, recs, grid, block, niter);
     run64<2>("u64 (c) bulk reduce, 64 B/record", tab64, recs, grid, block, niter);
+    run64<3>("s32 (d) bulk reduce, 32 B/record", tab64, recs, grid, block, niter);
+    run64<4>("u64 (e) bulk reduce, 64 B at 32 mod 64", tab64, recs, grid, block, niter);
   }
   return 0;
 }
