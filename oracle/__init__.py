@@ -1,11 +1,14 @@
 """oracle -- CPU checkers for the parity tests.  TEST INFRASTRUCTURE ONLY.
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl
-reference legs may import this package.  Two checkers:
+reference legs may import this package.  Three checkers:
 
   port  oracle/libfm_oracle.so        plain-C restatement (fm_oracle.c)
   ref   oracle/_ref/libfm_ref.so      the UNMODIFIED reference headers behind a
                                       C shim (ref_harness.cpp), built in place from
                                       /root/reference by oracle/Makefile
+  rowlane_epoch_model                 fp64 numpy model of the reproducible row-lane HOGWILD
+                                      epoch's windows (rowlane_model.py)
 """
 from .binding import Port, Ref, build, have_ref  # noqa: F401
+from .rowlane_model import Budget, HParams, State, rowlane_epoch_model  # noqa: F401

@@ -5,6 +5,10 @@ that the epoch still draws the same windows: which rows share a window decides w
 different schedule would be reproducible and still compute something else.  This pins what the epoch computes
 on C2 and C2-Zipf (the bias-ramp epoch and two more) to SHA-256 digests of the parameters recorded on an H100
 (scripts/make_rowlane_digests.py), and checks that the epoch is one launch.
+
+The digests were recorded from this kernel, so they pin that its bits stay what they were, on the recorded
+geometry; that those bits are right, on any geometry, is pinned by test_rowlane_model_gpu.py, which compares
+the epoch with an fp64 model of its windows.
 """
 import json
 import os
