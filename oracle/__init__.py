@@ -9,6 +9,9 @@ reference legs may import this package.  Three checkers:
                                       /root/reference by oracle/Makefile
   rowlane_epoch_model                 fp64 numpy model of the reproducible row-lane HOGWILD
                                       epoch's windows (rowlane_model.py)
+  rowgroup_epoch_model                fp64 numpy model of the free-running row-group HOGWILD epoch on
+                                      data whose result no schedule can change (rowgroup_model.py)
 """
 from .binding import Port, Ref, build, have_ref  # noqa: F401
-from .rowlane_model import Budget, HParams, State, rowlane_epoch_model  # noqa: F401
+from .rowgroup_model import concurrency, geometry, row_scores, rowgroup_epoch_model  # noqa: F401
+from .rowlane_model import Budget, HParams, State, rowlane_epoch_model, ulp32  # noqa: F401

@@ -141,6 +141,15 @@ def loss_step(hp: HParams, p, y):
     return -y * (1.0 - sg), sg * (1.0 - sg), np.zeros(p.shape, dtype=bool)
 
 
+def row_curvature(hp: HParams, curv, xx, s2, sq, damp: bool):
+    """(hrow, hjoint) of rows whose score has per-factor sums s_f (s2 = sum_f s_f^2), sq = sum_i,f (v_if x_i)^2
+    and xx = sum_i x_i^2: hrow = |d p / d(w, V)|^2 by the one-hot identity (RowGroup::reduce), and the joint
+    curvature every block of the row contracts with (the loss curvature alone without damping)."""
+    hrow = (xx if hp.k1 else 0.0) + np.maximum((xx - 2.0) * s2 + sq, 0.0)
+    hjoint = curv * ((1.0 if hp.k0 else 0.0) + hrow) if damp else curv
+    return hrow, hjoint
+
+
 def _exact_sums(idx, q, n):
     """Per-index sums of the integers q, exact: integers add exactly in fp64 while every partial sum stays
     below 2^53, which is checked."""
@@ -190,8 +199,7 @@ def rowlane_epoch_model(state: State, data, hp: HParams, TR: int, grid: int, dam
         p = (st.w0 if hp.k0 else 0.0) + lin + 0.5 * (s2 - sq)
         mult, curv, edge = loss_step(hp, p, y)
         xx = np.bincount(er, weights=x * x, minlength=R)
-        hrow = (xx if hp.k1 else 0.0) + np.maximum((xx - 2.0) * s2 + sq, 0.0)
-        hjoint = curv * ((1.0 if hp.k0 else 0.0) + hrow) if damp else curv
+        hrow, hjoint = row_curvature(hp, curv, xx, s2, sq, damp)
         row_err = EPS_P * (1.0 + np.abs(p)) + EPS_M * np.abs(mult)
 
         # ---- per entry: concurrency, damping, steps ----
