@@ -190,6 +190,31 @@ int timed(fmb200_ctx* c, double* device_seconds, F&& body) {
 
 }  // namespace
 
+constexpr int kMaxPhaseSlots = 16;
+
+cudaError_t PhaseTimers::start(int n_slots, cudaStream_t st) {
+  if (n_slots > kMaxPhaseSlots) return cudaErrorInvalidValue;
+  n = n_slots;
+  const cudaError_t e = alloc(slots, (uint64_t)n);
+  return e != cudaSuccess ? e : cudaMemsetAsync(slots.get(), 0, n * sizeof(unsigned long long), st);
+}
+
+cudaError_t PhaseTimers::print(cudaStream_t st, const char* const* names, double per, int decimals, bool skip_zero,
+                               const char* head, ...) {
+  unsigned long long h[kMaxPhaseSlots];
+  cudaError_t e = cudaMemcpyAsync(h, slots.get(), n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return e;
+  va_list ap;
+  va_start(ap, head);
+  vfprintf(stderr, head, ap);
+  va_end(ap);
+  for (int i = 0; i < n; i++)
+    if (h[i] || !skip_zero) fprintf(stderr, " %s=%.*f", names[i], decimals, (double)h[i] / per);
+  fprintf(stderr, "\n");
+  return cudaSuccess;
+}
+
 // Everything of fmb200_create that can fail after the context object exists; the caller
 // destroys the partially built context on a non-zero return.
 static int create_resources(fmb200_ctx* c, int device, const cudaDeviceProp& prop, uint32_t n_attr,

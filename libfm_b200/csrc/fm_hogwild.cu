@@ -50,7 +50,6 @@
 // Algorithmic HBM traffic per example (roofline numerator, BASELINE.json):
 // 2*k*nnz*4 bytes (V rows read + written back).
 #include <algorithm>
-#include <cstdio>
 
 #include "fm_hogwild_common.cuh"
 #include "fm_rowgroup.cuh"
@@ -58,7 +57,7 @@
 namespace fmb {
 
 template <int G, int S, int R, int RW, int U, bool DAMP>
-__global__ void __launch_bounds__(HW_MAX_THREADS, (R * U <= 4 ? 3 : (R > 20 ? 1 : 2)))
+__global__ void __launch_bounds__(HW_MAX_THREADS, row_class_ctas(R, U))
     fm_sgd_hogwild_kernel(const HogwildArgs a) {
   using RG = RowGroup<G, S, R, RW>;
   constexpr int E = RG::E;
@@ -265,53 +264,21 @@ __global__ void __launch_bounds__(HW_MAX_THREADS, (R * U <= 4 ? 3 : (R > 20 ? 1 
 // ---------------------------------------------------------------------------
 using KernelFn = HogwildKernelFn;
 
-template <int G, int S, int R, int RW, int U>
+template <int G, int S, int CLS>
 KernelFn pick_damp(bool damp) {
-  return damp ? fm_sgd_hogwild_kernel<G, S, R, RW, U, true>
-              : fm_sgd_hogwild_kernel<G, S, R, RW, U, false>;
+  constexpr RowClass k = row_class(CLS, G);
+  return damp ? fm_sgd_hogwild_kernel<G, S, k.R, k.RW, k.U, true>
+              : fm_sgd_hogwild_kernel<G, S, k.R, k.RW, k.U, false>;
 }
 
-// (R factor chunks, RW weights) cached per lane, U row sets in flight:
-//   class 0: rows of <= 2*S entries           -> R=2,  RW=1, U=2
-//   class 1: medium rows (<= 8*S entries)     -> R=8,  RW=2, U=1
-//   class 2: long rows (Criteo-like, 39/row)  -> R=20, RW=2, U=1  (no re-gather up to 20*S)
 template <int G, int S>
 KernelFn pick_r(int cls, bool damp) {
   switch (cls) {
-    case -1: return pick_damp<G, S, 1, 1, 4>(damp);  // rows of <= S entries: 4 row sets in flight
-    case 0: return pick_damp<G, S, 2, 1, 2>(damp);
-    case 1: return pick_damp<G, S, 8, 2, 1>(damp);
-    case 2: return pick_damp<G, S, 20, 2, 1>(damp);
-    default:
-      // k = 128 (G = 32, S = 1): a lane walks every entry of the row; 40 cached chunks
-      // (160 registers, one CTA per SM) keep a 39-entry row entirely in registers
-      if constexpr (G == 32) return pick_damp<G, S, 40, 2, 1>(damp);
-      else return pick_damp<G, S, 20, 2, 1>(damp);
-  }
-}
-
-template <int G>
-KernelFn pick_s(int S, int R, bool damp) {
-  if constexpr (G <= 4) {
-    if (S >= 8) return pick_r<G, 8>(R, damp);
-  }
-  if constexpr (G <= 8) {
-    if (S >= 4) return pick_r<G, 4>(R, damp);
-  }
-  if constexpr (G <= 16) {
-    if (S >= 2) return pick_r<G, 2>(R, damp);
-  }
-  return pick_r<G, 1>(R, damp);
-}
-
-static KernelFn pick_kernel(int G, int S, int R, bool damp) {
-  switch (G) {
-    case 1: return pick_s<1>(S, R, damp);
-    case 2: return pick_s<2>(S, R, damp);
-    case 4: return pick_s<4>(S, R, damp);
-    case 8: return pick_s<8>(S, R, damp);
-    case 16: return pick_s<16>(S, R, damp);
-    default: return pick_s<32>(S, R, damp);
+    case -1: return pick_damp<G, S, -1>(damp);
+    case 0: return pick_damp<G, S, 0>(damp);
+    case 1: return pick_damp<G, S, 1>(damp);
+    case 2: return pick_damp<G, S, 2>(damp);
+    default: return pick_damp<G, S, 3>(damp);
   }
 }
 
@@ -327,7 +294,7 @@ void pick_geometry(int kp, uint64_t n_rows, uint64_t nnz, int* G, int* S, int* c
   if (s < 1) s = 1;
   *G = g;
   *S = s;
-  // the register-cache class of pick_r: slot iterations of an average row
+  // the register-cache class (row_class): slot iterations of an average row
   const int iters = (int)((avg + s - 1) / s);
   *cls = iters <= 1 ? -1 : (iters <= 2 ? 0 : (iters <= 8 ? 1 : ((iters <= 20 || g < 32) ? 2 : 3)));
 }
@@ -411,6 +378,18 @@ cudaError_t clear_acc_flag(fmb200_ctx* c) {
   return c->d_acc ? cudaMemsetAsync(acc_flag(c), 0, sizeof(unsigned long long), c->stream) : cudaSuccess;
 }
 
+// A launch of the row-lane epoch: its kernel, the entries it stages per tile, the bytes of a stage, and its
+// shared memory (a header of hdr_bytes, then the ring)
+struct RowlaneShape {
+  HogwildKernelFn fn = nullptr;
+  uint32_t cap = 0, sbytes = 0;
+  int smem = 0;
+};
+static RowlaneShape rowlane_shape(HogwildKernelFn fn, int TR, uint32_t cap, int hdr_bytes) {
+  const uint32_t sbytes = (uint32_t)hw_stage_bytes(TR, cap);
+  return RowlaneShape{fn, cap, sbytes, hdr_bytes + HW_NSTAGE * (int)sbytes};
+}
+
 // How the one-lane-per-row variant (fm_rowlane.cu, k <= 8, rows of at most 4 entries) runs a data set.
 // dealable: the reproducible epoch may run the dealt schedule (fm_deal.cu), whose windows are those of the
 // file-order schedule (the same grid).  It is left out where the rows of a warp decide the result (COMBINE's
@@ -418,10 +397,8 @@ cudaError_t clear_acc_flag(fmb200_ctx* c) {
 // file-order schedule (133: with phase timers), to compare the two on one build.
 struct RowlanePlan {
   int threads = 0, TR = 0, launch_threads = 0, grid = 0;
-  uint32_t cap = 0, sbytes = 0, cap_dealt = 0, sbytes_dealt = 0;
-  int smem = 0, smem_dealt = 0;
   bool damp = false, combine = false, ws = false, prof = false, dealable = false;
-  HogwildKernelFn fn = nullptr, fn_dealt = nullptr;
+  RowlaneShape file, dealt;  // the file-order schedule; the dealt one (when dealable)
 };
 
 static cudaError_t plan_rowlane(fmb200_ctx* c, const DataSlot& d, RowlanePlan* p, bool* ok) {
@@ -433,8 +410,6 @@ static cudaError_t plan_rowlane(fmb200_ctx* c, const DataSlot& d, RowlanePlan* p
   while ((32 << (tr_idx + 1)) <= threads) tr_idx++;
   p->threads = 32 << tr_idx;  // rows_per_tile == threads: lane t owns row t of the tile
   p->TR = p->threads;
-  p->cap = (d.tile_span[tr_idx] + 3u) & ~3u;
-  p->sbytes = (uint32_t)hw_stage_bytes(p->TR, p->cap);
   p->damp = want_damp(c, d, 3.0 * p->TR);
   // in-warp merging of same-feature steps pays once a warp of 32 rows is likely to hold
   // the hottest feature more than once
@@ -443,23 +418,21 @@ static cudaError_t plan_rowlane(fmb200_ctx* c, const DataSlot& d, RowlanePlan* p
   p->ws = c->tune_variant == 3;
   // variant 132 / 133 = the window kernel with phase timers, printed per window (development aid)
   p->prof = c->tune_variant == 132 || c->tune_variant == 133;
-  p->fn = p->ws ? pick_rowlane_ws_kernel(gp, (int)d.max_row_nnz, p->damp, p->combine)
-                : pick_rowlane_kernel(gp, (int)d.max_row_nnz, p->damp, p->combine, p->prof, false);
-  if (p->fn == nullptr) return cudaSuccess;
-  p->smem = (p->ws ? HW_WS_HDR_BYTES : HW_HDR_BYTES) + HW_NSTAGE * (int)p->sbytes;
+  const uint32_t cap = (d.tile_span[tr_idx] + 3u) & ~3u;
+  p->file = rowlane_shape(pick_rowlane_kernel(gp, (int)d.max_row_nnz, p->ws, p->damp, p->combine, p->prof, false),
+                          p->TR, cap, p->ws ? HW_WS_HDR_BYTES : HW_HDR_BYTES);
+  if (p->file.fn == nullptr) return cudaSuccess;
   p->launch_threads = p->ws ? p->threads + 32 : p->threads;
   const uint64_t n_tiles = (d.n_rows + p->TR - 1) / p->TR;
-  cudaError_t e = fit_grid(c, p->fn, p->launch_threads, p->smem, n_tiles, &p->grid);
+  cudaError_t e = fit_grid(c, p->file.fn, p->launch_threads, p->file.smem, n_tiles, &p->grid);
   if (e != cudaSuccess) return e;
   *ok = true;
   if (p->ws || p->combine || c->tune_variant == 5 || c->tune_variant == 133) return cudaSuccess;
-  p->fn_dealt = pick_rowlane_kernel(gp, (int)d.max_row_nnz, p->damp, false, p->prof, true);
   // a dealt tile gathers rows from all over its window: stage the longest rows' worth of entries
-  p->cap_dealt = std::max<uint32_t>(p->cap, (uint32_t)p->TR * d.max_row_nnz + 4u);
-  p->sbytes_dealt = (uint32_t)hw_stage_bytes(p->TR, p->cap_dealt);
-  p->smem_dealt = HW_HDR_BYTES + HW_NSTAGE * (int)p->sbytes_dealt;
+  p->dealt = rowlane_shape(pick_rowlane_kernel(gp, (int)d.max_row_nnz, false, p->damp, false, p->prof, true), p->TR,
+                           std::max<uint32_t>(cap, (uint32_t)p->TR * d.max_row_nnz + 4u), HW_HDR_BYTES);
   int grid_dealt = 0;
-  if ((e = fit_grid(c, p->fn_dealt, p->threads, p->smem_dealt, n_tiles, &grid_dealt)) != cudaSuccess) return e;
+  if ((e = fit_grid(c, p->dealt.fn, p->threads, p->dealt.smem, n_tiles, &grid_dealt)) != cudaSuccess) return e;
   p->dealable = grid_dealt == p->grid;
   return cudaSuccess;
 }
@@ -482,7 +455,7 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, DataSlot& d, bool* handled) {
   const int TR = p.TR;
   const int grid = p.grid;
   const uint64_t n_tiles = (d.n_rows + TR - 1) / TR;
-  const bool ws = p.ws, want_prof = p.prof;
+  const bool ws = p.ws;
   // First epoch after the state was (re)set: the bias starts far from its equilibrium (w0 = 0 against a
   // target mean of ~3.5 on ratings) and a window of grid*TR rows would all be scored with that bias -- the
   // sequential loop corrects it within its first few hundred rows (fm_sgd.h:34-37: 1 - lr per row).  So
@@ -497,10 +470,11 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, DataSlot& d, bool* handled) {
   // dealt by the upload, one uploaded asynchronously from its second epoch on.
   const bool dealt = p.dealable && !ramp && (d.deal.matches(d.upload_gen, TR, (uint32_t)grid) || d.hogwild_epochs > 0);
   d.hogwild_epochs++;
-  HogwildKernelFn fn = dealt ? p.fn_dealt : p.fn;
-  const int smem = dealt ? p.smem_dealt : p.smem;
+  const RowlaneShape& shape = dealt ? p.dealt : p.file;
+  const HogwildKernelFn fn = shape.fn;
+  const int smem = shape.smem;
   const int launch_threads = p.launch_threads;
-  HogwildArgs a = make_args(c, d, n_tiles, TR, dealt ? p.cap_dealt : p.cap, dealt ? p.sbytes_dealt : p.sbytes);
+  HogwildArgs a = make_args(c, d, n_tiles, TR, shape.cap, shape.sbytes);
   a.conc_scale = (float)(std::min<double>((double)d.n_rows, (double)grid * TR) / (double)d.n_rows);
   // the warp-specialised kernel reads the bias when a stage is filled: HW_NSTAGE tiles ahead
   a.w0_conc = (float)std::min<double>((double)d.n_rows, (double)grid * TR * (ws ? HW_NSTAGE : 1));
@@ -565,34 +539,26 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, DataSlot& d, bool* handled) {
     }
     a.gbar = c->d_gbar.get();
     a.gbar_base = c->gbar_count;
-    if (want_prof) {
-      if ((e = cudaMalloc(&a.prof, RL_PROF_SLOTS * sizeof(unsigned long long))) != cudaSuccess) return e;
-      if ((e = cudaMemsetAsync(a.prof, 0, RL_PROF_SLOTS * sizeof(unsigned long long), c->stream)) != cudaSuccess)
-        return e;
-    }
+    PhaseTimers prof;
+    if (p.prof && (e = prof.start(RL_PROF_SLOTS, c->stream)) != cudaSuccess) return e;
+    a.prof = prof.slots.get();
     // cooperative: the grid barriers between windows need every CTA resident; a grid that cannot be
     // fails to launch instead of hanging (grid <= occ * SMs holds by construction)
     void* args[] = {&a};
     e = cudaLaunchCooperativeKernel((const void*)fn, dim3(grid), dim3(launch_threads), args, (size_t)smem,
                                     c->stream);
-    if (e != cudaSuccess) {
-      cudaFree(a.prof);
-      return e;
-    }
+    if (e != cudaSuccess) return e;
     c->launches++;
     // every CTA arrives once at each grid barrier of the launch (wraps modulo 2^32, as the counter does)
     const uint32_t n_win = rowlane_windows(a.n_tiles, a.ramp_tiles, (uint32_t)grid);
     c->gbar_count += (uint32_t)grid * rowlane_barriers(a.n_tiles, a.ramp_tiles, (uint32_t)grid, dealt);
-    if (want_prof) {
-      unsigned long long h[RL_PROF_SLOTS];
-      if ((e = cudaMemcpyAsync(h, a.prof, sizeof(h), cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess) return e;
-      if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) return e;
-      cudaFree(a.prof);
+    if (p.prof) {
       static const char* name[RL_PROF_SLOTS] = {"bias+gather", "score+issue", "bulk_wait", "barrier1", "fold",
                                                 "barrier2"};
-      fprintf(stderr, "[rowlane phases, cycles per window of CTA thread 0 (%u windows x %d CTAs)]", n_win, grid);
-      for (int i = 0; i < RL_PROF_SLOTS; i++) fprintf(stderr, " %s=%.1f", name[i], (double)h[i] / n_win / grid);
-      fprintf(stderr, "\n");
+      if ((e = prof.print(c->stream, name, (double)n_win * grid, 1, false,
+                          "[rowlane phases, cycles per window of CTA thread 0 (%u windows x %d CTAs)]", n_win,
+                          grid)) != cudaSuccess)
+        return e;
     }
   }
   c->last_cfg = EpochConfig{1, (int)std::max<uint32_t>(1, d.max_row_nnz), TR, grid, launch_threads, smem,
@@ -611,10 +577,9 @@ cudaError_t launch_sgd_hogwild(fmb200_ctx* c, DataSlot& d) {
   }
   int G, S, cls;
   pick_geometry(c->kp, d.n_rows, d.nnz, &G, &S, &cls);
-  const int R = cls < 0 ? 1 : (cls == 0 ? 2 : (cls == 1 ? 8 : (cls == 2 ? 20 : 40)));
-  const int U = cls < 0 ? 4 : (cls == 0 ? 2 : 1);
+  const RowClass rc = row_class(cls, G);
   const int threads = c->tune_threads > 0 ? std::min(c->tune_threads, HW_MAX_THREADS) : 256;
-  const int ctas_target = (R * U <= 4) ? 3 : (R > 20 ? 1 : 2);
+  const int ctas_target = row_class_ctas(rc.R, rc.U);
 
   // tile geometry: largest tile (<= 256 rows by default) whose worst-case
   // staged entry count keeps NSTAGE stages within the CTA's share of the SM's smem
@@ -639,10 +604,10 @@ cudaError_t launch_sgd_hogwild(fmb200_ctx* c, DataSlot& d) {
   const uint32_t sbytes = (uint32_t)hw_stage_bytes(TR, cap);
   const int smem = HW_HDR_BYTES + HW_NSTAGE * (int)sbytes;
 
-  const double rows_per_cta_step = (double)(threads / 32) * (32.0 / (G * S)) * U;
+  const double rows_per_cta_step = (double)(threads / 32) * (32.0 / (G * S)) * rc.U;
   const bool damp = want_damp(c, d, ctas_target * rows_per_cta_step);
 
-  KernelFn fn = pick_kernel(G, S, cls, damp);
+  const KernelFn fn = dispatch_gs(G, S, [&](auto g, auto s) { return pick_r<g, s>(cls, damp); });
   const uint64_t n_tiles = (d.n_rows + TR - 1) / TR;
   int grid = 0;
   cudaError_t e = fit_grid(c, fn, threads, smem, n_tiles, &grid);

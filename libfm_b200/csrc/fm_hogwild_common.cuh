@@ -288,13 +288,13 @@ struct TileSched {
 
 using HogwildKernelFn = void (*)(const HogwildArgs);
 
-// fm_rowlane.cu: kernel for (float4 chunks per row gp in {1,2}, rows of at most Z entries); a
-// cooperative launch whose grid size is the window size.  prof: the instantiation with phase timers.
-// dealt: the schedule over the dealt CSR (no COMBINE, no bias ramp).
-HogwildKernelFn pick_rowlane_kernel(int gp, int max_row_nnz, bool damp, bool combine, bool prof, bool dealt);
-// its phase timers: cycles of CTA thread 0 per window, summed over the CTAs
+// fm_rowlane.cu: kernel for (float4 chunks per row gp in {1,2}, rows of at most max_row_nnz <= 4
+// entries), nullptr for any other shape.  The window kernel: a cooperative launch whose grid size is
+// the window size; prof: the instantiation with phase timers; dealt: the schedule over the dealt CSR
+// (no COMBINE, no bias ramp).  ws: the warp-specialised variant instead (no phase timers, no dealt
+// schedule): blockDim = rows_per_tile + 32, smem header HW_WS_HDR_BYTES.
+HogwildKernelFn pick_rowlane_kernel(int gp, int max_row_nnz, bool ws, bool damp, bool combine, bool prof, bool dealt);
+// the window kernel's phase timers: cycles of CTA thread 0 per window, summed over the CTAs
 constexpr int RL_PROF_SLOTS = 6;  // bias+gather, score+issue, bulk wait, barrier 1, fold, barrier 2
-// warp-specialised variant: blockDim = rows_per_tile + 32, smem header HW_WS_HDR_BYTES
-HogwildKernelFn pick_rowlane_ws_kernel(int gp, int max_row_nnz, bool damp, bool combine);
 
 }  // namespace fmb

@@ -4,7 +4,6 @@
 // depends on.  Both are pure functions of col[] / row_ptr[] (bit-exact ordering work) and
 // are built once per upload, on the device, the first time an ORDERED epoch needs them.
 #include <algorithm>
-#include <cstdio>
 
 #include <cub/device/device_radix_sort.cuh>
 
@@ -250,13 +249,11 @@ cudaError_t launch_sgd_ordered(fmb200_ctx* c, DataSlot& d, bool* handled) {
   a.csr_bytes = ord_csr_bytes(TR, TE);
   a.rec_bytes = TE * (uint32_t)rs * 8u;
   a.debug = (c->tune_variant >= 100) ? c->tune_variant - 100 : 0;  // timing experiments (wrong results)
-  a.prof = nullptr;
   const bool want_prof = (a.debug & 32) != 0;  // variant 132 (+ skip bits): print the phase timers
   a.debug &= 31;
-  if (want_prof) {
-    if ((e = cudaMalloc(&a.prof, 16 * sizeof(unsigned long long))) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(a.prof, 0, 16 * sizeof(unsigned long long), c->stream)) != cudaSuccess) return e;
-  }
+  PhaseTimers prof;
+  if (want_prof && (e = prof.start(16, c->stream)) != cudaSuccess) return e;
+  a.prof = prof.slots.get();
 
   int GL = 1, KF = 1;
   ordered_shape(c->k, &GL, &KF);
@@ -281,17 +278,12 @@ cudaError_t launch_sgd_ordered(fmb200_ctx* c, DataSlot& d, bool* handled) {
   c->last_cfg = EpochConfig{GL, std::min(ORD_SMAX, ncompute / GL), TR, 1, threads, (int)smem, 0};
   *handled = true;
   if (want_prof) {
-    unsigned long long h[16];
-    if ((e = cudaMemcpyAsync(h, a.prof, sizeof(h), cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess) return e;
-    if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) return e;
-    cudaFree(a.prof);
     static const char* name[16] = {"A scores", "A barrier", "chain", "chain barrier", "check+sgd", "closing barrier",
                                    "tile prologue", "wait for helpers", "H write-back", "H csr", "H fetch issue",
                                    "H fetch landing", "H wait for compute", "-", "-", "between"};
-    fprintf(stderr, "[ordered phases, cycles per tile (%u tiles)]", a.n_tiles);
-    for (int i = 0; i < 16; i++)
-      if (h[i]) fprintf(stderr, " %s=%.0f", name[i], (double)h[i] / a.n_tiles);
-    fprintf(stderr, "\n");
+    if ((e = prof.print(c->stream, name, a.n_tiles, 0, true, "[ordered phases, cycles per tile (%u tiles)]",
+                        a.n_tiles)) != cudaSuccess)
+      return e;
   }
   return cudaGetLastError();
 }

@@ -100,29 +100,16 @@ __global__ void __launch_bounds__(256) fm_predict32_kernel(const PredictArgs a) 
 
 using PredictFn = void (*)(const PredictArgs);
 
-// the (R, RW) register-cache classes 0..2 of the training kernel: all of a row's gathers
-// are in flight before the first is consumed
+// the (R, RW) of the training kernel's register-cache classes 0..2 (row_class): all of a row's
+// gathers are in flight before the first is consumed
 template <int G, int S>
 static PredictFn pick_predict_r(int cls) {
+  constexpr RowClass c0 = row_class(0, G), c1 = row_class(1, G), c2 = row_class(2, G);
   switch (cls) {
-    case 0: return fm_predict32_kernel<G, S, 2, 1>;
-    case 1: return fm_predict32_kernel<G, S, 8, 2>;
-    default: return fm_predict32_kernel<G, S, 20, 2>;
+    case 0: return fm_predict32_kernel<G, S, c0.R, c0.RW>;
+    case 1: return fm_predict32_kernel<G, S, c1.R, c1.RW>;
+    default: return fm_predict32_kernel<G, S, c2.R, c2.RW>;
   }
-}
-
-template <int G>
-static PredictFn pick_predict_s(int S, int cls) {
-  if constexpr (G <= 4) {
-    if (S >= 8) return pick_predict_r<G, 8>(cls);
-  }
-  if constexpr (G <= 8) {
-    if (S >= 4) return pick_predict_r<G, 4>(cls);
-  }
-  if constexpr (G <= 16) {
-    if (S >= 2) return pick_predict_r<G, 2>(cls);
-  }
-  return pick_predict_r<G, 1>(cls);
 }
 
 cudaError_t launch_predict32(fmb200_ctx* c, const DataSlot& d, int transform, double* out_pred,
@@ -131,15 +118,7 @@ cudaError_t launch_predict32(fmb200_ctx* c, const DataSlot& d, int transform, do
   int G, S, cls;
   pick_geometry(c->kp, d.n_rows, d.nnz, &G, &S, &cls);
   cls = std::clamp(cls, 0, 2);  // the training kernel's classes -1 and 3 are not instantiated here
-  PredictFn fn;
-  switch (G) {
-    case 1: fn = pick_predict_s<1>(S, cls); break;
-    case 2: fn = pick_predict_s<2>(S, cls); break;
-    case 4: fn = pick_predict_s<4>(S, cls); break;
-    case 8: fn = pick_predict_s<8>(S, cls); break;
-    case 16: fn = pick_predict_s<16>(S, cls); break;
-    default: fn = pick_predict_s<32>(S, cls); break;
-  }
+  const PredictFn fn = dispatch_gs(G, S, [cls](auto g, auto s) { return pick_predict_r<g, s>(cls); });
   PredictArgs a;
   a.row_ptr = d.row_ptr.get();
   a.col = d.col.get();

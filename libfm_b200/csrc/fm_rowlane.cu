@@ -682,57 +682,32 @@ __global__ void __launch_bounds__(HW_MAX_THREADS + 32, 3) fm_sgd_rowlane_ws_kern
   }
 }
 
-template <int GP, int Z, bool PROF>
-static HogwildKernelFn pick_d(bool damp, bool combine, bool dealt) {
-  if (dealt)  // the dealt schedule never merges in fp32 (COMBINE): that merge depends on which rows share a warp
-    return combine ? nullptr
-                   : (damp ? fm_sgd_rowlane_kernel<GP, Z, true, false, PROF, true>
-                           : fm_sgd_rowlane_kernel<GP, Z, false, false, PROF, true>);
-  if (combine)
-    return damp ? fm_sgd_rowlane_kernel<GP, Z, true, true, PROF, false>
-                : fm_sgd_rowlane_kernel<GP, Z, false, true, PROF, false>;
-  return damp ? fm_sgd_rowlane_kernel<GP, Z, true, false, PROF, false>
-              : fm_sgd_rowlane_kernel<GP, Z, false, false, PROF, false>;
+// f(std::integral_constant<decltype(V), V>{}) for the V of Vs equal to v; nullptr if there is none
+template <auto... Vs, class T, class F>
+static HogwildKernelFn dispatch(T v, F f) {
+  HogwildKernelFn fn = nullptr;
+  (void)((v == Vs && (fn = f(std::integral_constant<decltype(Vs), Vs>{}), true)) || ...);
+  return fn;
 }
 
-template <int GP, int Z>
-static HogwildKernelFn pick_p(bool damp, bool combine, bool prof, bool dealt) {
-  return prof ? pick_d<GP, Z, true>(damp, combine, dealt) : pick_d<GP, Z, false>(damp, combine, dealt);
-}
-
-template <int GP>
-static HogwildKernelFn pick_z(int z, bool damp, bool combine, bool prof, bool dealt) {
-  if (z <= 1) return pick_p<GP, 1>(damp, combine, prof, dealt);
-  if (z <= 2) return pick_p<GP, 2>(damp, combine, prof, dealt);
-  if (z <= 4) return pick_p<GP, 4>(damp, combine, prof, dealt);
-  return nullptr;
-}
-
-template <int GP, int Z>
-static HogwildKernelFn pick_d_ws(bool damp, bool combine) {
-  if (combine)
-    return damp ? fm_sgd_rowlane_ws_kernel<GP, Z, true, true> : fm_sgd_rowlane_ws_kernel<GP, Z, false, true>;
-  return damp ? fm_sgd_rowlane_ws_kernel<GP, Z, true, false> : fm_sgd_rowlane_ws_kernel<GP, Z, false, false>;
-}
-
-template <int GP>
-static HogwildKernelFn pick_z_ws(int z, bool damp, bool combine) {
-  if (z <= 1) return pick_d_ws<GP, 1>(damp, combine);
-  if (z <= 2) return pick_d_ws<GP, 2>(damp, combine);
-  if (z <= 4) return pick_d_ws<GP, 4>(damp, combine);
-  return nullptr;
-}
-
-HogwildKernelFn pick_rowlane_ws_kernel(int gp, int max_row_nnz, bool damp, bool combine) {
-  if (gp == 1) return pick_z_ws<1>(max_row_nnz, damp, combine);
-  if (gp == 2) return pick_z_ws<2>(max_row_nnz, damp, combine);
-  return nullptr;
-}
-
-HogwildKernelFn pick_rowlane_kernel(int gp, int max_row_nnz, bool damp, bool combine, bool prof, bool dealt) {
-  if (gp == 1) return pick_z<1>(max_row_nnz, damp, combine, prof, dealt);
-  if (gp == 2) return pick_z<2>(max_row_nnz, damp, combine, prof, dealt);
-  return nullptr;
+HogwildKernelFn pick_rowlane_kernel(int gp, int max_row_nnz, bool ws, bool damp, bool combine, bool prof, bool dealt) {
+  const int z = max_row_nnz <= 1 ? 1 : (max_row_nnz <= 2 ? 2 : (max_row_nnz <= 4 ? 4 : 0));
+  return dispatch<1, 2>(gp, [&](auto GP) {
+    return dispatch<1, 2, 4>(z, [&](auto Z) {
+      return dispatch<false, true>(damp, [&](auto D) {
+        return dispatch<false, true>(combine, [&](auto C) {
+          if (ws) return fm_sgd_rowlane_ws_kernel<GP, Z, D, C>;
+          return dispatch<false, true>(prof, [&](auto P) {
+            return dispatch<false, true>(dealt, [&](auto DL) -> HogwildKernelFn {
+              // the dealt schedule never merges in fp32 (COMBINE): that merge depends on which rows share a warp
+              if constexpr (DL && C) return nullptr;
+              else return fm_sgd_rowlane_kernel<GP, Z, D, C, P, DL>;
+            });
+          });
+        });
+      });
+    });
+  });
 }
 
 }  // namespace fmb

@@ -341,7 +341,72 @@ cudaError_t launch_onehot_fill(fmb200_ctx* c, cudaStream_t st, uint64_t n_rows, 
 
 // pick the sub-warp geometry for a data set: G lanes per V row (power of two
 // covering kp/4 float4 chunks), S entry slots per row group, and the row-group
-// register-cache class (fm_hogwild.cu, pick_r: -1 .. 3 from short to long rows)
+// register-cache class (row_class: -1 .. 3 from short to long rows)
 void pick_geometry(int kp, uint64_t n_rows, uint64_t nnz, int* G, int* S, int* cls);
+
+// The register-cache classes of the row-group kernels (fm_rowgroup.cuh): R factor chunks and RW linear
+// weights cached per lane, U row sets in flight per warp.
+//   class -1: rows of <= S entries            -> R=1,  RW=1, U=4
+//   class 0: rows of <= 2*S entries           -> R=2,  RW=1, U=2
+//   class 1: medium rows (<= 8*S entries)     -> R=8,  RW=2, U=1
+//   class 2: long rows (Criteo-like, 39/row)  -> R=20, RW=2, U=1  (no re-gather up to 20*S)
+//   class 3: k = 128 (G = 32, S = 1): a lane walks every entry of the row; 40 cached chunks (160 registers,
+//            one CTA per SM) keep a 39-entry row entirely in registers.  Narrower groups stay at class 2.
+// U sets the rows a CTA has in flight, and with them the damping's concurrency.
+struct RowClass {
+  int R, RW, U;
+};
+constexpr RowClass row_class(int cls, int G) {
+  return cls < 0                 ? RowClass{1, 1, 4}
+         : cls == 0              ? RowClass{2, 1, 2}
+         : cls == 1              ? RowClass{8, 2, 1}
+         : (cls == 2 || G < 32) ? RowClass{20, 2, 1}
+                                 : RowClass{40, 2, 1};
+}
+// CTAs per SM the training kernel of (R, U) is built for (its __launch_bounds__); the launcher sizes the
+// tiles to that share of the SM's shared memory
+constexpr int row_class_ctas(int R, int U) { return R * U <= 4 ? 3 : (R > 20 ? 1 : 2); }
+
+// f(Int<G>{}, Int<S>{}) for the (G, S) of pick_geometry as compile-time constants.  The row-group kernels
+// exist for every G of pick_geometry and every power of two S <= 8 with G * S <= 32.
+template <int V>
+using Int = std::integral_constant<int, V>;
+template <int G, class F>
+auto dispatch_s(int S, F& f) {
+  if constexpr (G <= 4) {
+    if (S >= 8) return f(Int<G>{}, Int<8>{});
+  }
+  if constexpr (G <= 8) {
+    if (S >= 4) return f(Int<G>{}, Int<4>{});
+  }
+  if constexpr (G <= 16) {
+    if (S >= 2) return f(Int<G>{}, Int<2>{});
+  }
+  return f(Int<G>{}, Int<1>{});
+}
+template <class F>
+auto dispatch_gs(int G, int S, F f) {
+  switch (G) {
+    case 1: return dispatch_s<1>(S, f);
+    case 2: return dispatch_s<2>(S, f);
+    case 4: return dispatch_s<4>(S, f);
+    case 8: return dispatch_s<8>(S, f);
+    case 16: return dispatch_s<16>(S, f);
+    default: return dispatch_s<32>(S, f);
+  }
+}
+
+// Phase timers, a development aid (fmb200_set_tuning variant 132): a kernel adds the cycles of each of its
+// phases to one slot of `slots` (null when the timers are off).  fm_context.cu.
+struct PhaseTimers {
+  DevPtr<unsigned long long> slots;
+  int n = 0;
+  // n_slots zeroed slots, on stream st
+  cudaError_t start(int n_slots, cudaStream_t st);
+  // after the stream's work: one line to stderr, the printf `head` then " name=<slot / per>" for each slot
+  // with `decimals` digits; slots that stayed zero are left out when skip_zero
+  cudaError_t print(cudaStream_t st, const char* const* names, double per, int decimals, bool skip_zero,
+                    const char* head, ...);
+};
 
 }  // namespace fmb

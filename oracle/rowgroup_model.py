@@ -52,7 +52,7 @@ __all__ = ["EPS_S", "SEQ_EXTRA", "Geometry", "geometry", "concurrency", "row_sco
 EPS_S = 2.0 ** -22  # error of an fp32 sum per term it adds in sequence, relative to the terms' magnitudes
 SEQ_EXTRA = 6       # the shuffle tree over a group's <= 32 lanes (5 levels) and the bias add
 
-# pick_r (fm_hogwild.cu): register-cache class -> (R factor chunks, RW weights cached per lane, U row sets)
+# row_class (fmb200_internal.h): register-cache class -> (R factor chunks, RW weights cached per lane, U row sets)
 CLASSES = {-1: (1, 1, 4), 0: (2, 1, 2), 1: (8, 2, 1), 2: (20, 2, 1), 3: (40, 2, 1)}
 
 
