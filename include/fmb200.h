@@ -96,6 +96,17 @@ int fmb200_upload_onehot(fmb200_ctx* ctx, int slot, uint64_t n_rows, uint32_t nn
                          const uint32_t* ids, const float* target);
 int fmb200_upload_onehot_async(fmb200_ctx* ctx, int slot, uint64_t n_rows, uint32_t nnz_per_row,
                                const uint32_t* ids, const float* target);
+/* Same, from n_rows consecutive rows of a binary .x file exactly as the file stores them (util/fmatrix.h:
+ * per row {uint size; size x {uint id; float value}}, 4 n_rows + 8 nnz bytes at `words`), with the rows'
+ * sizes row_size[n_rows] (what the caller read from the headers) and their targets.  Row offsets, the
+ * id / value split and the check that every row's header word equals its row_size run on the device; a
+ * mismatch fails the upload and names the row (0-based within the block).  The _async form behaves
+ * like fmb200_upload_data_async.  This is how the command line streams a data set larger than
+ * -cache_size through the GPU, one block at a time. */
+int fmb200_upload_xblock(fmb200_ctx* ctx, int slot, uint64_t n_rows, uint64_t nnz, const void* words,
+                         const uint32_t* row_size, const float* target);
+int fmb200_upload_xblock_async(fmb200_ctx* ctx, int slot, uint64_t n_rows, uint64_t nnz, const void* words,
+                               const uint32_t* row_size, const float* target);
 int fmb200_free_data(fmb200_ctx* ctx, int slot);
 
 /* Page-locked host memory for the arrays handed to fmb200_upload_data: uploads from it

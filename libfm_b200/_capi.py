@@ -32,6 +32,8 @@ SYMBOLS = {
     "fmb200_upload_data_aos": (C.c_int, [_ctx, C.c_int, C.c_uint64, C.c_void_p, _f32p]),
     "fmb200_upload_onehot": (C.c_int, [_ctx, C.c_int, C.c_uint64, C.c_uint32, _u32p, _f32p]),
     "fmb200_upload_onehot_async": (C.c_int, [_ctx, C.c_int, C.c_uint64, C.c_uint32, _u32p, _f32p]),
+    "fmb200_upload_xblock": (C.c_int, [_ctx, C.c_int, C.c_uint64, C.c_uint64, C.c_void_p, _u32p, _f32p]),
+    "fmb200_upload_xblock_async": (C.c_int, [_ctx, C.c_int, C.c_uint64, C.c_uint64, C.c_void_p, _u32p, _f32p]),
     "fmb200_free_data": (C.c_int, [_ctx, C.c_int]),
     "fmb200_host_alloc": (C.c_int, [C.POINTER(C.c_void_p), C.c_uint64]),
     "fmb200_host_free": (C.c_int, [C.c_void_p]),

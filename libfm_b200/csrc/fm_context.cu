@@ -81,6 +81,7 @@ int upload_begin(fmb200_ctx* c, int slot, uint64_t n_rows, uint64_t nnz, cudaStr
     s.cap_rows = n_rows;
     s.cap_nnz = nnz;
   }
+  CK(cudaMemsetAsync(s.d_flag.get(), 0, 16 * sizeof(unsigned int), st));  // the upload's verdicts start at 0
   s.present = false;
   s.links_ready = false;
   s.upload_gen = ++c->upload_counter;
@@ -93,11 +94,11 @@ int upload_begin(fmb200_ctx* c, int slot, uint64_t n_rows, uint64_t nnz, cudaStr
 // Inspection runs on the device: offsets monotone and consistent, longest row, tile
 // spans, largest column id (the reference asserts id < num_attribute per access,
 // fm_model.h:112), and the per-feature occurrence counts used by the HOGWILD damping.
-// Leaves the results in the slot's pinned flag mirror; upload_finish() collects them.
+// Leaves the results in the slot's pinned flag mirror (zeroed by upload_begin; words 0-9, and word 10
+// for .x blocks); upload_finish() collects them.
 int upload_inspect(fmb200_ctx* c, int slot, cudaStream_t st) {
   DataSlot& s = c->slots[slot];
   unsigned int* flag = s.d_flag.get();
-  CK(cudaMemsetAsync(flag, 0, 16 * sizeof(unsigned int), st));
   CK(launch_csr_inspect(c, st, s.row_ptr.get(), s.n_rows, s.nnz, flag));
   CK(launch_feature_counts(c, st, s.col.get(), s.nnz, s.feat_cnt.get(), flag + 8, flag + 9));
   CK(cudaMemcpyAsync(s.h_flag.get(), flag, 16 * sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
@@ -140,6 +141,8 @@ int upload_finish(fmb200_ctx* c, int slot, bool deal = false) {
   CK(cudaEventSynchronize(s.ready.get()));
   s.pending = false;
   const unsigned int* h = s.h_flag.get();
+  if (h[10]) return fail("row %llu of the .x block: its header word is not row_size[%llu]",
+                         (unsigned long long)(s.n_rows - h[10]), (unsigned long long)(s.n_rows - h[10]));
   if (h[0] & 1u) return fail("row_ptr[0] must be 0");
   if (h[0] & 2u) return fail("row_ptr is not monotone");
   if (h[0] & 4u) return fail("row_ptr[n_rows] != nnz");
@@ -439,7 +442,7 @@ int fmb200_upload_data_aos(fmb200_ctx* c, int slot, uint64_t n_rows, const void*
   CK(cudaMemcpyAsync(c->h_flag.get(), flag, sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(&nnz, d_rp.get() + n_rows, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  if (c->h_flag.get()[0] & 1u) return upload_aos_host_gather(c, slot, n_rows, r, target);
+  if (c->h_flag.get()[0] != 0) return upload_aos_host_gather(c, slot, n_rows, r, target);
   if (upload_begin(c, slot, n_rows, nnz, st)) return 1;
   DataSlot& s = c->slots[slot];
   CK(alloc(d_ent, nnz));
@@ -471,6 +474,48 @@ int fmb200_upload_onehot_async(fmb200_ctx* c, int slot, uint64_t n_rows, uint32_
   if (bind(c)) return 1;
   if (c->copy_stream == nullptr) CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
   return upload_onehot_enqueue(c, slot, n_rows, nnz_per_row, ids, target, c->copy_stream);
+}
+
+// n_rows rows of a .x file as it stores them (words: per row {size; size x {id, value}}): the words, the
+// sizes and the targets cross PCIe; row offsets, the header check and the id / value split run on the device.
+static int upload_xblock_enqueue(fmb200_ctx* c, int slot, uint64_t n_rows, uint64_t nnz, const void* words,
+                                 const uint32_t* row_size, const float* target, cudaStream_t st) {
+  if (upload_begin(c, slot, n_rows, nnz, st)) return 1;
+  DataSlot& s = c->slots[slot];
+  const uint64_t n_words = n_rows + 2 * nnz;
+  CK(grow(s.x_words, s.x_words_cap, n_words ? n_words : 1));
+  CK(grow(s.x_row_size, s.x_row_size_cap, n_rows ? n_rows : 1));
+  CK(grow(s.x_scan, s.x_scan_cap, aos_scan_tiles(n_rows) + 1));
+  CK(cudaMemcpyAsync(s.x_words.get(), words, n_words * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(s.x_row_size.get(), row_size, n_rows * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(s.target.get(), target, n_rows * sizeof(float), cudaMemcpyHostToDevice, st));
+  CK(launch_xblock_to_csr(c, st, s.x_words.get(), s.x_row_size.get(), n_rows, nnz, s.x_scan.get(), s.row_ptr.get(),
+                          s.col.get(), s.val.get(), s.d_flag.get() + 10));
+  return upload_inspect(c, slot, st);
+}
+
+static int xblock_args(fmb200_ctx* c, int slot, uint64_t n_rows, const void* words, const uint32_t* row_size,
+                       const float* target) {
+  if (slot < 0 || slot >= FMB200_MAX_SLOTS) return fail("slot %d out of range", slot);
+  if (n_rows && (!words || !row_size || !target)) return fail("null data pointer");
+  if (n_rows > 0xffffffffull) return fail("row count exceeds the reference's uint range");
+  return bind(c);
+}
+
+int fmb200_upload_xblock(fmb200_ctx* c, int slot, uint64_t n_rows, uint64_t nnz, const void* words,
+                         const uint32_t* row_size, const float* target) {
+  NEED_CTX(c);
+  if (xblock_args(c, slot, n_rows, words, row_size, target)) return 1;
+  if (upload_xblock_enqueue(c, slot, n_rows, nnz, words, row_size, target, c->stream)) return 1;
+  return upload_finish(c, slot, true);
+}
+
+int fmb200_upload_xblock_async(fmb200_ctx* c, int slot, uint64_t n_rows, uint64_t nnz, const void* words,
+                               const uint32_t* row_size, const float* target) {
+  NEED_CTX(c);
+  if (xblock_args(c, slot, n_rows, words, row_size, target)) return 1;
+  if (c->copy_stream == nullptr) CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
+  return upload_xblock_enqueue(c, slot, n_rows, nnz, words, row_size, target, c->copy_stream);
 }
 
 int fmb200_host_alloc(void** out, uint64_t bytes) {

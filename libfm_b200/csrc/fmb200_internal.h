@@ -118,6 +118,11 @@ struct DataSlot {
   bool links_ready = false;
   DevPtr<unsigned char> ord_scratch;  // scratch of the index build (kept for re-uploads of moderate size)
   size_t ord_scratch_bytes = 0;
+  // fmb200_upload_xblock: the block as the file stores it, the rows' sizes and the offset scan's tile sums
+  // (kept with the slot: an asynchronous upload reads them after the call returns)
+  DevPtr<unsigned int> x_words, x_row_size;
+  DevPtr<unsigned long long> x_scan;
+  uint64_t x_words_cap = 0, x_row_size_cap = 0, x_scan_cap = 0;
   RowlaneDeal deal;  // built by a synchronous upload, else at the second HOGWILD epoch (fm_hogwild.cu)
   uint32_t hogwild_epochs = 0;  // HOGWILD epochs run on this upload
 };
@@ -337,6 +342,11 @@ cudaError_t launch_aos_to_csr(fmb200_ctx* c, cudaStream_t st, const void* d_rows
                               uint64_t* row_ptr, uint32_t* col, float* val, unsigned int* flag);
 cudaError_t launch_aos_split(fmb200_ctx* c, cudaStream_t st, const void* d_entries, uint64_t nnz, uint32_t* col, float* val);
 uint64_t aos_scan_tiles(uint64_t n_rows);
+// d_words: a .x block of n_rows rows and nnz entries (n_rows + 2 nnz words); d_row_size: the rows' sizes.
+// Writes row_ptr[0..n_rows], col and val; *flag := n_rows - (first row whose header word is not its size), or 0.
+cudaError_t launch_xblock_to_csr(fmb200_ctx* c, cudaStream_t st, const unsigned int* d_words, const unsigned int* d_row_size,
+                                 uint64_t n_rows, uint64_t nnz, unsigned long long* scratch, uint64_t* row_ptr,
+                                 uint32_t* col, float* val, unsigned int* flag);
 cudaError_t launch_onehot_fill(fmb200_ctx* c, cudaStream_t st, uint64_t n_rows, uint32_t z, uint64_t* row_ptr, float* val);
 
 // pick the sub-warp geometry for a data set: G lanes per V row (power of two

@@ -56,6 +56,11 @@ class CmdLine {
     auto it = values_.find(name);
     return it == values_.end() ? dflt : atoi(it->second.c_str());
   }
+  // a 64-bit count (byte sizes past 2^31-1, which atoi cannot read)
+  long long integer64(const std::string& name, long long dflt) const {
+    auto it = values_.find(name);
+    return it == values_.end() ? dflt : strtoll(it->second.c_str(), nullptr, 10);
+  }
 
   std::vector<std::string> list(const std::string& name) const {
     std::vector<std::string> out;

@@ -194,8 +194,29 @@ class GpuLearner {
     if (rc != 0) throw std::string(fmb200_last_error());
   }
 
-  // slot 0 = the GPU's train shard (contiguous rows), slot 1 = test (GPU 0 only)
-  void attach(const SparseData& train, const SparseData& test) {
+  // slot 0 = the GPU's train shard (contiguous rows), slot 1 = test (GPU 0 only).  A data set given as
+  // blocks (one GPU, -method sgd) is not uploaded here: every pass over it streams its blocks through
+  // slots s and s + 2 (GpuSgdLearner::pass).
+  void attach(const SparseData& train, const SparseData& test, const BinaryBlocks* train_blocks = nullptr,
+              const BinaryBlocks* test_blocks = nullptr) {
+    const BinaryBlocks* blocks[2] = {train_blocks, test_blocks};
+    for (int i = 0; i < 2; i++)
+      if (blocks[i]) {
+        streamed_[i].data = blocks[i];
+        streamed_[i].reader.reset(new BlockReader(*blocks[i], pinned_alloc, pinned_free));
+      }
+    n_train_ = train_blocks ? train_blocks->num_cases() : train.num_cases();
+    n_test_ = test_blocks ? test_blocks->num_cases() : test.num_cases();
+    if (!train_blocks) attach_train(train);
+    if (!test_blocks)
+      ck(fmb200_upload_data(ctx_[0], 1, test.num_cases(), test.num_values(), test.row_ptr.data(), test.col.data(),
+                            test.val.data(), test.target.data()));
+  }
+
+  void pull_state() { ck(fmb200_get_params(ctx_[0], &fm->w0, fm->w.data(), fm->v.data())); }
+
+ protected:
+  void attach_train(const SparseData& train) {
     const uint64_t n = train.num_cases();
     for (int g = 0; g < num_gpus; g++) {
       const uint64_t lo = n * g / num_gpus, hi = n * (g + 1) / num_gpus;
@@ -205,15 +226,16 @@ class GpuLearner {
       ck(fmb200_upload_data(ctx_[g], 0, hi - lo, rp.back(), rp.data(), train.col.data() + base,
                             train.val.data() + base, train.target.data() + lo));
     }
-    ck(fmb200_upload_data(ctx_[0], 1, test.num_cases(), test.num_values(), test.row_ptr.data(),
-                          test.col.data(), test.val.data(), test.target.data()));
-    n_train_ = n;
-    n_test_ = test.num_cases();
   }
 
-  void pull_state() { ck(fmb200_get_params(ctx_[0], &fm->w0, fm->w.data(), fm->v.data())); }
+  // the reader's two block buffers: page-locked, so the block uploads are asynchronous copies
+  static void* pinned_alloc(uint64_t bytes) {
+    void* p = nullptr;
+    ck(fmb200_host_alloc(&p, bytes));
+    return p;
+  }
+  static void pinned_free(void* p) { fmb200_host_free(p); }
 
- protected:
   // fm_learn::init (fm_learn.h:73-91): the log fields every method writes
   void add_log_fields() {
     if (!log) return;
@@ -242,6 +264,13 @@ class GpuLearner {
     }
   }
 
+  // a data set read block by block (train = 0, test = 1); data == nullptr: resident in its slot
+  struct Streamed {
+    const BinaryBlocks* data = nullptr;
+    std::unique_ptr<BlockReader> reader;
+  };
+  // (its buffers are freed after ~GpuLearner has destroyed the contexts, which ends every copy from them)
+  Streamed streamed_[2];
   std::vector<fmb200_ctx*> ctx_;
   uint64_t n_train_ = 0, n_test_ = 0;
 };
@@ -291,7 +320,10 @@ class GpuSgdLearner : public GpuLearner {
   // the body of fm_learn_sgd_element::learn's epoch (fm_learn_sgd_element.h:56-67)
   double epoch() {
     const auto t0 = std::chrono::steady_clock::now();
-    for (auto c : ctx_) ck(fmb200_sgd_epoch_async(c, 0));
+    if (streamed_[0].data)
+      pass(0, [&](int slot, const BinaryBlocks::Block&) { ck(fmb200_sgd_epoch_async(ctx_[0], slot)); });
+    else
+      for (auto c : ctx_) ck(fmb200_sgd_epoch_async(c, 0));
     if (use_peer_)
       for (auto c : ctx_) ck(fmb200_allreduce_mean(c));
 #ifdef FMB200_WITH_NCCL
@@ -318,14 +350,32 @@ class GpuSgdLearner : public GpuLearner {
     const auto t0 = std::chrono::steady_clock::now();
     double sq = 0, ab = 0;
     uint64_t ok = 0;
-    const int ng = which == 0 ? num_gpus : 1;
-    for (int g = 0; g < ng; g++) {
+    auto add = [&](fmb200_ctx* ctx, int slot) {
       double a = 0, b = 0;
       uint64_t c = 0;
-      ck(fmb200_evaluate(ctx_[g], which, &a, &b, &c));
+      ck(fmb200_evaluate(ctx, slot, &a, &b, &c));
       sq += a;
       ab += b;
       ok += c;
+    };
+    if (streamed_[which].data) {
+      // The fp64 modes add the regression errors in row order (fm_learn.h:136-146): across the blocks too,
+      // so the host adds them from the clamped predictions, err = p - y exactly as fmb200_evaluate forms it.
+      const BinaryBlocks& d = *streamed_[which].data;
+      const bool in_order = mode != FMB200_MODE_HOGWILD && task == FMB200_TASK_REGRESSION;
+      std::vector<double> pred;
+      pass(which, [&](int slot, const BinaryBlocks::Block& b) {
+        if (!in_order) return add(ctx_[0], slot);
+        pred.resize(b.rows());
+        ck(fmb200_predict(ctx_[0], slot, 1, pred.data()));
+        for (uint64_t i = 0; i < b.rows(); i++) {
+          const double err = pred[i] - (double)d.target[b.row_lo + i];
+          sq += err * err;
+          ab += std::abs(err);
+        }
+      });
+    } else {
+      for (int g = 0; g < (which == 0 ? num_gpus : 1); g++) add(ctx_[g], which);
     }
     const double n = (double)(which == 0 ? n_train_ : n_test_);
     const double dt = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
@@ -370,7 +420,10 @@ class GpuSgdLearner : public GpuLearner {
   // fm_learn_sgd::predict (fm_learn_sgd.h:76-90) on the test slot
   void predict_test(std::vector<double>& out) {
     out.resize(n_test_);
-    ck(fmb200_predict(ctx_[0], 1, 1, out.data()));
+    if (streamed_[1].data)
+      pass(1, [&](int slot, const BinaryBlocks::Block& b) { ck(fmb200_predict(ctx_[0], slot, 1, out.data() + b.row_lo)); });
+    else
+      ck(fmb200_predict(ctx_[0], 1, 1, out.data()));
   }
 
   void debug() const {  // fm_learn_sgd.h:71-74 + fm_learn.h:107-111
@@ -381,6 +434,34 @@ class GpuSgdLearner : public GpuLearner {
   }
 
  private:
+  // One pass over the streamed data set `which` (0 train, 1 test) in file order: use(slot, block) once per
+  // block, in order.  Block b goes to slot which + 2 (b % 2) on the copy stream, so the copy of block b + 1
+  // runs while the work use() enqueued on block b does; use() waits for its block's upload itself (every
+  // call on a slot does).  Before block b + 1 overwrites block b - 1's slot, the work on b - 1 has run.
+  template <class F>
+  void pass(int which, F use) {
+    fmb200_ctx* const c = ctx_[0];
+    const std::vector<BinaryBlocks::Block>& blocks = streamed_[which].data->blocks;
+    BlockReader& rd = *streamed_[which].reader;
+    auto slot = [&](size_t b) { return which + 2 * (int)(b % 2); };
+    auto upload = [&](size_t b) {
+      const BlockReader::Buffer buf = rd.wait(b);
+      ck(fmb200_upload_xblock_async(c, slot(b), blocks[b].rows(), blocks[b].nnz, buf.x, buf.row_size, buf.target));
+    };
+    ck(fmb200_sync(c));  // the slots may hold blocks the previous pass still works on
+    rd.start();
+    upload(0);
+    for (size_t b = 0; b < blocks.size(); b++) {
+      if (b + 1 < blocks.size()) {
+        if (b > 0) ck(fmb200_sync(c));
+        upload(b + 1);
+      }
+      use(slot(b), blocks[b]);
+      rd.release(b);  // its upload has finished: use() waited for it
+    }
+    rd.stop();
+  }
+
 #ifdef FMB200_WITH_NCCL
   std::vector<ncclComm_t> comms_;
 #endif

@@ -111,6 +111,55 @@ def pinned_copy(arr: np.ndarray) -> np.ndarray:
     return out  # never freed explicitly: process-lifetime staging buffers
 
 
+def write_binary(data: Data, path_x: str, path_y: str) -> None:
+    """`data` as the reference's convert tool writes it: <file>.x = file_header {uint id = 2, uint float_size = 4,
+    uint64 num_values, uint num_rows, uint num_cols} + per row {uint size; size x {uint id; float value}}
+    (util/fmatrix.h:44-50), <file>.y = {uint 1, uint 4, uint n} + float[n] (util/matrix.h:364-380)."""
+    sizes = np.diff(data.row_ptr.astype(np.int64)).astype(np.uint32)
+    words = np.empty(data.num_cases + 2 * data.num_values, dtype=np.uint32)
+    head = np.arange(data.num_cases, dtype=np.int64) + 2 * data.row_ptr[:-1].astype(np.int64)
+    words[head] = sizes
+    ent = np.ones(words.size, dtype=bool)
+    ent[head] = False
+    pairs = np.empty((data.num_values, 2), dtype=np.uint32)
+    pairs[:, 0] = data.col
+    pairs[:, 1] = data.val.view(np.uint32)
+    words[ent] = pairs.reshape(-1)
+    with open(path_x, "wb") as f:
+        f.write(np.array([2, 4], np.uint32).tobytes() + np.array([data.num_values], np.uint64).tobytes()
+                + np.array([data.num_cases, data.num_feature], np.uint32).tobytes())
+        f.write(words.tobytes())
+    with open(path_y, "wb") as f:
+        f.write(np.array([1, 4, data.num_cases], np.uint32).tobytes() + data.target.astype(np.float32).tobytes())
+
+
+def read_xblocks(path_x: str, cache_size: int):
+    """The blocks the command line streams a .x file in under -cache_size: greedy in file order, each block's
+    bytes at most cache_size // 2 (so two blocks fit), at least one row per block.  Yields
+    (row_lo, row_hi, words, row_size): the block's uint32 words as the file stores them and its rows' sizes."""
+    budget = cache_size // 2
+    raw = np.fromfile(path_x, dtype=np.uint32)
+    n_rows = int(raw[4])
+    words = raw[6:]
+    sizes = np.empty(n_rows, dtype=np.uint32)
+    pos = 0
+    for r in range(n_rows):
+        sizes[r] = words[pos]
+        pos += 1 + 2 * int(sizes[r])
+    lo, pos, lo_pos, used = 0, 0, 0, 0
+    for r in range(n_rows):
+        b = 4 + 8 * int(sizes[r])
+        if b > budget:
+            raise FmError("row %d of %s takes %d bytes: -cache_size must be at least %d" % (r, path_x, b, 2 * b))
+        if used + b > budget:
+            yield lo, r, words[lo_pos:pos], sizes[lo:r]
+            lo, lo_pos, used = r, pos, 0
+        used += b
+        pos += b // 4
+    if n_rows > lo or n_rows == 0:
+        yield lo, n_rows, words[lo_pos:pos], sizes[lo:n_rows]
+
+
 class _LibcRand:
     """glibc srand()/rand(): the reference's only entropy source (random.h:172-174)."""
 
@@ -304,6 +353,20 @@ class FmLearnSgdElement:
         for key in [k for k, (s, _) in self._slots.items() if s == slot]:
             del self._slots[key]
         self._slots[id(data)] = (slot, data)
+
+    def upload_xblock(self, words: np.ndarray, row_size: np.ndarray, target: np.ndarray, slot: int,
+                      asynchronous: bool = False) -> None:
+        """fmb200_upload_xblock(_async): rows of a .x file as the file stores them (read_xblocks) into `slot`.
+        The asynchronous form needs the arrays alive until the slot is next used."""
+        words = np.ascontiguousarray(words, dtype=np.uint32)
+        row_size = np.ascontiguousarray(row_size, dtype=np.uint32)
+        target = np.ascontiguousarray(target, dtype=np.float32)
+        nnz = (words.size - row_size.size) // 2
+        fn = self.lib.fmb200_upload_xblock_async if asynchronous else self.lib.fmb200_upload_xblock
+        self._check(fn(self._ctx, slot, row_size.size, nnz, words.ctypes.data_as(C.c_void_p),
+                       _p(row_size, C.c_uint32), _p(target, C.c_float)))
+        for key in [k for k, (s, _) in self._slots.items() if s == slot]:
+            del self._slots[key]
 
     def release(self, data: Data) -> None:
         """Free the device copy of `data` and its slot."""
