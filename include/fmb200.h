@@ -173,6 +173,36 @@ int fmb200_mcmc_eterms(fmb200_ctx* ctx, int slot, double* e_out);
 int fmb200_mcmc_begin(fmb200_ctx* ctx, int train_slot, int test_slot, int do_sample, int do_multilevel,
                       uint32_t n_groups, const uint32_t* attr_group, const uint32_t* attr_per_group, double reg0,
                       const double* w_lambda, const double* v_lambda);
+/* Out-of-core form of _begin (the reference's Data with has_xt and -cache_size: LargeSparseMatrixHD over
+ * <file>.xt, Data.h:120-176).  A data set given as fmb200_xt_blocks (non-NULL) is not held on the device: every
+ * pass of every iteration (the sweeps, the q rebuilds, the e-terms) streams its .xt blocks in file order
+ * through the two slots it names, decoding each on the device like fmb200_upload_xblock; the copy of block b+1
+ * overlaps the work on block b.  A NULL blocks pointer takes that data set from its slot as _begin does; train
+ * and test decide independently.  Results are bit-identical to _begin's.  fmb200_mcmc_iteration, _get_hyper,
+ * _get_pred and _runs serve both.  _runs counts the runs the streamed sweep walks: the resident cut plus a
+ * cut at every block start (a run never spans two blocks).
+ * The .xt layout is the .x layout with rows = features and ids = cases: per column {uint size; size x
+ * {uint case; float value}}, a column's cases ascending, a case named twice by a column adjacent in entry order.
+ * Limits: fewer than 2^32 cases and fewer than 2^32 entries per block; the total entry count is not bounded. */
+typedef struct fmb200_xt_blocks {
+  uint64_t n_cases;        /* the .xt header's num_cols; equals the number of targets */
+  const float* target;     /* [n_cases], read during the call */
+  uint64_t n_blocks;       /* >= 1 */
+  const uint32_t* col_lo;  /* [n_blocks + 1]: block b holds columns (feature ids) [col_lo[b], col_lo[b+1]);
+                              col_lo[0] = 0, col_lo[n_blocks] = the .xt's num_rows <= num_attribute */
+  const uint64_t* nnz;     /* [n_blocks] entries of each block */
+  int slot[2];             /* the two slots the blocks pass through (distinct, and not the other set's slot) */
+  void* user;
+  /* Block b as the file stores it (col_lo[b+1] - col_lo[b] columns, 4 per column + 8 per entry bytes at *words)
+   * and its columns' sizes; page-locked memory makes the copy asynchronous.  The memory must stay valid until
+   * release(user, b).  Blocks are fetched in order, from 0, once per pass; non-zero fails the call. */
+  int (*fetch)(void* user, uint64_t block, const void** words, const uint32_t** col_size);
+  void (*release)(void* user, uint64_t block);
+} fmb200_xt_blocks;
+int fmb200_mcmc_begin_xt(fmb200_ctx* ctx, int train_slot, const fmb200_xt_blocks* train_xt, int test_slot,
+                         const fmb200_xt_blocks* test_xt, int do_sample, int do_multilevel, uint32_t n_groups,
+                         const uint32_t* attr_group, const uint32_t* attr_per_group, double reg0,
+                         const double* w_lambda, const double* v_lambda);
 int fmb200_mcmc_iteration(fmb200_ctx* ctx, double* train_metric, uint32_t* counters);
 int fmb200_mcmc_get_hyper(fmb200_ctx* ctx, double* alpha, double* w_mu, double* w_lambda, double* v_mu,
                           double* v_lambda);

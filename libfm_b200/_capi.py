@@ -21,6 +21,16 @@ _f64p = C.POINTER(C.c_double)
 _intp = C.POINTER(C.c_int)
 _ctx = C.c_void_p
 
+# fmb200_xt_blocks: a data set given as blocks of its .xt file (fmb200_mcmc_begin_xt)
+XT_FETCH = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_uint64, C.POINTER(C.c_void_p), C.POINTER(_u32p))
+XT_RELEASE = C.CFUNCTYPE(None, C.c_void_p, C.c_uint64)
+
+
+class XtBlocksC(C.Structure):
+    _fields_ = [("n_cases", C.c_uint64), ("target", _f32p), ("n_blocks", C.c_uint64), ("col_lo", _u32p),
+                ("nnz", _u64p), ("slot", C.c_int * 2), ("user", C.c_void_p), ("fetch", XT_FETCH),
+                ("release", XT_RELEASE)]
+
 SYMBOLS = {
     "fmb200_create": (C.c_int, [C.POINTER(_ctx), C.c_int, C.c_uint32, C.c_int, C.c_int, C.c_int]),
     "fmb200_destroy": (None, [_ctx]),
@@ -50,6 +60,8 @@ SYMBOLS = {
     "fmb200_mcmc_eterms": (C.c_int, [_ctx, C.c_int, _f64p]),
     "fmb200_mcmc_begin": (C.c_int, [_ctx, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint32, _u32p, _u32p, C.c_double,
                                     _f64p, _f64p]),
+    "fmb200_mcmc_begin_xt": (C.c_int, [_ctx, C.c_int, C.POINTER(XtBlocksC), C.c_int, C.POINTER(XtBlocksC), C.c_int,
+                                       C.c_int, C.c_uint32, _u32p, _u32p, C.c_double, _f64p, _f64p]),
     "fmb200_mcmc_iteration": (C.c_int, [_ctx, _f64p, _u32p]),
     "fmb200_mcmc_get_hyper": (C.c_int, [_ctx] + [_f64p] * 5),
     "fmb200_mcmc_get_pred": (C.c_int, [_ctx] + [_f64p] * 3),

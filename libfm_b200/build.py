@@ -2,6 +2,7 @@
 
   libfm_b200/lib/libfmb200.so   CUDA kernels + the C ABI of include/fmb200.h
   bin/libFM                     drop-in C++ command line (host/), links the above
+  bin/convert, bin/transpose    drop-ins for the reference's tools (text -> .x/.y, .x -> .xt)
 
 Build products are git-ignored.
 """
@@ -107,10 +108,11 @@ def build_cli(force: bool = False) -> str | None:
         if nccl:
             cmd += ["-DFMB200_WITH_NCCL", "-I", cuda_inc, "-lnccl", "-L/usr/local/cuda/lib64", "-lcudart"]
         _run(cmd)
-    conv_src = os.path.join(HOST, "convert_main.cpp")
-    conv = os.path.join(BINDIR, "convert")
-    if os.path.exists(conv_src) and (force or _newer(conv, [conv_src] + hdrs)):
-        _run(["g++", "-O2", "-std=c++17", "-Wall", conv_src, "-o", conv, "-pthread"])
+    for tool in ("convert", "transpose"):  # the reference's tools/ (text -> binary, .x -> .xt)
+        src = os.path.join(HOST, tool + "_main.cpp")
+        exe = os.path.join(BINDIR, tool)
+        if os.path.exists(src) and (force or _newer(exe, [src] + hdrs)):
+            _run(["g++", "-O2", "-std=c++17", "-Wall", src, "-o", exe, "-pthread"])
     return out
 
 

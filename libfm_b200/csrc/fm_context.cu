@@ -518,6 +518,48 @@ int fmb200_upload_xblock_async(fmb200_ctx* c, int slot, uint64_t n_rows, uint64_
   return upload_xblock_enqueue(c, slot, n_rows, nnz, words, row_size, target, c->copy_stream);
 }
 
+}  // extern "C"
+
+namespace fmb {
+
+int upload_xt_enqueue(fmb200_ctx* c, int slot, uint64_t n_cols, uint64_t nnz, const void* words,
+                      const uint32_t* col_size, cudaStream_t st) {
+  if (upload_begin(c, slot, n_cols, nnz, st)) return 1;
+  DataSlot& s = c->slots[slot];
+  const uint64_t n_words = n_cols + 2 * nnz;
+  CK(grow(s.x_words, s.x_words_cap, n_words ? n_words : 1));
+  CK(grow(s.x_row_size, s.x_row_size_cap, n_cols ? n_cols : 1));
+  CK(grow(s.x_scan, s.x_scan_cap, aos_scan_tiles(n_cols) + 1));
+  CK(cudaMemcpyAsync(s.x_words.get(), words, n_words * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(s.x_row_size.get(), col_size, n_cols * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+  CK(launch_xblock_to_csr(c, st, s.x_words.get(), s.x_row_size.get(), n_cols, nnz, s.x_scan.get(), s.row_ptr.get(),
+                          s.col.get(), s.val.get(), s.d_flag.get() + 10));
+  CK(launch_max_id(c, st, s.col.get(), nnz, s.d_flag.get() + 8));
+  CK(cudaMemcpyAsync(s.h_flag.get(), s.d_flag.get(), 16 * sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
+  CK(cudaEventRecord(s.ready.get(), st));
+  s.pending = true;
+  return 0;
+}
+
+int upload_xt_finish(fmb200_ctx* c, int slot, uint64_t first_col, uint64_t n_cases) {
+  DataSlot& s = c->slots[slot];
+  if (!s.pending) return 0;
+  CK(cudaEventSynchronize(s.ready.get()));
+  s.pending = false;
+  const unsigned int* h = s.h_flag.get();
+  if (h[10]) return fail("column %llu of the .xt: its header word is not its size",
+                         (unsigned long long)(first_col + s.n_rows - h[10]));
+  if (s.nnz > 0 && h[8] >= n_cases)
+    return fail("case id %u in the .xt block from column %llu is out of range (%llu cases)", h[8],
+                (unsigned long long)first_col, (unsigned long long)n_cases);
+  s.present = true;
+  return 0;
+}
+
+}  // namespace fmb
+
+extern "C" {
+
 int fmb200_host_alloc(void** out, uint64_t bytes) {
   if (!out) return fail("null out pointer");
   *out = nullptr;
@@ -805,6 +847,29 @@ int fmb200_mcmc_begin(fmb200_ctx* c, int train_slot, int test_slot, int do_sampl
     if (!e.empty()) {
       c->mcmc.reset();
       return fail("fmb200_mcmc_begin: %s", e.c_str());
+    }
+    return 0;
+  });
+}
+
+int fmb200_mcmc_begin_xt(fmb200_ctx* c, int train_slot, const fmb200_xt_blocks* train_xt, int test_slot,
+                         const fmb200_xt_blocks* test_xt, int do_sample, int do_multilevel, uint32_t n_groups,
+                         const uint32_t* attr_group, const uint32_t* attr_per_group, double reg0,
+                         const double* w_lambda, const double* v_lambda) {
+  NEED_CTX(c);
+  if ((!train_xt && need_slot(c, train_slot)) || (!test_xt && need_slot(c, test_slot))) return 1;
+  if (bind(c)) return 1;
+  if (need_fp64(c, "MCMC / ALS run on the fp64 state: set INORDER or ORDERED mode first")) return 1;
+  if (!w_lambda || (!v_lambda && c->k > 0)) return fail("null w_lambda / v_lambda");
+  if (c->peer_world > 1) return fail("MCMC / ALS run on one GPU: this context is attached to a multi-GPU peer world");
+  if ((train_xt || test_xt) && c->copy_stream == nullptr)
+    CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
+  return guarded([&]() {
+    const std::string e = mcmc_begin(c, train_slot, test_slot, do_sample, do_multilevel, n_groups, attr_group,
+                                      attr_per_group, reg0, w_lambda, v_lambda, train_xt, test_xt);
+    if (!e.empty()) {
+      c->mcmc.reset();
+      return fail("fmb200_mcmc_begin_xt: %s", e.c_str());
     }
     return 0;
   });

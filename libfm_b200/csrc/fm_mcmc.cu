@@ -14,12 +14,20 @@
 //    it, so a run's features are drawn in parallel (one warp each).  A warp gathers 32 entries
 //    of its column at a time and adds their terms in column order, so each column sum is the
 //    reference's serial chain.  The e-term re-prediction is fm_eterm64_kernel (fm_inorder.cu).
+// Out of core (fmb200_mcmc_begin_xt): a data set given as blocks of its .xt file is streamed through two slots
+// on every pass (xt_pass).  Column sums lie inside one column, so inside one block, and draw_feature runs as
+// it is on the block's columns.  Per-case chains (the q rebuild, the three e-term parts, the begin-time prev
+// index) cross blocks: each case accumulates block by block in file order and, inside a block, in column
+// order, through the block's entries stably sorted by case (xt_case_kernel).  Runs are cut at every block
+// start besides the resident cut.  Passes per iteration: train 1 + k sweeps (the q of factor f + 1 is rebuilt
+// on the pass that sweeps f, into the second q) and k + k1 e-term passes; test k + k1 e-term passes.
 // Each draw needs one standard normal; the host draws them in the reference's order before the
 // launch.  A sampled draw the reference would skip without consuming one (posterior variance
 // not finite, or stdev 0) cannot arise from a finite state; the device flags it and the
 // iteration fails instead of desynchronising the stream.
 // This TU is compiled with --fmad=false: every product and sum rounds as the reference's do.
 #include <cooperative_groups.h>
+#include <cub/device/device_radix_sort.cuh>
 
 #include <algorithm>
 #include <cmath>
@@ -41,8 +49,19 @@ constexpr double kAlpha0 = 1.0, kGamma0 = 1.0, kBeta0 = 1.0, kMu0 = 0.0, kW0Mean
 // device flag words
 enum { F_NAN_W = 0, F_INF_W, F_NAN_V, F_INF_V, F_SKIP, F_WORDS = 8 };
 
+// A data set streamed from blocks of its .xt (fmb200_mcmc_begin_xt)
+struct XtSet {
+  fmb200_xt_blocks src{};
+  std::vector<uint32_t> col_lo;  // [n_blocks + 1]
+  std::vector<uint64_t> nnz;     // [n_blocks]
+  std::vector<uint32_t> run_lo;  // train: block b sweeps the runs [run_lo[b], run_lo[b + 1])
+  DevPtr<double> acc[2];         // test: the two per-case chains of the e-term passes (train uses q and q2)
+  uint64_t n_blocks() const { return nnz.size(); }
+};
+
 struct McmcState {
   int train = 0, test = 1;
+  std::unique_ptr<XtSet> xt[2];  // train, test: null when the set is resident in its slot
   uint64_t train_gen = 0, test_gen = 0;
   bool sample = true, multilevel = true;
   uint32_t G = 1;
@@ -56,12 +75,22 @@ struct McmcState {
   std::vector<uint32_t> runs;  // run starts, then n
   uint32_t iter = 0;
   uint32_t counters[16] = {0};
+  uint64_t n_train = 0, n_test = 0;
   // device
-  DevPtr<uint32_t> col_ptr, cs_case, dup, group_d, runs_d;
+  DevPtr<uint64_t> col_ptr;
+  DevPtr<uint32_t> cs_case, dup, group_d, runs_d;
   DevPtr<float> cs_x;
   DevPtr<double> e_d, q_d, e_test_d, z_d, hyp_d;
   DevPtr<unsigned int> flag_d;
   int grid = 0;
+  // streamed sets: the train targets, the second q, and a block's entries stably sorted by case (the case
+  // ids and the entries' positions in the block; iota = 0, 1, ... is the sort's input)
+  DevPtr<float> y_d;
+  DevPtr<double> q2_d;
+  DevPtr<uint32_t> srt_key, srt_pos, iota;
+  DevPtr<unsigned char> srt_tmp;
+  size_t srt_tmp_bytes = 0;
+  const float* y_dev = nullptr;  // the train targets on the device
 };
 
 void McmcDelete::operator()(McmcState* s) const { delete s; }
@@ -97,7 +126,7 @@ __global__ void mcmc_csc_kernel(const uint32_t* __restrict__ ids, const uint32_t
   }
 }
 
-__global__ void mcmc_colptr_kernel(const uint32_t* __restrict__ ids, uint64_t nnz, uint32_t n, uint32_t* col_ptr) {
+__global__ void mcmc_colptr_kernel(const uint32_t* __restrict__ ids, uint64_t nnz, uint32_t n, uint64_t* col_ptr) {
   for (uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; j <= n; j += (uint64_t)gridDim.x * blockDim.x) {
     uint64_t lo = 0, hi = nnz;  // first position with id >= j
     while (lo < hi) {
@@ -105,7 +134,7 @@ __global__ void mcmc_colptr_kernel(const uint32_t* __restrict__ ids, uint64_t nn
       if (ids[mid] < j) lo = mid + 1;
       else hi = mid;
     }
-    col_ptr[j] = (uint32_t)lo;
+    col_ptr[j] = lo;
   }
 }
 
@@ -116,7 +145,8 @@ __global__ void mcmc_residual_kernel(double* e, const float* __restrict__ y, uin
 
 // ---- device: the sweep -----------------------------------------------------------------------
 struct SweepArgs {
-  const uint32_t* col_ptr;
+  const uint64_t* col_ptr;  // column j's positions: [col_ptr[j - col_lo], col_ptr[j - col_lo + 1]) for j < col_hi;
+  uint32_t col_lo, col_hi;  // columns from col_hi on are empty (a streamed block and the features after the .xt)
   const uint32_t* cs_case;
   const float* cs_x;
   const uint32_t* dup;
@@ -156,7 +186,11 @@ __device__ void draw_feature(const SweepArgs& a, uint32_t j, int f, int lane) {
     zz = a.sample ? a.z[j] : 0.0;
   }
   const double old = *par;
-  const uint32_t beg = a.col_ptr[j], end = a.col_ptr[j + 1];
+  uint32_t beg = 0, end = 0;
+  if (j < a.col_hi) {
+    beg = (uint32_t)a.col_ptr[j - a.col_lo];
+    end = (uint32_t)a.col_ptr[j - a.col_lo + 1];
+  }
   double m = 0.0, s = 0.0;
   for (uint32_t b = beg; b < end; b += 32) {
     const uint32_t idx = b + lane;
@@ -226,9 +260,11 @@ __device__ void draw_feature(const SweepArgs& a, uint32_t j, int f, int lane) {
   }
 }
 
+// runs [r_lo, r_hi)
 template <bool V>
-__device__ void sweep_runs(const SweepArgs& a, cg::grid_group& grid, int f, uint32_t warp, uint32_t nwarp, int lane) {
-  for (uint32_t r = 0; r < a.n_runs; r++) {
+__device__ void sweep_runs(const SweepArgs& a, cg::grid_group& grid, int f, uint32_t r_lo, uint32_t r_hi, uint32_t warp,
+                           uint32_t nwarp, int lane) {
+  for (uint32_t r = r_lo; r < r_hi; r++) {
     const uint32_t j1 = a.runs[r + 1];
     for (uint32_t j = a.runs[r] + warp; j < j1; j += nwarp) draw_feature<V>(a, j, f, lane);
     grid.sync();
@@ -245,7 +281,7 @@ __global__ void __launch_bounds__(256) mcmc_sweep_kernel(const SweepArgs a) {
     for (uint64_t c = tid; c < a.n_rows; c += nth) a.e[c] -= a.e_shift;
     grid.sync();
   }
-  if (a.use_w) sweep_runs<false>(a, grid, 0, warp, nwarp, lane);
+  if (a.use_w) sweep_runs<false>(a, grid, 0, 0, a.n_runs, warp, nwarp, lane);
   for (int f = 0; f < a.k; f++) {
     for (uint64_t c = tid; c < a.n_rows; c += nth) {  // the q rebuild (add_main_q, :406-428)
       const uint64_t beg = a.row_ptr[c];
@@ -254,8 +290,111 @@ __global__ void __launch_bounds__(256) mcmc_sweep_kernel(const SweepArgs a) {
       a.q[c] = row_q(o, a.v, a.k, f, a.val + beg);
     }
     grid.sync();
-    sweep_runs<true>(a, grid, f, warp, nwarp, lane);
+    sweep_runs<true>(a, grid, f, 0, a.n_runs, warp, nwarp, lane);
   }
+}
+
+// ---- device: the streamed passes ---------------------------------------------------------------
+// the sweep of w (V = false) or of factor f over the runs [r_lo, r_hi) of one block
+template <bool V>
+__global__ void __launch_bounds__(256) mcmc_block_sweep_kernel(const SweepArgs a, uint32_t r_lo, uint32_t r_hi, int f) {
+  cg::grid_group grid = cg::this_grid();
+  const uint64_t tid = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+  const uint64_t nth = (uint64_t)gridDim.x * blockDim.x;
+  sweep_runs<V>(a, grid, f, r_lo, r_hi, (uint32_t)(tid >> 5), (uint32_t)(nth >> 5), threadIdx.x & 31);
+}
+
+// What a case adds from one block, in column order (the block's entries stably sorted by case):
+//   CH_Q        q[c] += v[j][f] x                           the q rebuild (add_main_q, fm_learn_mcmc.h:406-428)
+//   CH_ETERM_V  q[c] += v[j][f] x;  q2[c] -= 0.5 v^2 x^2    e-term parts (1) and (2) of factor f (:172-306)
+//   CH_ETERM_W  q2[c] += w[j] x                             e-term part (3) (:309-346)
+//   CH_PREV     prev[j] := max(prev[j], 1 + the largest id below j the case names, in this block or before
+//               it: last[c]); dup[j] := 1 when the case is named twice by column j; last[c] := 1 + its last id
+// Every sum is the one fm_eterm64_kernel / row_q form for the case, in the same order (--fmad=false).
+enum { CH_Q = 0, CH_ETERM_V, CH_ETERM_W, CH_PREV };
+struct ChainArgs {
+  const uint32_t* key;      // the entries' cases, sorted
+  const uint32_t* pos;      // the entries' positions in the block, in that order
+  uint64_t nnz;
+  const uint64_t* col_ptr;  // the block's column offsets
+  uint64_t n_cols;
+  uint32_t col_lo;          // the block's first column
+  const float* val;
+  const double* v;
+  const double* w;
+  int k, f;
+  double* q;
+  double* q2;
+  uint32_t* last;
+  unsigned int* prev;
+  uint32_t* dup;
+};
+
+template <int OP>
+__global__ void xt_case_kernel(const ChainArgs a) {
+  for (uint64_t p = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; p < a.nnz; p += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t c = a.key[p];
+    if (p > 0 && a.key[p - 1] == c) continue;  // one thread per case: the one at its first entry
+    double q = 0.0, q2 = 0.0;
+    if (OP == CH_Q || OP == CH_ETERM_V) q = a.q[c];
+    if (OP == CH_ETERM_V || OP == CH_ETERM_W) q2 = a.q2[c];
+    uint32_t below = 0, cur = 0xffffffffu;
+    if (OP == CH_PREV) below = a.last[c];
+    for (uint64_t i = p; i < a.nnz && a.key[i] == c; i++) {
+      const uint32_t e = a.pos[i];
+      const uint32_t j = a.col_lo + (uint32_t)row_of(a.col_ptr, a.n_cols, e);
+      if (OP == CH_Q) q += a.v[(size_t)j * a.k + a.f] * (double)a.val[e];
+      if (OP == CH_ETERM_V) {
+        const double vif = a.v[(size_t)j * a.k + a.f];
+        const float xi = a.val[e];
+        q += vif * (double)xi;
+        q2 -= 0.5 * vif * vif * xi * xi;
+      }
+      if (OP == CH_ETERM_W) q2 += a.w[j] * (double)a.val[e];
+      if (OP == CH_PREV) {
+        if (j == cur) {
+          a.dup[j] = 1u;
+        } else {
+          if (cur != 0xffffffffu) below = cur + 1;
+          cur = j;
+        }
+        if (below) atomicMax(a.prev + j, below);
+      }
+    }
+    if (OP == CH_Q || OP == CH_ETERM_V) a.q[c] = q;
+    if (OP == CH_ETERM_V || OP == CH_ETERM_W) a.q2[c] = q2;
+    if (OP == CH_PREV) a.last[c] = cur + 1;
+  }
+}
+
+// after the e-term pass of a factor: e += 0.5 q^2 (:250), and q restarts at 0 for the next factor
+__global__ void eterm_factor_kernel(double* e, double* q, uint64_t n) {
+  for (uint64_t c = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; c < n; c += (uint64_t)gridDim.x * blockDim.x) {
+    const double qc = q[c];
+    e[c] += 0.5 * qc * qc;
+    q[c] = 0.0;
+  }
+}
+
+// e = (e + q2) + w0 (:350-362)
+__global__ void eterm_final_kernel(double* e, const double* q2, uint64_t n, int use_w0, const double* w0) {
+  for (uint64_t c = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; c < n; c += (uint64_t)gridDim.x * blockDim.x) {
+    double x = e[c];
+    x = x + q2[c];
+    if (use_w0) x += *w0;
+    e[c] = x;
+  }
+}
+
+// draw_w0's update of e (:680-682)
+__global__ void mcmc_shift_kernel(double* e, uint64_t n, double e_shift) {
+  for (uint64_t c = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; c < n; c += (uint64_t)gridDim.x * blockDim.x)
+    e[c] -= e_shift;
+}
+
+__global__ void iota_kernel(uint32_t* x, uint64_t n) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
+    x[i] = (uint32_t)i;
 }
 
 }  // namespace
@@ -269,14 +408,189 @@ __global__ void __launch_bounds__(256) mcmc_sweep_kernel(const SweepArgs a) {
 
 namespace {
 
+// ---- streamed sets -----------------------------------------------------------------------------
+// One pass over a streamed set in file order: use(slot, b) once per block, in order.  Block b is fetched and
+// goes to slot src.slot[b % 2] on the copy stream, so the copy of block b + 1 runs while the work use()
+// enqueued on block b does; before block b + 1 overwrites block b - 1's slot, the work on b - 1 has run.
+template <class F>
+std::string xt_pass(fmb200_ctx* c, XtSet& x, F use) {
+  const uint64_t nb = x.n_blocks();
+  auto slot = [&](uint64_t b) { return x.src.slot[b % 2]; };
+  auto upload = [&](uint64_t b) -> std::string {
+    const void* words = nullptr;
+    const uint32_t* sizes = nullptr;
+    if (x.src.fetch(x.src.user, b, &words, &sizes) != 0) return "fetching block " + std::to_string(b) + " of the .xt failed";
+    if (upload_xt_enqueue(c, slot(b), x.col_lo[b + 1] - x.col_lo[b], x.nnz[b], words, sizes, c->copy_stream))
+      return fmb200_last_error();
+    return "";
+  };
+  MK(cudaStreamSynchronize(c->stream));  // the slots may hold blocks the previous pass still works on
+  std::string err = upload(0);
+  for (uint64_t b = 0; err.empty() && b < nb; b++) {
+    if (b + 1 < nb) {
+      if (b > 0) MK(cudaStreamSynchronize(c->stream));
+      err = upload(b + 1);
+      if (!err.empty()) break;
+    }
+    if (upload_xt_finish(c, slot(b), x.col_lo[b], x.src.n_cases)) {
+      err = fmb200_last_error();
+      break;
+    }
+    x.src.release(x.src.user, b);  // its copy has finished
+    err = use(slot(b), b);
+  }
+  if (!err.empty()) cudaStreamSynchronize(c->copy_stream);  // no copy may still read a fetched block
+  return err;
+}
+
+// The block in `slot` by case, stably: s.srt_key = the entries' cases, s.srt_pos = their positions.  The chain
+// arguments for it.
+std::string sort_block(fmb200_ctx* c, McmcState& s, const DataSlot& d, uint64_t n_cases, uint32_t col_lo, ChainArgs* a) {
+  int bits = 1;
+  while (bits < 32 && ((n_cases - 1) >> bits) != 0) bits++;
+  size_t tmp = s.srt_tmp_bytes;
+  MK(cub::DeviceRadixSort::SortPairs(s.srt_tmp.get(), tmp, d.col.get(), s.srt_key.get(), s.iota.get(), s.srt_pos.get(),
+                                     d.nnz, 0, bits, c->stream));
+  c->launches++;
+  *a = ChainArgs{};
+  a->key = s.srt_key.get();
+  a->pos = s.srt_pos.get();
+  a->nnz = d.nnz;
+  a->col_ptr = d.row_ptr.get();
+  a->n_cols = d.n_rows;
+  a->col_lo = col_lo;
+  a->val = d.val.get();
+  a->v = c->p64.v();
+  a->w = c->p64.w();
+  a->k = c->k;
+  return "";
+}
+
+template <int OP>
+std::string chain(fmb200_ctx* c, const ChainArgs& a) {
+  xt_case_kernel<OP><<<grid_for(c, a.nnz), 256, 0, c->stream>>>(a);
+  c->launches++;
+  MK(cudaGetLastError());
+  return "";
+}
+
+// The e-terms of a streamed set into e[n] (fm_eterm64_kernel's sums, case by case in the same order):
+// one pass per factor for parts (1) and (2), one for part (3); acc, acc2: two per-case chains.
+std::string xt_eterms(fmb200_ctx* c, McmcState& s, XtSet& x, double* e, double* acc, double* acc2) {
+  const uint64_t n = x.src.n_cases;
+  if (n == 0) return "";
+  MK(cudaMemsetAsync(e, 0, n * sizeof(double), c->stream));
+  MK(cudaMemsetAsync(acc, 0, n * sizeof(double), c->stream));
+  MK(cudaMemsetAsync(acc2, 0, n * sizeof(double), c->stream));
+  for (int f = 0; f <= c->k; f++) {
+    if (f == c->k && !c->k1) break;
+    const std::string err = xt_pass(c, x, [&](int slot, uint64_t b) -> std::string {
+      const DataSlot& d = c->slots[slot];
+      if (d.nnz == 0) return "";
+      ChainArgs a;
+      std::string r = sort_block(c, s, d, n, x.col_lo[b], &a);
+      if (!r.empty()) return r;
+      a.f = f;
+      a.q = acc;
+      a.q2 = acc2;
+      return f < c->k ? chain<CH_ETERM_V>(c, a) : chain<CH_ETERM_W>(c, a);
+    });
+    if (!err.empty()) return err;
+    if (f < c->k) {
+      eterm_factor_kernel<<<grid_for(c, n), 256, 0, c->stream>>>(e, acc, n);
+      c->launches++;
+    }
+  }
+  eterm_final_kernel<<<grid_for(c, n), 256, 0, c->stream>>>(e, acc2, n, c->k0, c->p64.w0());
+  c->launches++;
+  MK(cudaGetLastError());
+  return "";
+}
+
+// The sweep over a streamed training set: pass -1 draws w, pass f draws factor f, block by block over the
+// block's runs.  The q of factor f + 1 (which reads only v(f + 1, .), untouched by the sweep of f) is rebuilt on
+// pass f into the other q array.
+std::string xt_sweep(fmb200_ctx* c, McmcState& s, SweepArgs a) {
+  XtSet& x = *s.xt[0];
+  const uint64_t N = s.n_train;
+  double* q[2] = {s.q_d.get(), s.q2_d.get()};
+  for (int p = -1; p < a.k; p++) {
+    const bool sweep = p >= 0 || a.use_w, rebuild = p + 1 < a.k;
+    if (!sweep && !rebuild) continue;
+    double* qn = rebuild ? q[(p + 1) % 2] : nullptr;
+    if (rebuild) MK(cudaMemsetAsync(qn, 0, N * sizeof(double), c->stream));
+    if (p >= 0) a.q = q[p % 2];
+    const std::string err = xt_pass(c, x, [&](int slot, uint64_t b) -> std::string {
+      const DataSlot& d = c->slots[slot];
+      if (rebuild && d.nnz > 0) {
+        ChainArgs ca;
+        std::string r = sort_block(c, s, d, N, x.col_lo[b], &ca);
+        if (r.empty()) {
+          ca.f = p + 1;
+          ca.q = qn;
+          r = chain<CH_Q>(c, ca);
+        }
+        if (!r.empty()) return r;
+      }
+      uint32_t r_lo = x.run_lo[b], r_hi = x.run_lo[b + 1];
+      if (sweep && r_lo < r_hi) {
+        a.col_ptr = d.row_ptr.get();
+        a.cs_case = d.col.get();
+        a.cs_x = d.val.get();
+        a.col_lo = x.col_lo[b];
+        a.col_hi = x.col_lo[b + 1];
+        int f = p < 0 ? 0 : p;
+        void* args[] = {(void*)&a, (void*)&r_lo, (void*)&r_hi, (void*)&f};
+        const void* fn = p < 0 ? (const void*)mcmc_block_sweep_kernel<false> : (const void*)mcmc_block_sweep_kernel<true>;
+        MK(cudaLaunchCooperativeKernel(fn, dim3(s.grid), dim3(256), args, 0, c->stream));
+        c->launches++;
+      }
+      return "";
+    });
+    if (!err.empty()) return err;
+  }
+  return "";
+}
+
 std::string repredict(fmb200_ctx* c, McmcState& s) {
-  const DataSlot& tr = c->slots[s.train];
-  const DataSlot& te = c->slots[s.test];
-  MK(launch_mcmc_eterms(c, tr, s.e_d.get()));
-  MK(launch_mcmc_eterms(c, te, s.e_test_d.get()));
-  MK(cudaMemcpyAsync(s.e.data(), s.e_d.get(), tr.n_rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  if (te.n_rows) MK(cudaMemcpyAsync(s.e_test.data(), s.e_test_d.get(), te.n_rows * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  if (s.xt[0]) {
+    const std::string err = xt_eterms(c, s, *s.xt[0], s.e_d.get(), s.q_d.get(), s.q2_d.get());
+    if (!err.empty()) return err;
+  } else {
+    MK(launch_mcmc_eterms(c, c->slots[s.train], s.e_d.get()));
+  }
+  if (s.xt[1]) {
+    const std::string err = xt_eterms(c, s, *s.xt[1], s.e_test_d.get(), s.xt[1]->acc[0].get(), s.xt[1]->acc[1].get());
+    if (!err.empty()) return err;
+  } else {
+    MK(launch_mcmc_eterms(c, c->slots[s.test], s.e_test_d.get()));
+  }
+  MK(cudaMemcpyAsync(s.e.data(), s.e_d.get(), s.n_train * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  if (s.n_test) MK(cudaMemcpyAsync(s.e_test.data(), s.e_test_d.get(), s.n_test * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   MK(cudaStreamSynchronize(c->stream));
+  return "";
+}
+
+// The checks of a fmb200_xt_blocks and the set it describes; "" when it may be streamed.
+std::string xt_open(const fmb200_ctx* c, const fmb200_xt_blocks& src, const char* which, std::unique_ptr<XtSet>* out) {
+  const std::string w = std::string("the ") + which + " .xt blocks: ";
+  if (src.n_blocks == 0 || !src.col_lo || !src.nnz || !src.fetch || !src.release) return w + "no blocks or a null pointer";
+  if (src.n_cases && !src.target) return w + "null target";
+  if (src.n_cases >= 0xffffffffull) return w + "2^32 cases and more are not supported";
+  for (int i = 0; i < 2; i++)
+    if (src.slot[i] < 0 || src.slot[i] >= FMB200_MAX_SLOTS) return w + "slot out of range";
+  if (src.slot[0] == src.slot[1]) return w + "the two slots must differ";
+  if (src.col_lo[0] != 0 || src.col_lo[src.n_blocks] > c->n)
+    return w + "the columns must start at 0 and end at or below num_attribute";
+  std::unique_ptr<XtSet> x(new XtSet());
+  x->src = src;
+  x->col_lo.assign(src.col_lo, src.col_lo + src.n_blocks + 1);
+  x->nnz.assign(src.nnz, src.nnz + src.n_blocks);
+  for (uint64_t b = 0; b < src.n_blocks; b++) {
+    if (x->col_lo[b + 1] < x->col_lo[b]) return w + "column ranges out of order";
+    if (x->nnz[b] >= 0xffffffffull) return w + "a block of 2^32 entries and more is not supported";
+  }
+  *out = std::move(x);
   return "";
 }
 
@@ -330,11 +644,37 @@ bool draw_mu(const McmcState& s, const double* par, double* mu, const double* la
 
 std::string mcmc_begin(fmb200_ctx* c, int train, int test, int do_sample, int do_multilevel, uint32_t G,
                        const uint32_t* attr_group, const uint32_t* attr_per_group, double reg0,
-                       const double* w_lambda0, const double* v_lambda0) {
-  DataSlot& d = c->slots[train];
-  const DataSlot& dt = c->slots[test];
-  if (d.n_rows == 0) return "the training set is empty";
-  if (d.n_rows >= 0xffffffffull || d.nnz >= 0xffffffffull) return "training sets of 2^32 cases or entries and more are not supported";
+                       const double* w_lambda0, const double* v_lambda0, const fmb200_xt_blocks* train_xt,
+                       const fmb200_xt_blocks* test_xt) {
+  std::unique_ptr<XtSet> xt[2];
+  if (train_xt) {
+    const std::string e = xt_open(c, *train_xt, "train", &xt[0]);
+    if (!e.empty()) return e;
+  }
+  if (test_xt) {
+    const std::string e = xt_open(c, *test_xt, "test", &xt[1]);
+    if (!e.empty()) return e;
+  }
+  {  // no slot may serve two purposes
+    std::vector<int> used;
+    used.push_back(train_xt ? train_xt->slot[0] : train);
+    if (train_xt) used.push_back(train_xt->slot[1]);
+    if (test_xt) {
+      used.push_back(test_xt->slot[0]);
+      used.push_back(test_xt->slot[1]);
+    } else if (test != train) {
+      used.push_back(test);
+    }
+    for (size_t i = 0; i < used.size(); i++)
+      for (size_t j = 0; j < i; j++)
+        if (used[i] == used[j]) return "a streamed set's slots must differ from every other slot in use";
+  }
+  const DataSlot* d = train_xt ? nullptr : &c->slots[train];
+  const DataSlot* dt = test_xt ? nullptr : &c->slots[test];
+  const uint64_t n_train = d ? d->n_rows : train_xt->n_cases, n_test = dt ? dt->n_rows : test_xt->n_cases;
+  if (n_train == 0) return "the training set is empty";
+  if (d && (d->n_rows >= 0xffffffffull || d->nnz >= 0xffffffffull))
+    return "training sets of 2^32 cases or entries and more are not supported";
   if (G == 0) return "n_groups must be >= 1";
   c->mcmc.reset(new McmcState());
   McmcState& s = *c->mcmc;
@@ -342,8 +682,12 @@ std::string mcmc_begin(fmb200_ctx* c, int train, int test, int do_sample, int do
   const int k = c->k;
   s.train = train;
   s.test = test;
-  s.train_gen = d.upload_gen;
-  s.test_gen = dt.upload_gen;
+  s.xt[0] = std::move(xt[0]);
+  s.xt[1] = std::move(xt[1]);
+  s.n_train = n_train;
+  s.n_test = n_test;
+  s.train_gen = d ? d->upload_gen : 0;
+  s.test_gen = dt ? dt->upload_gen : 0;
   s.sample = do_sample != 0;
   s.multilevel = do_multilevel != 0;
   s.G = G;
@@ -363,68 +707,135 @@ std::string mcmc_begin(fmb200_ctx* c, int train, int test, int do_sample, int do
   s.v_mu.assign((size_t)G * k, 0.0);
   s.w_lambda.assign(w_lambda0, w_lambda0 + G);
   s.v_lambda.assign(v_lambda0, v_lambda0 + (size_t)G * k);
-  s.y.resize(d.n_rows);
-  s.y_test.resize(dt.n_rows);
-  s.e.resize(d.n_rows);
-  s.e_test.resize(dt.n_rows);
-  s.pred_this.assign(dt.n_rows, 0.0);
-  s.pred_all.assign(dt.n_rows, 0.0);
-  s.pred_but5.assign(dt.n_rows, 0.0);
-  MK(alloc(s.col_ptr, n + 1));
-  MK(alloc(s.cs_case, d.nnz));
-  MK(alloc(s.cs_x, d.nnz));
+  s.y.resize(n_train);
+  s.y_test.resize(n_test);
+  s.e.resize(n_train);
+  s.e_test.resize(n_test);
+  s.pred_this.assign(n_test, 0.0);
+  s.pred_all.assign(n_test, 0.0);
+  s.pred_but5.assign(n_test, 0.0);
+  if (d) {
+    MK(alloc(s.col_ptr, n + 1));
+    MK(alloc(s.cs_case, d->nnz));
+    MK(alloc(s.cs_x, d->nnz));
+  }
   MK(alloc(s.dup, n));
   MK(alloc(s.group_d, n));
-  MK(alloc(s.e_d, d.n_rows));
-  MK(alloc(s.q_d, d.n_rows));
-  MK(alloc(s.e_test_d, dt.n_rows));
+  MK(alloc(s.e_d, n_train));
+  MK(alloc(s.q_d, n_train));
+  MK(alloc(s.e_test_d, n_test));
   MK(alloc(s.z_d, (size_t)(k + 1) * n));
   MK(alloc(s.hyp_d, 2 * G + 2 * (size_t)G * k));
   MK(alloc(s.flag_d, F_WORDS));
-  MK(cudaMemcpyAsync(s.y.data(), d.target.get(), d.n_rows * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-  if (dt.n_rows) MK(cudaMemcpyAsync(s.y_test.data(), dt.target.get(), dt.n_rows * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+  if (d) {
+    MK(cudaMemcpyAsync(s.y.data(), d->target.get(), n_train * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    s.y_dev = d->target.get();
+  } else {
+    std::copy(train_xt->target, train_xt->target + n_train, s.y.begin());
+    MK(alloc(s.y_d, n_train));
+    MK(alloc(s.q2_d, n_train));
+    MK(cudaMemcpyAsync(s.y_d.get(), s.y.data(), n_train * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    s.y_dev = s.y_d.get();
+  }
+  if (dt) {
+    if (n_test) MK(cudaMemcpyAsync(s.y_test.data(), dt->target.get(), n_test * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+  } else {
+    std::copy(test_xt->target, test_xt->target + n_test, s.y_test.begin());
+    for (auto& acc : s.xt[1]->acc) MK(alloc(acc, n_test));
+  }
+  if (s.xt[0] || s.xt[1]) {  // the by-case sort of the largest block
+    uint64_t max_nnz = 1;
+    for (const auto& x : s.xt)
+      if (x) max_nnz = std::max(max_nnz, *std::max_element(x->nnz.begin(), x->nnz.end()));
+    MK(alloc(s.srt_key, max_nnz));
+    MK(alloc(s.srt_pos, max_nnz));
+    MK(alloc(s.iota, max_nnz));
+    iota_kernel<<<grid_for(c, max_nnz), 256, 0, c->stream>>>(s.iota.get(), max_nnz);
+    c->launches++;
+    MK(cub::DeviceRadixSort::SortPairs(nullptr, s.srt_tmp_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr,
+                                       (const uint32_t*)nullptr, (uint32_t*)nullptr, max_nnz, 0, 32, c->stream));
+    MK(alloc(s.srt_tmp, s.srt_tmp_bytes ? s.srt_tmp_bytes : 1));
+  }
   MK(cudaMemcpyAsync(s.group_d.get(), s.group.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
   MK(cudaMemsetAsync(s.dup.get(), 0, n * sizeof(uint32_t), c->stream));
 
-  // transposed training data + feature runs, from the (id, entry) sort of the ORDERED index
+  // transposed training data + feature runs, from the (id, entry) sort of the ORDERED index, or from one pass
+  // over the streamed .xt
   std::vector<uint32_t> prev(n, 0u);
-  if (d.nnz > 0) {
+  if (s.xt[0]) {
+    DevPtr<unsigned int> prev_d;
+    DevPtr<uint32_t> last;
+    MK(alloc(prev_d, n ? n : 1));
+    MK(alloc(last, n_train));
+    MK(cudaMemsetAsync(prev_d.get(), 0, n * sizeof(unsigned int), c->stream));
+    MK(cudaMemsetAsync(last.get(), 0, n_train * sizeof(uint32_t), c->stream));
+    const std::string err = xt_pass(c, *s.xt[0], [&](int slot, uint64_t b) -> std::string {
+      const DataSlot& blk = c->slots[slot];
+      if (blk.nnz == 0) return "";
+      ChainArgs a;
+      const std::string r = sort_block(c, s, blk, n_train, s.xt[0]->col_lo[b], &a);
+      if (!r.empty()) return r;
+      a.last = last.get();
+      a.prev = prev_d.get();
+      a.dup = s.dup.get();
+      return chain<CH_PREV>(c, a);
+    });
+    if (!err.empty()) return err;
+    MK(cudaMemcpyAsync(prev.data(), prev_d.get(), n * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+    MK(cudaStreamSynchronize(c->stream));
+  } else if (d->nnz > 0) {
+    DataSlot& dm = c->slots[train];
     SortedEntries se;
-    MK(build_ordered_links(c, d, &se));
-    mcmc_csc_kernel<<<grid_for(c, d.nnz), 256, 0, c->stream>>>(se.ids, se.ent, d.nnz, d.row_ptr.get(), d.n_rows,
-                                                               d.val.get(), s.cs_case.get(), s.cs_x.get(), s.dup.get());
-    mcmc_colptr_kernel<<<grid_for(c, (uint64_t)n + 1), 256, 0, c->stream>>>(se.ids, d.nnz, n, s.col_ptr.get());
+    MK(build_ordered_links(c, dm, &se));
+    mcmc_csc_kernel<<<grid_for(c, dm.nnz), 256, 0, c->stream>>>(se.ids, se.ent, dm.nnz, dm.row_ptr.get(), dm.n_rows,
+                                                                dm.val.get(), s.cs_case.get(), s.cs_x.get(), s.dup.get());
+    mcmc_colptr_kernel<<<grid_for(c, (uint64_t)n + 1), 256, 0, c->stream>>>(se.ids, dm.nnz, n, s.col_ptr.get());
     DevPtr<unsigned int> prev_d;
     MK(alloc(prev_d, n));
     MK(cudaMemsetAsync(prev_d.get(), 0, n * sizeof(unsigned int), c->stream));
-    mcmc_prev_kernel<<<grid_for(c, d.n_rows), 256, 0, c->stream>>>(d.row_ptr.get(), d.col.get(), d.n_rows, prev_d.get());
+    mcmc_prev_kernel<<<grid_for(c, dm.n_rows), 256, 0, c->stream>>>(dm.row_ptr.get(), dm.col.get(), dm.n_rows, prev_d.get());
     c->launches += 3;
     MK(cudaGetLastError());
     MK(cudaMemcpyAsync(prev.data(), prev_d.get(), n * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
     MK(cudaStreamSynchronize(c->stream));
   } else {
-    MK(cudaMemsetAsync(s.col_ptr.get(), 0, (n + 1) * sizeof(uint32_t), c->stream));
+    MK(cudaMemsetAsync(s.col_ptr.get(), 0, (n + 1) * sizeof(uint64_t), c->stream));
   }
   MK(cudaStreamSynchronize(c->stream));
-  // cut greedily: j opens a new run when it shares a case with a feature of the current run
+  // cut greedily: j opens a new run when it shares a case with a feature of the current run; a streamed set
+  // also cuts at every block start, so that a run never spans two blocks
+  std::vector<bool> block_start(n, false);
+  if (s.xt[0])
+    for (uint64_t b = 1; b < s.xt[0]->n_blocks(); b++)
+      if (s.xt[0]->col_lo[b] < n) block_start[s.xt[0]->col_lo[b]] = true;
   s.runs.clear();
   if (n > 0) s.runs.push_back(0);
   for (uint32_t j = 1; j < n; j++)
-    if (prev[j] != 0 && prev[j] - 1 >= s.runs.back()) s.runs.push_back(j);
+    if ((prev[j] != 0 && prev[j] - 1 >= s.runs.back()) || block_start[j]) s.runs.push_back(j);
   s.runs.push_back(n);
+  if (s.xt[0]) {  // block b sweeps the runs that start in its columns; the last block also the features after them
+    XtSet& x = *s.xt[0];
+    x.run_lo.resize(x.n_blocks() + 1);
+    for (uint64_t b = 0; b < x.n_blocks(); b++)
+      x.run_lo[b] = (uint32_t)(std::lower_bound(s.runs.begin(), s.runs.end() - 1, x.col_lo[b]) - s.runs.begin());
+    x.run_lo[x.n_blocks()] = (uint32_t)s.runs.size() - 1;
+  }
   MK(alloc(s.runs_d, s.runs.size()));
   MK(cudaMemcpyAsync(s.runs_d.get(), s.runs.data(), s.runs.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
 
-  int occ = 0;
+  int occ = 0, occ_w = 0, occ_v = 0;
   MK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, mcmc_sweep_kernel, 256, 0));
+  MK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_w, mcmc_block_sweep_kernel<false>, 256, 0));
+  MK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_v, mcmc_block_sweep_kernel<true>, 256, 0));
+  if (s.xt[0]) occ = std::min(occ_w, occ_v);
   if (occ < 1) return "the sweep kernel does not fit an SM";
   s.grid = occ * c->sm_count;
 
   // fm_learn_mcmc_simultaneous.h:69-86: predict, then e := prediction - target (both tasks)
   const std::string err = repredict(c, s);
   if (!err.empty()) return err;
-  for (uint64_t i = 0; i < d.n_rows; i++) s.e[i] = s.e[i] - s.y[i];
-  MK(cudaMemcpyAsync(s.e_d.get(), s.e.data(), d.n_rows * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  for (uint64_t i = 0; i < n_train; i++) s.e[i] = s.e[i] - s.y[i];
+  MK(cudaMemcpyAsync(s.e_d.get(), s.e.data(), n_train * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   MK(cudaStreamSynchronize(c->stream));
   s.state.resize(c->p64.n_doubles);
   s.z.resize((size_t)(k + 1) * n);
@@ -434,13 +845,11 @@ std::string mcmc_begin(fmb200_ctx* c, int train, int test, int do_sample, int do
 
 std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counters) {
   McmcState& s = *c->mcmc;
-  const DataSlot& d = c->slots[s.train];
-  const DataSlot& dt = c->slots[s.test];
-  if (d.upload_gen != s.train_gen || dt.upload_gen != s.test_gen)
+  if ((!s.xt[0] && c->slots[s.train].upload_gen != s.train_gen) || (!s.xt[1] && c->slots[s.test].upload_gen != s.test_gen))
     return "the train or test slot was re-uploaded: call fmb200_mcmc_begin again";
   const uint32_t n = c->n, G = s.G;
   const int k = c->k;
-  const uint64_t N = d.n_rows;
+  const uint64_t N = s.n_train, NT = s.n_test;
   const bool sample = s.sample, ml = s.multilevel;
   uint32_t* cnt = s.counters;  // nan, inf of: alpha, w0, w, v, w_mu, w_lambda, v_mu, v_lambda
   std::fill(cnt, cnt + 16, 0u);
@@ -508,18 +917,23 @@ std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counte
   MK(cudaMemcpyAsync(s.hyp_d.get(), s.hyp.data(), s.hyp.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   if (sample) MK(cudaMemcpyAsync(s.z_d.get(), s.z.data(), s.z.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
   SweepArgs a{};
-  a.col_ptr = s.col_ptr.get();
-  a.cs_case = s.cs_case.get();
-  a.cs_x = s.cs_x.get();
+  if (!s.xt[0]) {
+    const DataSlot& d = c->slots[s.train];
+    a.col_ptr = s.col_ptr.get();
+    a.col_lo = 0;
+    a.col_hi = n;
+    a.cs_case = s.cs_case.get();
+    a.cs_x = s.cs_x.get();
+    a.row_ptr = d.row_ptr.get();
+    a.col = d.col.get();
+    a.val = d.val.get();
+  }
   a.dup = s.dup.get();
   a.group = s.group_d.get();
   a.runs = s.runs_d.get();
   a.n_runs = (uint32_t)s.runs.size() - 1;
   a.n = n;
   a.G = G;
-  a.row_ptr = d.row_ptr.get();
-  a.col = d.col.get();
-  a.val = d.val.get();
   a.n_rows = N;
   a.e = s.e_d.get();
   a.q = s.q_d.get();
@@ -534,7 +948,14 @@ std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counte
   a.z = s.z_d.get();
   a.hyp = s.hyp_d.get();
   a.flag = s.flag_d.get();
-  if (a.shift || a.use_w || k > 0) {
+  if (s.xt[0]) {
+    if (shift) {
+      mcmc_shift_kernel<<<grid_for(c, N), 256, 0, c->stream>>>(s.e_d.get(), N, e_shift);
+      c->launches++;
+    }
+    const std::string err = xt_sweep(c, s, a);
+    if (!err.empty()) return err;
+  } else if (a.shift || a.use_w || k > 0) {
     void* args[] = {(void*)&a};
     MK(cudaLaunchCooperativeKernel((const void*)mcmc_sweep_kernel, dim3(s.grid), dim3(256), args, 0, c->stream));
     c->launches++;
@@ -559,7 +980,7 @@ std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counte
   const uint32_t i = s.iter;
   const double lo = c->hp.min_target, hi = c->hp.max_target;
   if (c->hp.task == FMB200_TASK_REGRESSION) {
-    for (uint64_t t = 0; t < dt.n_rows; t++) {
+    for (uint64_t t = 0; t < NT; t++) {
       double p = s.e_test[t];
       s.pred_this[t] = p;
       p = std::min(hi, p);
@@ -576,12 +997,12 @@ std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counte
       rmse += er * er;
     }
     *train_metric = std::sqrt(rmse / N);
-    mcmc_residual_kernel<<<grid_for(c, N), 256, 0, c->stream>>>(s.e_d.get(), d.target.get(), N);
+    mcmc_residual_kernel<<<grid_for(c, N), 256, 0, c->stream>>>(s.e_d.get(), s.y_dev, N);
     c->launches++;
     MK(cudaGetLastError());
     for (uint64_t t = 0; t < N; t++) s.e[t] = s.e[t] - s.y[t];
   } else {
-    for (uint64_t t = 0; t < dt.n_rows; t++) {
+    for (uint64_t t = 0; t < NT; t++) {
       const double p = cdf_gaussian(s.e_test[t]);
       s.pred_this[t] = p;
       s.pred_all[t] += p;

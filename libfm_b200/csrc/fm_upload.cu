@@ -197,6 +197,15 @@ void launch_row_offsets(fmb200_ctx* c, cudaStream_t st, Rows rows, uint64_t n_ro
   }
 }
 
+// *out := the largest id of col[0..nnz) (atomicMax; *out starts at 0)
+__global__ void max_id_kernel(const uint32_t* __restrict__ col, uint64_t nnz, unsigned int* out) {
+  unsigned int m = 0;
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < nnz; i += (uint64_t)gridDim.x * blockDim.x)
+    m = max(m, col[i]);
+  m = __reduce_max_sync(0xffffffffu, m);
+  if ((threadIdx.x & 31) == 0 && m) atomicMax(out, m);
+}
+
 __global__ void onehot_fill_kernel(uint64_t n_rows, uint32_t z, uint64_t* __restrict__ row_ptr,
                                    float* __restrict__ val) {
   const uint64_t nnz = n_rows * z;
@@ -235,6 +244,14 @@ cudaError_t launch_xblock_to_csr(fmb200_ctx* c, cudaStream_t st, const unsigned 
   if (n_rows > 0 && nnz > 0) {
     const uint64_t grid = (n_rows + XSPLIT_ROWS - 1) / XSPLIT_ROWS;
     xblock_split_kernel<<<(unsigned)grid, XSPLIT_ROWS, 0, st>>>(d_words, row_ptr, n_rows, nnz, col, val);
+    c->launches++;
+  }
+  return cudaGetLastError();
+}
+
+cudaError_t launch_max_id(fmb200_ctx* c, cudaStream_t st, const uint32_t* col, uint64_t nnz, unsigned int* out) {
+  if (nnz > 0) {
+    max_id_kernel<<<grid_for(c, nnz), 256, 0, st>>>(col, nnz, out);
     c->launches++;
   }
   return cudaGetLastError();

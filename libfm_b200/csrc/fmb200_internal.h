@@ -301,7 +301,8 @@ cudaError_t launch_mcmc_eterms(fmb200_ctx* c, const DataSlot& d, double* e_out);
 // fm_mcmc.cu: MCMC / ALS learning (fm_learn_mcmc_simultaneous); "" on success, else the error
 std::string mcmc_begin(fmb200_ctx* c, int train, int test, int do_sample, int do_multilevel, uint32_t n_groups,
                        const uint32_t* attr_group, const uint32_t* attr_per_group, double reg0,
-                       const double* w_lambda0, const double* v_lambda0);
+                       const double* w_lambda0, const double* v_lambda0, const fmb200_xt_blocks* train_xt = nullptr,
+                       const fmb200_xt_blocks* test_xt = nullptr);
 std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counters);
 bool mcmc_get(const fmb200_ctx* c, double* alpha, double* w_mu, double* w_lambda, double* v_mu, double* v_lambda,
               double* pred_this, double* pred_sum_all, double* pred_sum_all_but5, uint32_t* n_runs);
@@ -348,6 +349,16 @@ cudaError_t launch_xblock_to_csr(fmb200_ctx* c, cudaStream_t st, const unsigned 
                                  uint64_t n_rows, uint64_t nnz, unsigned long long* scratch, uint64_t* row_ptr,
                                  uint32_t* col, float* val, unsigned int* flag);
 cudaError_t launch_onehot_fill(fmb200_ctx* c, cudaStream_t st, uint64_t n_rows, uint32_t z, uint64_t* row_ptr, float* val);
+// *out := max(*out, the largest id in col[0..nnz))
+cudaError_t launch_max_id(fmb200_ctx* c, cudaStream_t st, const uint32_t* col, uint64_t nnz, unsigned int* out);
+
+// fm_context.cu: a block of a .xt file (rows = features, ids = cases, the .x layout) into `slot`, decoded on
+// the device like a .x block; no targets.  _enqueue puts the copies and the decode on `st`; _finish waits for
+// them and fails (fmb200_last_error) naming column first_col + r when a header word disagrees with its size,
+// or when a case id is not below n_cases.
+int upload_xt_enqueue(fmb200_ctx* c, int slot, uint64_t n_cols, uint64_t nnz, const void* words,
+                      const uint32_t* col_size, cudaStream_t st);
+int upload_xt_finish(fmb200_ctx* c, int slot, uint64_t first_col, uint64_t n_cases);
 
 // pick the sub-warp geometry for a data set: G lanes per V row (power of two
 // covering kp/4 float4 chunks), S entry slots per row group, and the row-group

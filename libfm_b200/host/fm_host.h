@@ -195,8 +195,8 @@ class GpuLearner {
   }
 
   // slot 0 = the GPU's train shard (contiguous rows), slot 1 = test (GPU 0 only).  A data set given as
-  // blocks (one GPU, -method sgd) is not uploaded here: every pass over it streams its blocks through
-  // slots s and s + 2 (GpuSgdLearner::pass).
+  // blocks (one GPU; .x blocks for -method sgd, .xt blocks for mcmc | als) is not uploaded here: every pass
+  // over it streams its blocks through slots s and s + 2 (pass() here, or the library's MCMC passes).
   void attach(const SparseData& train, const SparseData& test, const BinaryBlocks* train_blocks = nullptr,
               const BinaryBlocks* test_blocks = nullptr) {
     const BinaryBlocks* blocks[2] = {train_blocks, test_blocks};
@@ -268,7 +268,84 @@ class GpuLearner {
   struct Streamed {
     const BinaryBlocks* data = nullptr;
     std::unique_ptr<BlockReader> reader;
+    std::string error;  // what the reader met while the library fetched a block (fetch_block)
   };
+
+  // One pass over the streamed data set `which` (0 train, 1 test) in file order: use(slot, block) once per
+  // block, in order.  Block b goes to slot which + 2 (b % 2) on the copy stream, so the copy of block b + 1
+  // runs while the work use() enqueued on block b does; use() waits for its block's upload itself (every
+  // call on a slot does).  Before block b + 1 overwrites block b - 1's slot, the work on b - 1 has run.
+  template <class F>
+  void pass(int which, F use) {
+    fmb200_ctx* const c = ctx_[0];
+    const std::vector<BinaryBlocks::Block>& blocks = streamed_[which].data->blocks;
+    BlockReader& rd = *streamed_[which].reader;
+    auto slot = [&](size_t b) { return which + 2 * (int)(b % 2); };
+    auto upload = [&](size_t b) {
+      const BlockReader::Buffer buf = rd.wait(b);
+      ck(fmb200_upload_xblock_async(c, slot(b), blocks[b].rows(), blocks[b].nnz, buf.x, buf.row_size, buf.target));
+    };
+    ck(fmb200_sync(c));  // the slots may hold blocks the previous pass still works on
+    rd.start();
+    upload(0);
+    for (size_t b = 0; b < blocks.size(); b++) {
+      if (b + 1 < blocks.size()) {
+        if (b > 0) ck(fmb200_sync(c));
+        upload(b + 1);
+      }
+      use(slot(b), blocks[b]);
+      rd.release(b);  // its upload has finished: use() waited for it
+    }
+    rd.stop();
+  }
+
+  // The library's view of a streamed .xt (train = 0, test = 1): its block plan, and its blocks fetched from the
+  // reader (page-locked buffers) through slots which + 2 and which + 4.  col_lo / nnz are filled here and must
+  // outlive the MCMC state.
+  fmb200_xt_blocks xt_blocks(int which, std::vector<uint32_t>& col_lo, std::vector<uint64_t>& nnz) {
+    const BinaryBlocks& d = *streamed_[which].data;
+    col_lo.clear();
+    nnz.clear();
+    for (const auto& b : d.blocks) {
+      col_lo.push_back((uint32_t)b.row_lo);
+      nnz.push_back(b.nnz);
+    }
+    col_lo.push_back((uint32_t)d.blocks.back().row_hi);
+    fmb200_xt_blocks x{};
+    x.n_cases = d.num_cases();
+    x.target = d.target.data();
+    x.n_blocks = d.blocks.size();
+    x.col_lo = col_lo.data();
+    x.nnz = nnz.data();
+    x.slot[0] = which + 2;
+    x.slot[1] = which + 4;
+    x.user = &streamed_[which];
+    x.fetch = fetch_block;
+    x.release = release_block;
+    return x;
+  }
+  static int fetch_block(void* user, uint64_t b, const void** words, const uint32_t** col_size) {
+    Streamed& s = *static_cast<Streamed*>(user);
+    try {
+      if (b == 0) s.reader->start();  // every pass reads the file from its start
+      const BlockReader::Buffer buf = s.reader->wait(b);
+      *words = buf.x;
+      *col_size = buf.row_size;
+      return 0;
+    } catch (const std::string& e) {
+      s.error = e;
+      return 1;
+    }
+  }
+  static void release_block(void* user, uint64_t b) { static_cast<Streamed*>(user)->reader->release(b); }
+  // ck() for calls that stream: the reader's own error, when it had one, says more than the library's
+  void ck_streamed(int rc) {
+    if (rc == 0) return;
+    for (const auto& s : streamed_)
+      if (!s.error.empty()) throw s.error;
+    ck(rc);
+  }
+
   // (its buffers are freed after ~GpuLearner has destroyed the contexts, which ends every copy from them)
   Streamed streamed_[2];
   std::vector<fmb200_ctx*> ctx_;
@@ -434,34 +511,6 @@ class GpuSgdLearner : public GpuLearner {
   }
 
  private:
-  // One pass over the streamed data set `which` (0 train, 1 test) in file order: use(slot, block) once per
-  // block, in order.  Block b goes to slot which + 2 (b % 2) on the copy stream, so the copy of block b + 1
-  // runs while the work use() enqueued on block b does; use() waits for its block's upload itself (every
-  // call on a slot does).  Before block b + 1 overwrites block b - 1's slot, the work on b - 1 has run.
-  template <class F>
-  void pass(int which, F use) {
-    fmb200_ctx* const c = ctx_[0];
-    const std::vector<BinaryBlocks::Block>& blocks = streamed_[which].data->blocks;
-    BlockReader& rd = *streamed_[which].reader;
-    auto slot = [&](size_t b) { return which + 2 * (int)(b % 2); };
-    auto upload = [&](size_t b) {
-      const BlockReader::Buffer buf = rd.wait(b);
-      ck(fmb200_upload_xblock_async(c, slot(b), blocks[b].rows(), blocks[b].nnz, buf.x, buf.row_size, buf.target));
-    };
-    ck(fmb200_sync(c));  // the slots may hold blocks the previous pass still works on
-    rd.start();
-    upload(0);
-    for (size_t b = 0; b < blocks.size(); b++) {
-      if (b + 1 < blocks.size()) {
-        if (b > 0) ck(fmb200_sync(c));
-        upload(b + 1);
-      }
-      use(slot(b), blocks[b]);
-      rd.release(b);  // its upload has finished: use() waited for it
-    }
-    rd.stop();
-  }
-
 #ifdef FMB200_WITH_NCCL
   std::vector<ncclComm_t> comms_;
 #endif
@@ -500,14 +549,25 @@ class GpuMcmcLearner : public GpuLearner {
   }
 
   // after attach(): test is the set in slot 1, its targets score the predictions
-  void learn(const SparseData& test) {
+  // test_target: the targets of the test set (resident or streamed)
+  void learn(const std::vector<float>& test) {
     push_state(0.0);
     fmb200_ctx* const ctx = ctx_[0];
     const uint32_t G = (uint32_t)attr_per_group.size();
     const int k = fm->num_factor;
-    ck(fmb200_mcmc_begin(ctx, 0, 1, do_sample, do_multilevel, G, attr_group.data(), attr_per_group.data(),
-                         fm->reg0, w_lambda.data(), v_lambda.data()));
-    const uint64_t nt = test.num_cases();
+    if (streamed_[0].data || streamed_[1].data) {  // a set larger than -cache_size streams from its .xt
+      fmb200_xt_blocks xt[2];
+      for (int i = 0; i < 2; i++)
+        if (streamed_[i].data) xt[i] = xt_blocks(i, xt_col_lo_[i], xt_nnz_[i]);
+      ck_streamed(fmb200_mcmc_begin_xt(ctx, 0, streamed_[0].data ? &xt[0] : nullptr, 1,
+                                       streamed_[1].data ? &xt[1] : nullptr, do_sample, do_multilevel, G,
+                                       attr_group.data(), attr_per_group.data(), fm->reg0, w_lambda.data(),
+                                       v_lambda.data()));
+    } else {
+      ck(fmb200_mcmc_begin(ctx, 0, 1, do_sample, do_multilevel, G, attr_group.data(), attr_per_group.data(),
+                           fm->reg0, w_lambda.data(), v_lambda.data()));
+    }
+    const uint64_t nt = test.size();
     pred_this_.assign(nt, 0.0);
     pred_all_.assign(nt, 0.0);
     std::vector<double> but5(nt), w_mu(G), wl(G), v_mu((size_t)G * k), vl((size_t)G * k);
@@ -518,7 +578,7 @@ class GpuMcmcLearner : public GpuLearner {
       const auto w0 = std::chrono::steady_clock::now();
       double train_metric = 0;
       uint32_t cnt[16];
-      ck(fmb200_mcmc_iteration(ctx, &train_metric, cnt));
+      ck_streamed(fmb200_mcmc_iteration(ctx, &train_metric, cnt));
       for (int p = 0; p < 8; p++)  // fm_learn_mcmc_simultaneous.h:96-119
         if (cnt[2 * p] > 0 || cnt[2 * p + 1] > 0)
           std::cout << "#nans in " << cnt_names[p] << ":\t" << cnt[2 * p] << "\t#inf_in_" << cnt_names[p] << ":\t"
@@ -592,14 +652,14 @@ class GpuMcmcLearner : public GpuLearner {
 
  private:
   // fm_learn_mcmc_simultaneous::_evaluate / _evaluate_class (:272-309) over all test cases
-  void eval_reg(const std::vector<double>& pred, const SparseData& t, double norm, double* rmse, double* mae) const {
+  void eval_reg(const std::vector<double>& pred, const std::vector<float>& t, double norm, double* rmse, double* mae) const {
     double r = 0, m = 0;
     uint32_t n = 0;
     for (size_t c = 0; c < pred.size(); c++) {
       double p = pred[c] * norm;
       p = std::min(max_target, p);
       p = std::max(min_target, p);
-      const double err = p - t.target[c];
+      const double err = p - t[c];
       r += err * err;
       m += std::abs((double)err);
       n++;
@@ -607,13 +667,13 @@ class GpuMcmcLearner : public GpuLearner {
     *rmse = std::sqrt(r / n);
     *mae = m / n;
   }
-  void eval_cls(const std::vector<double>& pred, const SparseData& t, double norm, double* acc, double* ll) const {
+  void eval_cls(const std::vector<double>& pred, const std::vector<float>& t, double norm, double* acc, double* ll) const {
     double l = 0.0;
     uint32_t a = 0, n = 0;
     for (size_t c = 0; c < pred.size(); c++) {
       const double p = pred[c] * norm;
-      if (((p >= 0.5) && (t.target[c] > 0.0)) || ((p < 0.5) && (t.target[c] < 0.0))) a++;
-      const double m = (t.target[c] + 1.0) * 0.5;
+      if (((p >= 0.5) && (t[c] > 0.0)) || ((p < 0.5) && (t[c] < 0.0))) a++;
+      const double m = (t[c] + 1.0) * 0.5;
       double pll = p;
       if (pll > 0.99) pll = 0.99;
       if (pll < 0.01) pll = 0.01;
@@ -628,6 +688,8 @@ class GpuMcmcLearner : public GpuLearner {
   static constexpr const char* cls_fields_[6] = {"acc_mcmc_this", "acc_mcmc_all", "acc_mcmc_all_but5",
                                                  "ll_mcmc_this",  "ll_mcmc_all",  "ll_mcmc_all_but5"};
   std::vector<double> pred_this_, pred_all_;
+  std::vector<uint32_t> xt_col_lo_[2];
+  std::vector<uint64_t> xt_nnz_[2];
 };
 
 }  // namespace host

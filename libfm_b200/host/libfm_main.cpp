@@ -5,8 +5,8 @@
 // passes over the data run in libfmb200 (include/fmb200.h).  `-method sgd` runs in every mode;
 // `-method mcmc|als` (data sets without relations, one GPU) run with -mode inorder or ordered, the
 // fp64 state; sgda is refused with a clear error instead of silently doing something else.
-// -cache_size streams a binary data set larger than it through the GPU block by block (-method sgd, one
-// GPU); every other method, and text input, loads the data whole, as before.
+// -cache_size streams a binary data set larger than it through the GPU block by block (one GPU): -method sgd
+// its .x, -method mcmc|als its transposed .xt (as the reference's data_t); text input loads the data whole.
 //
 // New, optional flags (old command lines are unaffected):
 //   -mode hogwild|ordered|inorder   throughput (default); sequentially consistent fp64 (parallel over
@@ -63,12 +63,16 @@ static int run(const CmdLine& cmd, const std::string& method, std::chrono::stead
   };
 
   // (1) data, libfm.cpp:141-157.  -cache_size (bytes; 0 or absent: everything resident, the reference's
-  // unlimited): with -method sgd on one GPU, a binary data set whose rows exceed one block of cache_size / 2
-  // bytes is read and trained on block by block (BinaryBlocks); text input ignores it, as in the reference.
-  const long long cache_size = sgd && cmd.integer("gpus", 1) == 1 ? cmd.integer64("cache_size", 0) : 0;
+  // unlimited), on one GPU: with -method sgd, a binary data set whose rows exceed one block of cache_size / 2
+  // bytes is read and trained on block by block (BinaryBlocks); with -method mcmc | als, one whose transposed
+  // file <file>.xt exists and whose columns exceed such a block is streamed from .xt and .y alone, .x unread
+  // (BinaryBlocks::open_xt; MCMC and ALS run in -mode inorder | ordered on one GPU, checked before loading).
+  // Train and test decide independently.  Text input ignores the flag, as in the reference.
+  const long long cache_size = cmd.integer("gpus", 1) == 1 ? cmd.integer64("cache_size", 0) : 0;
   auto load = [&](const std::string& file, SparseData& d) {
     std::unique_ptr<BinaryBlocks> b;
-    if (cache_size > 0) b = BinaryBlocks::open(file, (uint64_t)cache_size);
+    if (cache_size > 0)
+      b = sgd ? BinaryBlocks::open(file, (uint64_t)cache_size) : BinaryBlocks::open_xt(file, (uint64_t)cache_size);
     if (b) b->print();
     else d.load(file);
     return b;
@@ -235,7 +239,7 @@ static int run(const CmdLine& cmd, const std::string& method, std::chrono::stead
                 << std::endl;
     std::cout << "Final\t" << "Train=" << fml.evaluate(0) << "\tTest=" << fml.evaluate(1) << std::endl;
   } else {
-    fml.learn(test);  // no Final line for MCMC / ALS (:417-420)
+    fml.learn(test_blocks ? test_blocks->target : test.target);  // no Final line for MCMC / ALS (:417-420)
   }
 
   // -out, libfm.cpp:422-428 (DVector::save: one value per line, matrix.h:332-342)
