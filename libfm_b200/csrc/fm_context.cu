@@ -766,6 +766,11 @@ int fmb200_sgda_begin(fmb200_ctx* c, uint32_t n_groups, const uint32_t* attr_gro
   if (need_fp64(c, "SGDA runs on the fp64 state: set INORDER or ORDERED mode first")) return 1;
   if (n_groups == 0 || n_groups > 1024) return fail("n_groups must be in [1,1024]");
   if (n_groups > 1 && !attr_group) return fail("attr_group is required for more than one group");
+  if (sgda_smem_bytes(n_groups, c->k) > (size_t)c->max_smem_optin)
+    return fail("SGDA with %u groups at num_factor = %d needs %zu bytes of shared memory per block (8 * groups * "
+                "(2 + 3 * num_factor)); this device allows %d: use at most %zu groups",
+                n_groups, c->k, sgda_smem_bytes(n_groups, c->k), c->max_smem_optin,
+                (size_t)c->max_smem_optin / sgda_smem_bytes(1, c->k));
   if (attr_group)
     for (uint32_t i = 0; i < c->n; i++)
       if (attr_group[i] >= n_groups) return fail("attr_group[%u] = %u >= n_groups", i, attr_group[i]);

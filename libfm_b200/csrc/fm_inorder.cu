@@ -497,8 +497,8 @@ cudaError_t launch_sgda_epoch(fmb200_ctx* c, const DataSlot& tr, const DataSlot&
   a.v_col = va.col.get();
   a.v_val = va.val.get();
   a.v_target = va.target.get();
-  const size_t smem = sizeof(double) * ((size_t)c->sgda_groups * (2 + 3 * (size_t)c->k));
-  if (smem > (size_t)c->max_smem_optin) return cudaErrorInvalidConfiguration;
+  const size_t smem = sgda_smem_bytes(c->sgda_groups, c->k);
+  if (smem > (size_t)c->max_smem_optin) return cudaErrorInvalidConfiguration;  // fmb200_sgda_begin refuses it
   const cudaError_t e = with_kf(c->k, [&](auto kf) {
     auto kernel = fm_sgda_epoch_kernel<decltype(kf)::value>;
     const cudaError_t e_ = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -306,7 +306,11 @@ std::string mcmc_begin(fmb200_ctx* c, int train, int test, int do_sample, int do
 std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counters);
 bool mcmc_get(const fmb200_ctx* c, double* alpha, double* w_mu, double* w_lambda, double* v_mu, double* v_lambda,
               double* pred_this, double* pred_sum_all, double* pred_sum_all_but5, uint32_t* n_runs);
-// fm_inorder.cu: one SGDA epoch (theta-step per training row, lambda-step per validation row)
+// fm_inorder.cu: one SGDA epoch (theta-step per training row, lambda-step per validation row).  Its
+// per-group state lives in dynamic shared memory: reg_w[G] | reg_v[G][k] | sum_f[G][k] | sum_f_dash_f[G][k] | lwg[G]
+inline size_t sgda_smem_bytes(uint32_t n_groups, int k) {
+  return sizeof(double) * ((size_t)n_groups * (2 + 3 * (size_t)k));
+}
 cudaError_t launch_sgda_epoch(fmb200_ctx* c, const DataSlot& tr, const DataSlot& va, int lambda_steps);
 // fm_hogwild.cu: throughput epoch
 cudaError_t launch_sgd_hogwild(fmb200_ctx* c, DataSlot& d);
