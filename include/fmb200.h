@@ -216,11 +216,17 @@ int fmb200_mcmc_runs(fmb200_ctx* ctx, uint32_t* n_runs);
  *  _epoch: one pass of :295-311 -- a theta-step (:136-169) per training row, each followed, when
  *          lambda_steps != 0 (the reference skips them in its first epoch, :301), by a lambda-step
  *          (:201-248) on the next validation row, the cursor restarting per epoch and wrapping.
- *          Sequential semantics, fp64, bit-identical to the reference (one warp: a parity path).
- *  _get_reg: reg_w[n_groups], reg_v[n_groups][num_factor]. */
+ *          Sequential semantics, fp64, bit-identical to the reference (one warp; for num_factor <= 8
+ *          and rows of at most 4 entries a wavefront of conflict-free steps, fmb200_set_tuning
+ *          variant 1 forcing the one-warp kernel).
+ *  _get_reg: reg_w[n_groups], reg_v[n_groups][num_factor].
+ *  _get_moments: var_w and var_v[num_factor] of the last epoch's last update_means (:250-274), taken
+ *          at the epoch's start or, when the validation cursor restarts, before the last restart's
+ *          lambda-step; the means the reference logs with them are always 0 (:270-273). */
 int fmb200_sgda_begin(fmb200_ctx* ctx, uint32_t n_groups, const uint32_t* attr_group);
 int fmb200_sgda_epoch(fmb200_ctx* ctx, int train_slot, int val_slot, int lambda_steps, double* device_seconds);
 int fmb200_sgda_get_reg(fmb200_ctx* ctx, double* reg_w, double* reg_v);
+int fmb200_sgda_get_moments(fmb200_ctx* ctx, double* var_w, double* var_v);
 
 /* Multi-GPU plumbing (row sharding + one all-reduce of w0|w|V per epoch; the
  * reference has no equivalent).  The HOGWILD state is one packed fp32 device

@@ -57,6 +57,7 @@ SYMBOLS = {
     "fmb200_sgda_begin": (C.c_int, [_ctx, C.c_uint32, _u32p]),
     "fmb200_sgda_epoch": (C.c_int, [_ctx, C.c_int, C.c_int, C.c_int, _f64p]),
     "fmb200_sgda_get_reg": (C.c_int, [_ctx, _f64p, _f64p]),
+    "fmb200_sgda_get_moments": (C.c_int, [_ctx, _f64p, _f64p]),
     "fmb200_mcmc_eterms": (C.c_int, [_ctx, C.c_int, _f64p]),
     "fmb200_mcmc_begin": (C.c_int, [_ctx, C.c_int, C.c_int, C.c_int, C.c_int, C.c_uint32, _u32p, _u32p, C.c_double,
                                     _f64p, _f64p]),

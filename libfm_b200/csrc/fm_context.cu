@@ -780,7 +780,9 @@ int fmb200_sgda_begin(fmb200_ctx* c, uint32_t n_groups, const uint32_t* attr_gro
     CK(alloc(c->sgda_grad_w, n1));
     CK(alloc(c->sgda_grad_v, nk));
     CK(alloc(c->sgda_group, n1));
+    CK(alloc(c->sgda_moments, 1 + (size_t)c->k));
   }
+  c->sgda_moments_ready = false;
   if (c->sgda_groups != n_groups) {
     c->sgda_groups = 0;
     CK(alloc(c->sgda_reg_w, n_groups));
@@ -807,8 +809,22 @@ int fmb200_sgda_epoch(fmb200_ctx* c, int train_slot, int val_slot, int lambda_st
   if (c->sgda_groups == 0) return fail("call fmb200_sgda_begin first");
   return timed(c, device_seconds, [&]() -> int {
     CK(launch_sgda_epoch(c, c->slots[train_slot], c->slots[val_slot], lambda_steps));
+    c->sgda_moments_ready = true;
     return 0;
   });
+}
+
+int fmb200_sgda_get_moments(fmb200_ctx* c, double* var_w, double* var_v) {
+  NEED_CTX(c);
+  if (bind(c)) return 1;
+  if (c->sgda_groups == 0) return fail("call fmb200_sgda_begin first");
+  if (!c->sgda_moments_ready) return fail("no SGDA epoch has run since fmb200_sgda_begin");
+  if (var_w) CK(cudaMemcpyAsync(var_w, c->sgda_moments.get(), sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  if (var_v && c->k)
+    CK(cudaMemcpyAsync(var_v, c->sgda_moments.get() + 1, (size_t)c->k * sizeof(double), cudaMemcpyDeviceToHost,
+                       c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  return 0;
 }
 
 int fmb200_sgda_get_reg(fmb200_ctx* c, double* reg_w, double* reg_v) {

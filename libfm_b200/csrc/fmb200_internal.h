@@ -263,6 +263,8 @@ struct fmb200_ctx {
   uint64_t upload_counter = 0;          // generations handed out to uploads
   // SGDA state (fm_learn_sgd_element_adapt_reg.h): stored gradients, per-group regularisation
   fmb::DevPtr<double> sgda_grad_w, sgda_grad_v, sgda_reg_w, sgda_reg_v;
+  fmb::DevPtr<double> sgda_moments;  // var_w | var_v[k] of the last epoch's last update_means
+  bool sgda_moments_ready = false;   // an epoch has run since fmb200_sgda_begin
   fmb::DevPtr<uint32_t> sgda_group;
   uint32_t sgda_groups = 0;
   int tune_damp = 0;  // 0 auto, 1 force on, -1 force off
@@ -310,6 +312,13 @@ bool mcmc_get(const fmb200_ctx* c, double* alpha, double* w_mu, double* w_lambda
 // per-group state lives in dynamic shared memory: reg_w[G] | reg_v[G][k] | sum_f[G][k] | sum_f_dash_f[G][k] | lwg[G]
 inline size_t sgda_smem_bytes(uint32_t n_groups, int k) {
   return sizeof(double) * ((size_t)n_groups * (2 + 3 * (size_t)k));
+}
+// The step t* whose lambda-step follows the epoch's last update_means (:298, :302-307), 0 when that call
+// is the one at the epoch's start: the cursor over V validation rows restarts before the lambda-steps
+// t = V, 2V, ... of an epoch of N theta-steps.
+inline uint64_t sgda_last_moments_step(uint64_t n_train, uint64_t n_val, bool lambda_steps) {
+  if (!lambda_steps || n_val == 0 || n_train <= n_val) return 0;
+  return (n_train - 1) / n_val * n_val;
 }
 cudaError_t launch_sgda_epoch(fmb200_ctx* c, const DataSlot& tr, const DataSlot& va, int lambda_steps);
 // fm_hogwild.cu: throughput epoch

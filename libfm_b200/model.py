@@ -487,6 +487,14 @@ class FmLearnSgdElement:
         self._check(self.lib.fmb200_sgda_get_reg(self._ctx, _p(reg_w, C.c_double), _p(reg_v, C.c_double)))
         return reg_w, reg_v
 
+    def sgda_moments(self):
+        """var_w and var_v[k] of the last epoch's last update_means (fm_learn_sgd_element_adapt_reg.h:250-274),
+        the wvar / vvar<f> columns of the reference's rlog (its wmean / vmean<f> are always 0)."""
+        var_w = C.c_double()
+        var_v = np.zeros(self.fm.num_factor)
+        self._check(self.lib.fmb200_sgda_get_moments(self._ctx, C.byref(var_w), _p(var_v, C.c_double)))
+        return var_w.value, var_v
+
     def mcmc_eterms(self, data: Data) -> np.ndarray:
         """fm_learn_mcmc::predict_data_and_write_to_eterms (fm_learn_mcmc.h:148-378) for one data set."""
         out = np.empty(data.num_cases, dtype=np.float64)
