@@ -18,6 +18,7 @@
 #include "fm_device.cuh"
 #include "fmb200_internal.h"
 #include "fm_inorder_wavefront.cuh"
+#include "fm_loss.cuh"
 #include "fm_roworder.cuh"
 #include "fm_sgda_wavefront.cuh"
 
@@ -116,12 +117,6 @@ __device__ __forceinline__ double predict_row_exact(const RowCtx& m, double w0,
   return predict_row_exact<KF, true>(
       m, w0, col, val, size, sum, lane, [&](uint32_t id) { return m.w[id]; },
       [&](uint32_t id, int f) { return m.v[(size_t)id * m.k + f]; });
-}
-
-// d loss / d score of the SGD learner (fm_learn_sgd_element.h:58-65); clamp_target: fm_sgda_wavefront.cuh
-__device__ __forceinline__ double sgd_mult(const HParams& hp, double p, double y) {
-  if (hp.task == FMB200_TASK_REGRESSION) return -(y - clamp_target(p, hp));
-  return -y * (1.0 - 1.0 / (1.0 + exp(-y * p)));
 }
 
 template <int KF>
@@ -494,7 +489,7 @@ cudaError_t launch_sgda_epoch(fmb200_ctx* c, const DataSlot& tr, const DataSlot&
   const bool lam = lambda_steps && va.n_rows > 0;
   const size_t wf_smem = sizeof(double) * (size_t)c->sgda_groups * (1 + (size_t)c->k);
   const bool wavefront = c->tune_variant != 1 &&
-                         sgda_wavefront_eligible(c->k, tr.max_row_nnz, lam ? va.max_row_nnz : 0) &&
+                         wavefront_fits(c->k, tr.max_row_nnz) && (!lam || wavefront_fits(c->k, va.max_row_nnz)) &&
                          sizeof(SgdaWindow) + wf_smem <= (size_t)c->max_smem_optin;
   const size_t smem = wavefront ? wf_smem : sgda_smem_bytes(c->sgda_groups, c->k);
   if (smem > (size_t)c->max_smem_optin) return cudaErrorInvalidConfiguration;  // fmb200_sgda_begin refuses it
@@ -537,8 +532,8 @@ cudaError_t launch_sgda_epoch(fmb200_ctx* c, const DataSlot& tr, const DataSlot&
              (e = run(2 * t_star + 1, 2 * N, V)) != cudaSuccess) {
     return e;
   }
-  c->last_cfg = wavefront ? EpochConfig{32, WF_Z, 32, 1, 32, (int)(sizeof(SgdaWindow) + smem), 0}
-                          : EpochConfig{32, 1, 1, 1, 32, (int)smem, 0};
+  c->last_cfg =
+      wavefront ? wavefront_config((int)(sizeof(SgdaWindow) + smem)) : EpochConfig{32, 1, 1, 1, 32, (int)smem, 0};
   return cudaSuccess;
 }
 
@@ -546,7 +541,7 @@ cudaError_t launch_sgd_inorder(fmb200_ctx* c, const DataSlot& d) {
   // The wavefront schedule (k <= 8, rows of <= 4 entries) is the default for eligible shapes:
   // bit-identical to the row-at-a-time kernel on the device (tests/test_wavefront_gpu.py, r02) and
   // 6.7x faster on C2 (0.210 s vs 1.416 s per epoch).  variant 1 forces the row-at-a-time kernel.
-  if (c->tune_variant != 1 && c->k <= WF_K && d.max_row_nnz <= (uint32_t)WF_Z && d.n_rows > 0) {
+  if (c->tune_variant != 1 && wavefront_fits(c->k, d.max_row_nnz) && d.n_rows > 0) {
 #define FMB_WAVEFRONT(K0, TASK)                                                                       \
   fm_sgd_inorder_wavefront_kernel<K0, TASK><<<1, 32, 0, c->stream>>>(c->p64, c->k, c->k0, c->k1, c->hp, \
                                                                      d.n_rows, d.row_ptr.get(), d.col.get(),  \
@@ -558,7 +553,7 @@ cudaError_t launch_sgd_inorder(fmb200_ctx* c, const DataSlot& d) {
     else FMB_WAVEFRONT(false, FMB200_TASK_CLASSIFICATION);
 #undef FMB_WAVEFRONT
     c->launches++;
-    c->last_cfg = EpochConfig{32, WF_Z, 32, 1, 32, 0};
+    c->last_cfg = wavefront_config(0);
     return cudaGetLastError();
   }
   const cudaError_t e = with_kf(c->k, [&](auto kf) {

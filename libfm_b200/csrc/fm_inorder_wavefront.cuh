@@ -1,9 +1,11 @@
-// fm_inorder_wavefront.cuh -- the wavefront schedule of the sequential-equivalent epoch.
-// Included by fm_inorder.cu (compiled with --fmad=false).  Kept in a header of its own so
-// that tests/simt/ can compile this exact source for the host and run it as 32 threads
-// (one per lane, barriers where the kernel synchronises) against the oracle and under
-// ThreadSanitizer.
+// fm_inorder_wavefront.cuh -- the wavefront schedule of the sequential-equivalent epochs: the
+// window pieces both wavefront kernels are built from, and the SGD epoch (the SGDA epoch is in
+// fm_sgda_wavefront.cuh).  Included by fm_inorder.cu (compiled with --fmad=false).  Kept in
+// headers of their own so that tests/simt/ can compile this exact source for the host and run it
+// as 32 threads (one per lane, barriers where the kernel synchronises) against the oracle and
+// under ThreadSanitizer.
 #pragma once
+#include "fm_loss.cuh"
 #include "fmb200_internal.h"
 
 namespace fmb {
@@ -22,25 +24,195 @@ namespace fmb {
 // in parallel, run the scalar chain one after the other, and scatter their updates in
 // parallel, with every rounding identical to the sequential loop.
 //
-// One warp, lane = example.  Per step:
-//   1. the next 32 examples load their entries; a shared-memory hash table finds the
-//      longest prefix P in which no example touches a feature of an earlier one (hash
-//      collisions only shorten P -- conservative);
-//   2. lanes < P gather w / V rows (fp64) and form their addends into shared memory;
+// One warp, lane = example.  Per window:
+//   1. the next 32 examples load their entries (WfRow); a shared-memory hash table (WfHash)
+//      finds the longest prefix P in which no example touches a feature of an earlier one
+//      (hash collisions only shorten P -- conservative);
+//   2. lanes < P gather w / V rows (fp64) and form their addends into shared memory (WfGather);
 //   3. all lanes walk the chain t = 0..P-1 redundantly from shared memory (broadcast
 //      reads, software-prefetched one example ahead): about nnz + k + 6 dependent fp64
 //      operations per example, the only serial part left;
-//   4. lanes < P apply fm_SGD to their own rows (cached values; a row that names the
-//      same feature twice re-reads memory so the second update sees the first).
-// The next step starts at example base + P.
+//   4. lanes < P apply fm_SGD to their own rows (WfGather::scatter: cached values; a row that
+//      names the same feature twice re-reads memory so the second update sees the first).
+// The next window starts at example base + P.
 constexpr int WF_Z = 4;        // entries per row
 constexpr int WF_K = 8;        // factors
 constexpr int WF_HASH = 2048;  // hash slots (power of two)
+
+// the shapes a wavefront kernel takes: k <= WF_K and rows of at most WF_Z entries
+inline bool wavefront_fits(int k, uint32_t max_row_nnz) { return k <= WF_K && max_row_nnz <= (uint32_t)WF_Z; }
+
+// what a wavefront epoch reports (fmb200_get_epoch_config): one warp, lane = row
+inline EpochConfig wavefront_config(int smem) { return EpochConfig{32, WF_Z, 32, 1, 32, smem, 0}; }
 
 __device__ __forceinline__ uint32_t wf_hash(uint32_t id) {
   return (id * 2654435761u) >> (32 - 11);
 }
 static_assert(WF_HASH == (1 << 11), "wf_hash produces 11 bits");
+
+// A CSR row of at most WF_Z (id, value) entries in registers; unused slots hold (0, 0).
+struct WfRow {
+  int size;
+  uint32_t id[WF_Z];
+  float x[WF_Z];
+
+  // entries [beg, end) of the CSR (beg == end: an empty row)
+  __device__ __forceinline__ void load(const uint32_t* __restrict__ col, const float* __restrict__ val,
+                                       uint64_t beg, uint64_t end) {
+    size = (int)(end - beg);
+#pragma unroll
+    for (int j = 0; j < WF_Z; j++) {
+      id[j] = 0;
+      x[j] = 0.f;
+      if (j < size) {
+        id[j] = col[beg + j];
+        x[j] = val[beg + j];
+      }
+    }
+  }
+
+  __device__ __forceinline__ bool names_a_feature_twice() const {
+    bool dup = false;
+#pragma unroll
+    for (int j = 1; j < WF_Z; j++)
+#pragma unroll
+      for (int j2 = 0; j2 < j; j2++)
+        if (j < size && id[j] == id[j2]) dup = true;
+    return dup;
+  }
+};
+
+// The window's conflict table: WF_HASH slots of shared memory.  Slot wf_hash(id) holds
+// (seq << 5) | (31 - lane) of the lowest lane of window seq whose marked row has feature id
+// (atomicMax: the larger tag is the later window, then the lower lane).
+struct WfHash {
+  unsigned int* slot;
+  unsigned int seq;
+  unsigned int tag;  // this lane's tag in the current window
+
+  // clears the table; the caller synchronises the warp before the first window
+  __device__ __forceinline__ WfHash(unsigned int* s, int lane) : slot(s), seq(0), tag(0) { clear(lane); }
+
+  __device__ __forceinline__ void clear(int lane) {
+    for (int i = lane; i < WF_HASH; i += 32) slot[i] = 0;
+  }
+
+  // every lane, once per window
+  __device__ __forceinline__ void next_window(int lane) {
+    if (++seq == (1u << 27)) {  // window counter about to leave its 27 bits: start over
+      clear(lane);
+      seq = 1;
+      __syncwarp();
+    }
+    tag = (seq << 5) | (unsigned int)(31 - lane);
+  }
+
+  // every lane marks its row's features; returns when all marks are in
+  __device__ __forceinline__ void mark(const WfRow& r) {
+#pragma unroll
+    for (int j = 0; j < WF_Z; j++)
+      if (j < r.size) atomicMax(&slot[wf_hash(r.id[j])], tag);
+    __syncwarp();
+  }
+
+  // an earlier lane's row has one of the features of r, this lane's marked row (whose slots
+  // therefore hold tags of this window)
+  __device__ __forceinline__ bool earlier_has(const WfRow& r, int lane) const {
+    bool hit = false;
+#pragma unroll
+    for (int j = 0; j < WF_Z; j++)
+      if (j < r.size) {
+        const unsigned int h = slot[wf_hash(r.id[j])];
+        if (31 - (int)(h & 31u) < lane) hit = true;
+      }
+    return hit;
+  }
+
+  // this lane's or an earlier lane's marked row has one of the features of r, an unmarked row
+  __device__ __forceinline__ bool this_or_earlier_has(const WfRow& r, int lane) const {
+    bool hit = false;
+#pragma unroll
+    for (int j = 0; j < WF_Z; j++)
+      if (j < r.size) {
+        const unsigned int h = slot[wf_hash(r.id[j])];
+        if ((h >> 5) == seq && 31 - (int)(h & 31u) <= lane) hit = true;
+      }
+    return hit;
+  }
+};
+
+// P, the window's conflict-free prefix: the lanes before the first whose stop is set (32 if none)
+__device__ __forceinline__ int wf_prefix(bool stop) {
+  const unsigned m = __ballot_sync(0xffffffffu, stop);
+  return m ? __ffs(m) - 1 : 32;
+}
+
+// A row's w and V as the window's start left them, its score's addends, and the scatter of its
+// updates.
+struct WfGather {
+  double wv[WF_Z], vv[WF_Z][WF_K], sum[WF_K];
+
+  __device__ __forceinline__ void gather(const WfRow& r, const double* w, const double* v, int k, bool k1) {
+#pragma unroll
+    for (int j = 0; j < WF_Z; j++) {
+      wv[j] = 0;
+      if (j < r.size && k1) wv[j] = w[r.id[j]];
+#pragma unroll
+      for (int f = 0; f < WF_K; f++) {
+        vv[j][f] = 0;
+        if (j < r.size && f < k) vv[j][f] = v[(size_t)r.id[j] * k + f];
+      }
+    }
+  }
+
+  // add[WF_Z + WF_K] (fm_model.h:107-121): a_i = w_i x_i, then b_f = 0.5 (sum_f^2 - sumsq_f)
+  // with sum_f = ((0 + d_0) + d_1) + ..., kept for the update.  Unused slots hold -0.0, the
+  // exact identity of IEEE addition (x + -0.0 == x for every x, signed zeros included), so a
+  // chain adds all WF_Z + WF_K of them without a select.
+  __device__ __forceinline__ void addends(const WfRow& r, int k, bool k1, double* add) {
+#pragma unroll
+    for (int j = 0; j < WF_Z; j++) add[j] = (j < r.size && k1) ? wv[j] * (double)r.x[j] : -0.0;
+#pragma unroll
+    for (int f = 0; f < WF_K; f++) {
+      double sf = 0, ss = 0;
+#pragma unroll
+      for (int j = 0; j < WF_Z; j++)
+        if (j < r.size) {
+          const double d = vv[j][f] * (double)r.x[j];
+          sf += d;
+          ss += d * d;
+        }
+      sum[f] = sf;
+      add[WF_Z + f] = (f < k) ? 0.5 * (sf * sf - ss) : -0.0;
+    }
+  }
+
+  // The row's updates in fm_sgd.h:38-50's order: the w entries, then V factor by factor.  The
+  // rule maps the current value c to the new one: upd_w(j, at, c) for w[at], upd_v(j, f, at, c)
+  // for v[at], at = id_j * k + f.  c is the gathered value, or, when the row names a feature
+  // twice, re-read from memory so that the second update sees the first.
+  template <class UpdW, class UpdV>
+  __device__ __forceinline__ void scatter(const WfRow& r, bool dup, double* w, double* v, int k, bool k1,
+                                          UpdW upd_w, UpdV upd_v) const {
+    if (k1)
+#pragma unroll
+      for (int j = 0; j < WF_Z; j++)
+        if (j < r.size) {
+          double* c = &w[r.id[j]];
+          *c = upd_w(j, r.id[j], dup ? *c : wv[j]);
+        }
+#pragma unroll
+    for (int f = 0; f < WF_K; f++)
+      if (f < k)
+#pragma unroll
+        for (int j = 0; j < WF_Z; j++)
+          if (j < r.size) {
+            const size_t at = (size_t)r.id[j] * k + f;
+            double* c = &v[at];
+            *c = upd_v(j, f, at, dup ? *c : vv[j][f]);
+          }
+  }
+};
 
 template <bool K0, int TASK>
 __global__ void __launch_bounds__(32, 1)
@@ -52,10 +224,9 @@ __global__ void __launch_bounds__(32, 1)
   constexpr int NA = WF_Z + WF_K;  // addends per example
   __shared__ __align__(16) double s_add[32][NA];
   __shared__ float s_y[32];
-  __shared__ unsigned int s_hash[WF_HASH];  // (step << 5) | (31 - lane): max = current step, lowest lane
+  __shared__ unsigned int s_hash[WF_HASH];
 
   const int lane = threadIdx.x;
-  const unsigned full = 0xffffffffu;
   const int k = n_factor;
   constexpr bool k0 = K0;
   const bool k1 = use_w != 0;
@@ -64,83 +235,40 @@ __global__ void __launch_bounds__(32, 1)
   double w0 = k0 ? *p.w0() : 0.0;
   const double lr = hp.lr, reg0 = hp.reg0, regw = hp.regw, regv = hp.regv;
 
-  const bool clamp_inverted = hp.max_target < hp.min_target;  // degenerate bounds: still fmin-then-fmax
-
-  for (int i = lane; i < WF_HASH; i += 32) s_hash[i] = 0;
+  WfHash hash(s_hash, lane);
   __syncwarp();
 
-  unsigned int seq = 0;
   uint64_t base = 0;
-  // Row bounds, targets and entries of the coming step are fetched one step ahead (the
-  // loads are in flight while the chain of the current step runs).
-  uint64_t beg = 0, end = 0;
+  // Row bounds, targets and entries of the coming window are fetched one window ahead (the
+  // loads are in flight while the chain of the current window runs).
+  WfRow row;
   float yf = 0.f;
-  uint32_t id[WF_Z];
-  float xf[WF_Z];
-  if (lane < n_rows) {
-    beg = row_ptr[lane];
-    end = row_ptr[lane + 1];
-    yf = target[lane];
-  }
-#pragma unroll
-  for (int j = 0; j < WF_Z; j++) {
-    id[j] = 0;
-    xf[j] = 0.f;
-    if (j < (int)(end - beg)) {
-      id[j] = col[beg + j];
-      xf[j] = val[beg + j];
+  {
+    uint64_t beg = 0, end = 0;
+    if (lane < n_rows) {
+      beg = row_ptr[lane];
+      end = row_ptr[lane + 1];
+      yf = target[lane];
     }
+    row.load(col, val, beg, end);
   }
 
   while (base < n_rows) {
-    const bool valid = base + lane < n_rows;
-    const int size = valid ? (int)(end - beg) : 0;
-    double x[WF_Z];
-#pragma unroll
-    for (int j = 0; j < WF_Z; j++) x[j] = (double)xf[j];
     // (1) conflict-free prefix
-    bool dup = false;
+    const bool valid = base + lane < n_rows;  // an invalid lane's row is empty
+    double x[WF_Z];  // converted once per window: the scatter reads each value k + 1 times
 #pragma unroll
-    for (int j = 1; j < WF_Z; j++)
-#pragma unroll
-      for (int j2 = 0; j2 < j; j2++)
-        if (j < size && id[j] == id[j2]) dup = true;
-    if (++seq == (1u << 27)) {  // step counter about to leave its 27 bits: start over
-      for (int i = lane; i < WF_HASH; i += 32) s_hash[i] = 0;
-      seq = 1;
-      __syncwarp();
-    }
-    const unsigned int tag = (seq << 5) | (unsigned int)(31 - lane);
-#pragma unroll
-    for (int j = 0; j < WF_Z; j++)
-      if (j < size) atomicMax(&s_hash[wf_hash(id[j])], tag);
-    __syncwarp();
-    bool conflict = false;
-#pragma unroll
-    for (int j = 0; j < WF_Z; j++)
-      if (j < size) {
-        const unsigned int h = s_hash[wf_hash(id[j])];  // written in this step: (h >> 5) == seq
-        if (31 - (int)(h & 31u) < lane) conflict = true;
-      }
-    const unsigned stop = __ballot_sync(full, conflict || !valid);
-    const int P = stop ? __ffs(stop) - 1 : 32;  // >= 1: lane 0 is valid and never in conflict
+    for (int j = 0; j < WF_Z; j++) x[j] = (double)row.x[j];
+    const bool dup = row.names_a_feature_twice();
+    hash.next_window(lane);
+    hash.mark(row);
+    const int P = wf_prefix(hash.earlier_has(row, lane) || !valid);  // >= 1: lane 0 is valid and never in conflict
     const bool active = lane < P;
 
     // (2) gather + addends
-    double wv[WF_Z], vv[WF_Z][WF_K], sum[WF_K];
-    if (active) {
-#pragma unroll
-      for (int j = 0; j < WF_Z; j++) {
-        wv[j] = 0;
-        if (j < size && k1) wv[j] = w[id[j]];
-#pragma unroll
-        for (int f = 0; f < WF_K; f++) {
-          vv[j][f] = 0;
-          if (j < size && f < k) vv[j][f] = v[(size_t)id[j] * k + f];
-        }
-      }
-    }
-    // bounds of the next step's examples: in flight during the chain
+    WfGather gat;
+    if (active) gat.gather(row, w, v, k, k1);
+    // bounds of the next window's examples: in flight during the chain
     const uint64_t nr = base + P + lane;
     uint64_t nbeg = 0, nend = 0;
     float nyf = 0.f;
@@ -150,36 +278,13 @@ __global__ void __launch_bounds__(32, 1)
       nyf = target[nr];
     }
     if (active) {
-#pragma unroll
-      for (int j = 0; j < WF_Z; j++) s_add[lane][j] = (j < size && k1) ? wv[j] * x[j] : -0.0;
-#pragma unroll
-      for (int f = 0; f < WF_K; f++) {
-        double sf = 0, ss = 0;
-#pragma unroll
-        for (int j = 0; j < WF_Z; j++)
-          if (j < size) {  // fm_model.h:113-121
-            double d = vv[j][f] * x[j];
-            sf += d;
-            ss += d * d;
-          }
-        sum[f] = sf;
-        s_add[lane][WF_Z + f] = (f < k) ? 0.5 * (sf * sf - ss) : -0.0;
-      }
+      gat.addends(row, k, k1, s_add[lane]);
       s_y[lane] = yf;
     }
     __syncwarp();
-    // entries of the next step's examples: in flight during the chain
-    uint32_t nid[WF_Z];
-    float nxf[WF_Z];
-#pragma unroll
-    for (int j = 0; j < WF_Z; j++) {
-      nid[j] = 0;
-      nxf[j] = 0.f;
-      if (j < (int)(nend - nbeg)) {
-        nid[j] = col[nbeg + j];
-        nxf[j] = val[nbeg + j];
-      }
-    }
+    // entries of the next window's examples: in flight during the chain
+    WfRow next;
+    next.load(col, val, nbeg, nend);
 
     // (3) the bias chain, every lane redundantly
     double my_mult = 0;
@@ -190,29 +295,12 @@ __global__ void __launch_bounds__(32, 1)
       const int tn = (t + 1 < P) ? t + 1 : t;
 #pragma unroll
       for (int a = 0; a < NA; a++) nxt[a] = s_add[tn][a];
-      const double y = (double)s_y[t];
-      const double m_lo = -(y - hp.min_target), m_hi = -(y - hp.max_target);  // off the chain
-      // Unused addend slots hold -0.0, the exact identity of IEEE addition (x + -0.0 == x
-      // for every x, signed zeros included): no select sits in the dependent chain.  A
-      // model without bias keeps the local w0 at +0.0, so 0.0 + w0 is the reference's
-      // `result = 0`.
+      // No select sits in the dependent chain (unused addends are -0.0).  A model without
+      // bias keeps the local w0 at +0.0, so 0.0 + w0 is the reference's `result = 0`.
       double pr = 0.0 + w0;
 #pragma unroll
       for (int a = 0; a < NA; a++) pr += cur[a];
-      double mult = 0;  // fm_learn_sgd_element.h:58-65
-      if (TASK == FMB200_TASK_REGRESSION) {
-        // mult = -(y - clamp(pr)).  The two comparisons and the unclamped difference all
-        // start from pr at once and one select picks among three candidates (two of them
-        // known before the chain), instead of compare -> select -> compare -> select ->
-        // subtract in series.  Same values as fmin(max, .) then fmax(min, .): a NaN or
-        // too-large score takes max_target, then anything below min_target takes it.
-        const bool hi = !(pr <= hp.max_target);
-        const bool lo = hi ? clamp_inverted : (pr < hp.min_target);
-        const double m_mid = -(y - pr);
-        mult = lo ? m_lo : (hi ? m_hi : m_mid);
-      } else {
-        mult = -y * (1.0 - 1.0 / (1.0 + exp(-y * pr)));
-      }
+      const double mult = sgd_mult_select<TASK>(hp, pr, (double)s_y[t]);  // fm_learn_sgd_element.h:58-65
       if (k0) w0 -= lr * (mult + reg0 * w0);  // fm_sgd.h:34-37
       if (lane == t) my_mult = mult;
 #pragma unroll
@@ -220,41 +308,18 @@ __global__ void __launch_bounds__(32, 1)
     }
 
     // (4) scatter: fm_sgd.h:38-50 for the lane's own example
-    if (active) {
-      if (k1) {
-#pragma unroll
-        for (int j = 0; j < WF_Z; j++)
-          if (j < size) {
-            double* wi = &w[id[j]];
-            double c = dup ? *wi : wv[j];
-            c -= lr * (my_mult * x[j] + regw * c);
-            *wi = c;
-          }
-      }
-#pragma unroll
-      for (int f = 0; f < WF_K; f++)
-        if (f < k) {
-#pragma unroll
-          for (int j = 0; j < WF_Z; j++)
-            if (j < size) {
-              double* vp = &v[(size_t)id[j] * k + f];
-              double c = dup ? *vp : vv[j][f];
-              double grad = sum[f] * x[j] - c * x[j] * x[j];
-              c -= lr * (my_mult * grad + regv * c);
-              *vp = c;
-            }
-        }
-    }
-    __syncwarp();  // the next step's gathers (other lanes) must see these stores
+    if (active)
+      gat.scatter(
+          row, dup, w, v, k, k1,
+          [&](int j, uint32_t, double c) { return c - lr * (my_mult * x[j] + regw * c); },
+          [&](int j, int f, size_t, double c) {
+            const double grad = gat.sum[f] * x[j] - c * x[j] * x[j];
+            return c - lr * (my_mult * grad + regv * c);
+          });
+    __syncwarp();  // the next window's gathers (other lanes) must see these stores
     base += P;
-    beg = nbeg;
-    end = nend;
+    row = next;
     yf = nyf;
-#pragma unroll
-    for (int j = 0; j < WF_Z; j++) {
-      id[j] = nid[j];
-      xf[j] = nxf[j];
-    }
   }
   if (lane == 0 && k0) *p.w0() = w0;
 }

@@ -1,23 +1,13 @@
 // fm_sgda_wavefront.cuh -- the SGDA epoch (fm_learn_sgd_element_adapt_reg.h:295-311): the one-warp
-// kernel's arguments and loss rule, and the wavefront schedule for short rows and small k.
-// Included by fm_inorder.cu (compiled with --fmad=false).
+// kernel's arguments, and the wavefront schedule for short rows and small k, built from the window
+// pieces of fm_inorder_wavefront.cuh.  Included by fm_inorder.cu (compiled with --fmad=false); also
+// compiled for the host by tests/simt/ (FMB_SIMT_HOST).
 #pragma once
-#include "fmb200_internal.h"
 #include "fm_inorder_wavefront.cuh"
+#include "fm_loss.cuh"
+#include "fmb200_internal.h"
 
 namespace fmb {
-
-// the score clipped to the target range (fm_learn_sgd_element.h:58-59, fm_learn.h:138-139)
-__device__ __forceinline__ double clamp_target(double p, const HParams& hp) {
-  p = fmin(hp.max_target, p);
-  return fmax(hp.min_target, p);
-}
-
-// d loss / d score of the SGDA learner (fm_learn_sgd_element_adapt_reg.h:151-157, :206-211)
-__device__ __forceinline__ double sgda_grad_loss(const HParams& hp, double p, double t) {
-  if (hp.task == FMB200_TASK_REGRESSION) return 2 * (clamp_target(p, hp) - t);
-  return t * ((1.0 / (1.0 + exp(-t * p))) - 1.0);
-}
 
 // One launch runs the half-steps [h_begin, h_end) of an epoch: half-step 2t is the theta-step on
 // training row t, 2t + 1 the lambda-step that follows it (skipped when lambda_steps == 0).  The
@@ -52,15 +42,15 @@ struct SgdaArgs {
 // window is split: the window ends after its theta-step, and the next one starts with its lambda-step.
 //
 // One warp.  Per window:
-//   1. lane = pair: load the pair's two rows, find the conflict-free prefix P (shared-memory hash);
+//   1. lane = pair: load the pair's two rows, find the conflict-free prefix P (WfHash: r_t is marked,
+//      s_t only looked up);
 //   2. lanes < P gather w / V (and for s_t grad_w / grad_v) and form the theta score's addends
 //      a_i = w_i x_i, b_f = 0.5 (sum_f^2 - sumsq_f) -- they read nothing the chain moves;
 //   3. the chain walks t = 0..P-1 with the one-warp kernel's arithmetic, lane = factor:
 //      theta score ((w0 + a_1) + ...) + b_k, loss, w0; a snapshot of the reg values theta_t's update
 //      reads; lambda score through w' / v' on the current reg; the reg_w / reg_v updates of all G
 //      groups.  Only this part is serial;
-//   4. lane = pair: the theta updates of w, v, grad_w, grad_v (a row naming a feature twice re-reads
-//      memory, so the second update sees the first, as in the one-warp kernel).
+//   4. lane = pair: the theta updates of w, v, grad_w, grad_v (WfGather::scatter).
 // Bit-identical to fm_sgda_epoch_kernel (tests/test_sgda_wavefront_gpu.py).
 struct SgdaWindow {
   static constexpr int NA = WF_Z + WF_K;  // addends of a theta score
@@ -74,16 +64,16 @@ struct SgdaWindow {
   float lx[32][WF_Z];
   float ty[32], ly[32];
   int tsize[32], lsize[32];               // -1: the pair has no theta- / lambda-step in this window
-  unsigned int hash[WF_HASH];             // (seq << 5) | (31 - lane) of the lowest lane whose r_t has the slot
+  unsigned int hash[WF_HASH];             // WfHash's table, marked with the r_t
 };
-
-inline bool sgda_wavefront_eligible(int k, uint32_t train_nnz, uint32_t val_nnz) {
-  return k <= WF_K && train_nnz <= (uint32_t)WF_Z && val_nnz <= (uint32_t)WF_Z;
-}
 
 __global__ void __launch_bounds__(32, 1) fm_sgda_wavefront_kernel(const SgdaArgs a) {
   __shared__ SgdaWindow s;
+#ifdef FMB_SIMT_HOST
+  double* const sw_smem = simt::dynamic_smem;
+#else
   extern __shared__ double sw_smem[];  // reg_w[G] | reg_v[G][k]
+#endif
   const int lane = threadIdx.x;
   const unsigned full = 0xffffffffu;
   const int k = a.k;
@@ -93,7 +83,7 @@ __global__ void __launch_bounds__(32, 1) fm_sgda_wavefront_kernel(const SgdaArgs
   double* s_reg_v = s_reg_w + G;
   for (uint32_t i = lane; i < G; i += 32) s_reg_w[i] = a.reg_w[i];
   for (uint32_t i = lane; i < G * (uint32_t)k; i += 32) s_reg_v[i] = a.reg_v[i];
-  for (int i = lane; i < WF_HASH; i += 32) s.hash[i] = 0;
+  WfHash hash(s.hash, lane);
   __syncwarp();
   double* w = a.p.w();
   double* v = a.p.v();
@@ -103,7 +93,6 @@ __global__ void __launch_bounds__(32, 1) fm_sgda_wavefront_kernel(const SgdaArgs
   const uint64_t vstart = (a.vc0 >= a.v_rows) ? 0 : a.vc0;  // the first lambda-step restarts a full cursor
   const uint64_t p_first = a.h_begin / 2;
 
-  unsigned int seq = 0;
   uint64_t hs = a.h_begin;
   while (hs < a.h_end) {
     // (1) the window's pairs and their conflict-free prefix
@@ -111,143 +100,77 @@ __global__ void __launch_bounds__(32, 1) fm_sgda_wavefront_kernel(const SgdaArgs
     const bool valid = 2 * p < a.h_end;
     const bool has_theta = valid && 2 * p >= hs;
     bool has_lambda = valid && lam && 2 * p + 1 < a.h_end;
-    int tsize = 0, lsize = 0;
-    uint32_t tid[WF_Z], lid[WF_Z];
-    float tx[WF_Z], lx[WF_Z];
+    uint64_t beg = 0, end = 0;
     float ty = 0.f, ly = 0.f;
-#pragma unroll
-    for (int j = 0; j < WF_Z; j++) {
-      tid[j] = lid[j] = 0;
-      tx[j] = lx[j] = 0.f;
-    }
     if (has_theta) {
-      const uint64_t beg = a.row_ptr[p];
-      tsize = (int)(a.row_ptr[p + 1] - beg);
+      beg = a.row_ptr[p];
+      end = a.row_ptr[p + 1];
       ty = a.target[p];
-#pragma unroll
-      for (int j = 0; j < WF_Z; j++)
-        if (j < tsize) {
-          tid[j] = a.col[beg + j];
-          tx[j] = a.val[beg + j];
-        }
     }
+    WfRow trow;
+    trow.load(a.col, a.val, beg, end);
+    beg = end = 0;
     if (has_lambda) {
       const uint64_t s_row = (vstart + (p - p_first)) % a.v_rows;  // :302-305
-      const uint64_t beg = a.v_row_ptr[s_row];
-      lsize = (int)(a.v_row_ptr[s_row + 1] - beg);
+      beg = a.v_row_ptr[s_row];
+      end = a.v_row_ptr[s_row + 1];
       ly = a.v_target[s_row];
-#pragma unroll
-      for (int j = 0; j < WF_Z; j++)
-        if (j < lsize) {
-          lid[j] = a.v_col[beg + j];
-          lx[j] = a.v_val[beg + j];
-        }
     }
-    bool dup = false;
-#pragma unroll
-    for (int j = 1; j < WF_Z; j++)
-#pragma unroll
-      for (int j2 = 0; j2 < j; j2++)
-        if (j < tsize && tid[j] == tid[j2]) dup = true;
-    if (++seq == (1u << 27)) {  // step counter about to leave its 27 bits: start over
-      for (int i = lane; i < WF_HASH; i += 32) s.hash[i] = 0;
-      seq = 1;
-      __syncwarp();
-    }
-    const unsigned int tag = (seq << 5) | (unsigned int)(31 - lane);
-#pragma unroll
-    for (int j = 0; j < WF_Z; j++)
-      if (j < tsize) atomicMax(&s.hash[wf_hash(tid[j])], tag);
-    __syncwarp();
-    bool conflict = false;
-#pragma unroll
-    for (int j = 0; j < WF_Z; j++) {
-      if (j < tsize) {  // an earlier r_t' has one of r_t's features
-        const unsigned int h = s.hash[wf_hash(tid[j])];
-        if (31 - (int)(h & 31u) < lane) conflict = true;
-      }
-      if (j < lsize) {  // r_t' with t' <= t has one of s_t's features
-        const unsigned int h = s.hash[wf_hash(lid[j])];
-        if ((h >> 5) == seq && 31 - (int)(h & 31u) <= lane) conflict = true;
-      }
-    }
-    const unsigned stop = __ballot_sync(full, conflict || !valid);
-    int P = stop ? __ffs(stop) - 1 : 32;
+    WfRow lrow;
+    lrow.load(a.v_col, a.v_val, beg, end);
+    const bool dup = trow.names_a_feature_twice();
+    hash.next_window(lane);
+    hash.mark(trow);
+    // r_t' with t' < t has one of r_t's features, or r_t' with t' <= t one of s_t's
+    int P = wf_prefix(hash.earlier_has(trow, lane) | hash.this_or_earlier_has(lrow, lane) | !valid);
     // Lane 0 conflicts only through its own pair: split it (theta now, lambda heads the next window).
     const bool split = P == 0;
     if (split) {
       P = 1;
-      if (lane == 0) has_lambda = false, lsize = 0;
+      if (lane == 0) has_lambda = false, lrow.size = 0;
     }
     const bool active = lane < P;
 
     // (2) gathers and theta addends
-    double wv[WF_Z], vv[WF_Z][WF_K], sum[WF_K];
+    WfGather gat;
     if (active) {
-      s.tsize[lane] = has_theta ? tsize : -1;
-      s.lsize[lane] = has_lambda ? lsize : -1;
+      s.tsize[lane] = has_theta ? trow.size : -1;
+      s.lsize[lane] = has_lambda ? lrow.size : -1;
       s.ty[lane] = ty;
       s.ly[lane] = ly;
 #pragma unroll
       for (int j = 0; j < WF_Z; j++) {
-        wv[j] = 0;
-        uint32_t g = 0;
-        if (j < tsize) {
-          g = a.group[tid[j]];
-          if (k1) wv[j] = w[tid[j]];
-        }
-        s.tg[lane][j] = g;
-#pragma unroll
-        for (int f = 0; f < WF_K; f++) {
-          vv[j][f] = 0;
-          if (j < tsize && f < k) vv[j][f] = v[(size_t)tid[j] * k + f];
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < WF_Z; j++) {
+        const uint32_t id = lrow.id[j];
         double lwj = 0, lgwj = 0;
         uint32_t g = 0;
-        if (j < lsize) {
-          g = a.group[lid[j]];
+        if (j < lrow.size) {
+          g = a.group[id];
           if (k1) {
-            lwj = w[lid[j]];
-            lgwj = a.grad_w[lid[j]];
+            lwj = w[id];
+            lgwj = a.grad_w[id];
           }
         }
         s.lg[lane][j] = g;
-        s.lx[lane][j] = lx[j];
+        s.lx[lane][j] = lrow.x[j];
         s.lw[lane][j] = lwj;
         s.lgw[lane][j] = lgwj;
 #pragma unroll
         for (int f = 0; f < WF_K; f++) {
           double a_v = 0, a_g = 0;
-          if (j < lsize && f < k) {
-            a_v = v[(size_t)lid[j] * k + f];
-            a_g = a.grad_v[(size_t)lid[j] * k + f];
+          if (j < lrow.size && f < k) {
+            a_v = v[(size_t)id * k + f];
+            a_g = a.grad_v[(size_t)id * k + f];
           }
           s.lv[lane][j][f] = a_v;
           s.lgv[lane][j][f] = a_g;
         }
       }
-      // fm_model.h:107-121: a_i = w_i * x_i, b_f = 0.5 * (sum_f^2 - sumsq_f), sum_f = ((0 + d_0) + d_1) + ...
+      gat.gather(trow, w, v, k, k1);
 #pragma unroll
-      for (int j = 0; j < WF_Z; j++) s.ta[lane][j] = (j < tsize && k1) ? wv[j] * (double)tx[j] : -0.0;
-#pragma unroll
-      for (int f = 0; f < WF_K; f++) {
-        double sf = 0, ss = 0;
-#pragma unroll
-        for (int j = 0; j < WF_Z; j++)
-          if (j < tsize) {
-            const double d = vv[j][f] * (double)tx[j];
-            sf += d;
-            ss += d * d;
-          }
-        sum[f] = sf;
-        s.ta[lane][WF_Z + f] = (f < k) ? 0.5 * (sf * sf - ss) : -0.0;
-      }
+      for (int j = 0; j < WF_Z; j++) s.tg[lane][j] = (j < trow.size) ? a.group[trow.id[j]] : 0;
+      gat.addends(trow, k, k1, s.ta[lane]);
     }
     __syncwarp();
-
     // (3) the chain, lane = factor
     for (int t = 0; t < P; t++) {
       const int ts = s.tsize[t];
@@ -332,30 +255,19 @@ __global__ void __launch_bounds__(32, 1) fm_sgda_wavefront_kernel(const SgdaArgs
     // (4) the theta updates, lane = pair (:153-168)
     if (active && has_theta) {
       const double mult = s.mult[lane];
-      if (k1)
-#pragma unroll
-        for (int j = 0; j < WF_Z; j++)
-          if (j < tsize) {
-            const uint32_t id = tid[j];
-            double cur = dup ? w[id] : wv[j];
-            const double gw = mult * tx[j];
-            a.grad_w[id] = gw;
-            cur -= lr * (gw + 2 * s.rw[lane][j] * cur);
-            w[id] = cur;
-          }
-#pragma unroll
-      for (int f = 0; f < WF_K; f++)
-        if (f < k)
-#pragma unroll
-          for (int j = 0; j < WF_Z; j++)
-            if (j < tsize) {
-              const size_t at = (size_t)tid[j] * k + f;
-              double cur = dup ? v[at] : vv[j][f];
-              const double gv = mult * (tx[j] * (sum[f] - cur * tx[j]));
-              a.grad_v[at] = gv;
-              cur -= lr * (gv + 2 * s.rv[lane][j][f] * cur);
-              v[at] = cur;
-            }
+      gat.scatter(
+          trow, dup, w, v, k, k1,
+          [&](int j, uint32_t at, double c) {
+            const double gw = mult * trow.x[j];
+            a.grad_w[at] = gw;
+            return c - lr * (gw + 2 * s.rw[lane][j] * c);
+          },
+          [&](int j, int f, size_t at, double c) {
+            const double x = trow.x[j];
+            const double gv = mult * (x * (gat.sum[f] - c * x));
+            a.grad_v[at] = gv;
+            return c - lr * (gv + 2 * s.rv[lane][j][f] * c);
+          });
     }
     __syncwarp();  // the next window's gathers (other lanes) must see these stores
     hs = split ? 2 * (hs / 2) + 1 : 2 * (hs / 2 + P);

@@ -2,10 +2,11 @@
 // warp-sized kernel for the host and run it as 32 OS threads, one per lane.
 //
 // The model is the one CUDA itself gives since independent thread scheduling: lanes run
-// freely and only meet where the kernel says so (__syncwarp, __ballot_sync).  Those become
-// pthread barriers here, `__shared__` variables become function-local statics (one copy for
-// the single CTA), shared-memory atomics become __atomic builtins.  Everything else -- the
-// arithmetic, the indexing, the order of memory operations -- is the kernel's own source.
+// freely and only meet where the kernel says so (__syncwarp, __ballot_sync, __shfl_sync).
+// Those become pthread barriers here, `__shared__` variables become function-local statics
+// (one copy for the single CTA), dynamic shared memory is simt::dynamic_smem (FMB_SIMT_HOST),
+// shared-memory atomics become __atomic builtins.  Everything else -- the arithmetic, the
+// indexing, the order of memory operations -- is the kernel's own source.
 // Because the barriers are real synchronisation, ThreadSanitizer can check that every
 // cross-lane hand-off through "shared" or "global" memory is ordered by one.
 #pragma once
@@ -14,6 +15,9 @@
 #include <math.h>
 #include <pthread.h>
 #include <stdint.h>
+#include <string.h>
+
+#define FMB_SIMT_HOST 1
 
 #undef __global__
 #undef __device__
@@ -39,6 +43,8 @@ struct Dim {
 extern thread_local Dim tid;
 extern pthread_barrier_t warp_barrier;
 extern unsigned ballot_in[kLanes];
+extern uint64_t shfl_in[kLanes];
+extern double dynamic_smem[];  // the kernel's `extern __shared__` memory
 
 inline void sync() { pthread_barrier_wait(&warp_barrier); }
 
@@ -60,6 +66,19 @@ inline unsigned __ballot_sync(unsigned, bool pred) {
     if (__atomic_load_n(&simt::ballot_in[l], __ATOMIC_RELAXED)) m |= 1u << l;
   simt::sync();  // nobody overwrites its slot for the next ballot before all have read
   return m;
+}
+
+template <class T>
+inline T __shfl_sync(unsigned, T v, int src) {
+  static_assert(sizeof(T) <= sizeof(uint64_t), "one word per lane");
+  uint64_t bits = 0;
+  memcpy(&bits, &v, sizeof(T));
+  __atomic_store_n(&simt::shfl_in[simt::tid.x], bits, __ATOMIC_RELAXED);
+  simt::sync();
+  bits = __atomic_load_n(&simt::shfl_in[src & (simt::kLanes - 1)], __ATOMIC_RELAXED);
+  simt::sync();  // nobody overwrites its slot for the next exchange before all have read
+  memcpy(&v, &bits, sizeof(T));
+  return v;
 }
 
 inline int __ffs(unsigned v) { return __builtin_ffs((int)v); }
