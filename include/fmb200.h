@@ -203,6 +203,32 @@ int fmb200_mcmc_begin_xt(fmb200_ctx* ctx, int train_slot, const fmb200_xt_blocks
                          const fmb200_xt_blocks* test_xt, int do_sample, int do_multilevel, uint32_t n_groups,
                          const uint32_t* attr_group, const uint32_t* attr_per_group, double reg0,
                          const double* w_lambda, const double* v_lambda);
+/* Relational data (block structure, BS): the reference's RelationData / RelationJoin (relation.h) and the
+ * relational parts of fm_learn_mcmc (fm_learn_mcmc.h:148-378, 430-641, 734-790, 849-935, 1183-1188).  Each case
+ * of train and test joins one row of each relation block; the block's attributes are the model's ids
+ * attr_offset .. attr_offset + num_feature - 1.  Called after the train and test uploads and before
+ * fmb200_mcmc_begin with the same two slots, it makes that _begin, and the _iteration, _get_hyper and _get_pred
+ * calls after it, run the relational learner; the next _begin without a new call runs without relations.  A
+ * _begin consumes them whether it succeeds or fails, and refuses them when either slot was re-uploaded.  The
+ * call copies everything it is given.  n_rel = 0 withdraws relations set before.  attr_group / attr_per_group of
+ * _begin are the joined meta table of libfm.cpp:213-240 over all n attributes.  Checks (a named error, nothing is
+ * kept): join lengths equal to the slots' case counts, join and row ids below num_cases, a .xt whose column
+ * starts ascend from 0, and offsets that follow one another and end at num_attribute.  _begin then checks that
+ * neither main data set names an id at or above the first attr_offset.  fmb200_mcmc_begin_xt refuses relations;
+ * fmb200_mcmc_eterms ignores them. */
+typedef struct fmb200_relation {
+  uint32_t num_cases;          /* rows of the block (RelationData::num_cases, the .xt's num_cols) */
+  uint32_t num_feature;        /* its attributes (the .xt's num_rows) */
+  uint32_t attr_offset;        /* model id of its attribute 0 */
+  const uint64_t* col_ptr;     /* [num_feature + 1]: the block's .xt, column j at [col_ptr[j], col_ptr[j + 1]) */
+  const uint32_t* row;         /* [col_ptr[num_feature]]: relation row of every entry, in file order */
+  const float* val;            /* [col_ptr[num_feature]] */
+  uint64_t n_train, n_test;    /* lengths of the two joins */
+  const uint32_t* train_join;  /* [n_train]: train case -> relation row (<rel>.train) */
+  const uint32_t* test_join;   /* [n_test]: test case -> relation row (<rel>.test) */
+} fmb200_relation;
+int fmb200_mcmc_set_relations(fmb200_ctx* ctx, int train_slot, int test_slot, uint32_t n_rel,
+                              const fmb200_relation* rel);
 int fmb200_mcmc_iteration(fmb200_ctx* ctx, double* train_metric, uint32_t* counters);
 int fmb200_mcmc_get_hyper(fmb200_ctx* ctx, double* alpha, double* w_mu, double* w_lambda, double* v_mu,
                           double* v_lambda);

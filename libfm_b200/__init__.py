@@ -5,7 +5,7 @@ driven by `fm_learn_sgd_element::learn`) as hand-written CUDA behind the C ABI
 of include/fmb200.h, plus the host mirror needed to drive it.  See DESIGN.md.
 """
 from .model import (Data, FmError, FmLearnSgdElement, FmModel, MODE_HOGWILD, MODE_INORDER, MODE_ORDERED,
-                    TASK_CLASSIFICATION, TASK_REGRESSION)
+                    RelationData, RelationJoin, TASK_CLASSIFICATION, TASK_REGRESSION)
 
 __all__ = ["Data", "FmError", "FmLearnSgdElement", "FmModel", "MODE_HOGWILD", "MODE_INORDER", "MODE_ORDERED",
-           "TASK_CLASSIFICATION", "TASK_REGRESSION"]
+           "RelationData", "RelationJoin", "TASK_CLASSIFICATION", "TASK_REGRESSION"]

@@ -31,6 +31,13 @@ class XtBlocksC(C.Structure):
                 ("nnz", _u64p), ("slot", C.c_int * 2), ("user", C.c_void_p), ("fetch", XT_FETCH),
                 ("release", XT_RELEASE)]
 
+
+class RelationC(C.Structure):
+    """fmb200_relation (fmb200_mcmc_set_relations)"""
+    _fields_ = [("num_cases", C.c_uint32), ("num_feature", C.c_uint32), ("attr_offset", C.c_uint32),
+                ("col_ptr", _u64p), ("row", _u32p), ("val", _f32p), ("n_train", C.c_uint64), ("n_test", C.c_uint64),
+                ("train_join", _u32p), ("test_join", _u32p)]
+
 SYMBOLS = {
     "fmb200_create": (C.c_int, [C.POINTER(_ctx), C.c_int, C.c_uint32, C.c_int, C.c_int, C.c_int]),
     "fmb200_destroy": (None, [_ctx]),
@@ -63,6 +70,7 @@ SYMBOLS = {
                                     _f64p, _f64p]),
     "fmb200_mcmc_begin_xt": (C.c_int, [_ctx, C.c_int, C.POINTER(XtBlocksC), C.c_int, C.POINTER(XtBlocksC), C.c_int,
                                        C.c_int, C.c_uint32, _u32p, _u32p, C.c_double, _f64p, _f64p]),
+    "fmb200_mcmc_set_relations": (C.c_int, [_ctx, C.c_int, C.c_int, C.c_uint32, C.POINTER(RelationC)]),
     "fmb200_mcmc_iteration": (C.c_int, [_ctx, _f64p, _u32p]),
     "fmb200_mcmc_get_hyper": (C.c_int, [_ctx] + [_f64p] * 5),
     "fmb200_mcmc_get_pred": (C.c_int, [_ctx] + [_f64p] * 3),

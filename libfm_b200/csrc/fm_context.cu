@@ -857,6 +857,10 @@ int fmb200_mcmc_begin(fmb200_ctx* c, int train_slot, int test_slot, int do_sampl
                       uint32_t n_groups, const uint32_t* attr_group, const uint32_t* attr_per_group, double reg0,
                       const double* w_lambda, const double* v_lambda) {
   NEED_CTX(c);
+  struct DropRelations {  // relations set before apply to this call only, whichever way it ends
+    fmb200_ctx* c;
+    ~DropRelations() { c->mcmc_rel.clear(); }
+  } drop{c};
   if (need_slot(c, train_slot) || need_slot(c, test_slot)) return 1;
   if (bind(c)) return 1;
   if (need_fp64(c, "MCMC / ALS run on the fp64 state: set INORDER or ORDERED mode first")) return 1;
@@ -873,11 +877,34 @@ int fmb200_mcmc_begin(fmb200_ctx* c, int train_slot, int test_slot, int do_sampl
   });
 }
 
+int fmb200_mcmc_set_relations(fmb200_ctx* c, int train_slot, int test_slot, uint32_t n_rel,
+                              const fmb200_relation* rel) {
+  NEED_CTX(c);
+  c->mcmc_rel.clear();
+  if (n_rel == 0) return 0;
+  if (need_slot(c, train_slot) || need_slot(c, test_slot)) return 1;
+  return guarded([&]() {
+    std::vector<RelationHost> r;
+    const std::string e = mcmc_check_relations(c, train_slot, test_slot, n_rel, rel, &r);
+    if (!e.empty()) return fail("fmb200_mcmc_set_relations: %s", e.c_str());
+    c->mcmc_rel = std::move(r);
+    c->mcmc_rel_slot[0] = train_slot;
+    c->mcmc_rel_slot[1] = test_slot;
+    c->mcmc_rel_gen[0] = c->slots[train_slot].upload_gen;
+    c->mcmc_rel_gen[1] = c->slots[test_slot].upload_gen;
+    return 0;
+  });
+}
+
 int fmb200_mcmc_begin_xt(fmb200_ctx* c, int train_slot, const fmb200_xt_blocks* train_xt, int test_slot,
                          const fmb200_xt_blocks* test_xt, int do_sample, int do_multilevel, uint32_t n_groups,
                          const uint32_t* attr_group, const uint32_t* attr_per_group, double reg0,
                          const double* w_lambda, const double* v_lambda) {
   NEED_CTX(c);
+  if (!c->mcmc_rel.empty()) {
+    c->mcmc_rel.clear();
+    return fail("fmb200_mcmc_begin_xt: relations are not streamed: call fmb200_mcmc_begin for relational data");
+  }
   if ((!train_xt && need_slot(c, train_slot)) || (!test_xt && need_slot(c, test_slot))) return 1;
   if (bind(c)) return 1;
   if (need_fp64(c, "MCMC / ALS run on the fp64 state: set INORDER or ORDERED mode first")) return 1;

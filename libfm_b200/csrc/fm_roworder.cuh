@@ -67,6 +67,33 @@ __device__ __forceinline__ double row_q(const RowOrder& o, const double* v, int 
   return q;
 }
 
+// The e-term of one case (fm_learn_mcmc.h:172-362), every operation in the reference's order:
+//   e = sum_f 0.5 q_f^2 ;  q = sum_f sum_i -0.5 v_if^2 x_i^2  (+ sum_i w_i x_i) ;  e = (e + q) + w0
+// rel_f(f, q_f) adds the relation blocks' q_f of the case to q_f before it is squared (:227-240), rel(q) their
+// q to q before the merge (:352-368); without relations both leave their argument alone.
+template <class RF, class R>
+__device__ __forceinline__ double case_eterm(const RowOrder& o, const double* v, const double* w, int k, int use_w,
+                                             int use_w0, double w0, const float* x, RF&& rel_f, R&& rel) {
+  double e = 0.0;
+  for (int f = 0; f < k; f++) {  // :172-252
+    double q = row_q(o, v, k, f, x);
+    rel_f(f, q);
+    e += 0.5 * q * q;
+  }
+  double q = 0.0;
+  for (int f = 0; f < k; f++)  // :255-306
+    o.for_each([&](uint32_t pos) {
+      const double vif = v[(size_t)o.c[pos] * k + f];
+      const float xi = x[pos];
+      q -= 0.5 * vif * vif * xi * xi;  // (((0.5*v)*v)*x)*x, x promoted to double per factor
+    });
+  if (use_w) o.for_each([&](uint32_t pos) { q += w[o.c[pos]] * (double)x[pos]; });  // :309-346
+  rel(q);
+  e = e + q;  // :350-362
+  if (use_w0) e += w0;
+  return e;
+}
+
 // row containing entry e: the last r with row_ptr[r] <= e (empty rows skipped by construction)
 __device__ __forceinline__ uint64_t row_of(const uint64_t* __restrict__ rp, uint64_t n_rows, uint64_t e) {
   uint64_t lo = 0, hi = n_rows;  // invariant: rp[lo] <= e < rp[hi]

@@ -7,6 +7,7 @@
 #include <memory>
 #include <string>
 #include <type_traits>
+#include <vector>
 
 #include "../../include/fmb200.h"
 
@@ -207,6 +208,15 @@ struct McmcDelete {
   void operator()(McmcState* s) const;
 };
 
+// One relation block as fmb200_mcmc_set_relations was given it, copied and checked
+struct RelationHost {
+  uint32_t num_cases = 0, num_feature = 0, attr_offset = 0;
+  std::vector<uint64_t> col_ptr;  // [num_feature + 1]
+  std::vector<uint32_t> row;
+  std::vector<float> val;
+  std::vector<uint32_t> join[2];  // train, test
+};
+
 struct EpochConfig {
   int lanes_per_row = 0, slots = 0, rows_per_tile = 0, grid = 0, block = 0, smem = 0, damp = 0;
   int dealt = 0;  // the row-lane epoch ran the dealt schedule
@@ -270,6 +280,10 @@ struct fmb200_ctx {
   int tune_damp = 0;  // 0 auto, 1 force on, -1 force off
   int tune_variant = 0;  // 0 auto, 1 row-group kernel, 2 row-lane kernel when eligible
   std::unique_ptr<fmb::McmcState, fmb::McmcDelete> mcmc;  // MCMC / ALS learner state (fm_mcmc.cu)
+  // relation blocks for the next fmb200_mcmc_begin on these slots (fmb200_mcmc_set_relations), consumed by it
+  std::vector<fmb::RelationHost> mcmc_rel;
+  int mcmc_rel_slot[2] = {-1, -1};
+  uint64_t mcmc_rel_gen[2] = {0, 0};  // the two slots' upload generations when the relations were set
 };
 
 namespace fmb {
@@ -306,6 +320,9 @@ std::string mcmc_begin(fmb200_ctx* c, int train, int test, int do_sample, int do
                        const double* w_lambda0, const double* v_lambda0, const fmb200_xt_blocks* train_xt = nullptr,
                        const fmb200_xt_blocks* test_xt = nullptr);
 std::string mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counters);
+// fm_mcmc.cu: the checks of fmb200_mcmc_set_relations and the host copy; "" on success
+std::string mcmc_check_relations(const fmb200_ctx* c, int train, int test, uint32_t n_rel, const fmb200_relation* rel,
+                                 std::vector<RelationHost>* out);
 bool mcmc_get(const fmb200_ctx* c, double* alpha, double* w_mu, double* w_lambda, double* v_mu, double* v_lambda,
               double* pred_this, double* pred_sum_all, double* pred_sum_all_but5, uint32_t* n_runs);
 // fm_inorder.cu: one SGDA epoch (theta-step per training row, lambda-step per validation row).  Its
