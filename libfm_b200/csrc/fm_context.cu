@@ -853,28 +853,39 @@ int fmb200_mcmc_eterms(fmb200_ctx* c, int slot, double* e_out) {
   return 0;
 }
 
-int fmb200_mcmc_begin(fmb200_ctx* c, int train_slot, int test_slot, int do_sample, int do_multilevel,
-                      uint32_t n_groups, const uint32_t* attr_group, const uint32_t* attr_per_group, double reg0,
-                      const double* w_lambda, const double* v_lambda) {
+// The body of fmb200_mcmc_begin and fmb200_mcmc_begin_xt; fn names the entry point in messages
+static int mcmc_begin_entry(const char* fn, fmb200_ctx* c, int train_slot, const fmb200_xt_blocks* train_xt,
+                            int test_slot, const fmb200_xt_blocks* test_xt, int do_sample, int do_multilevel,
+                            uint32_t n_groups, const uint32_t* attr_group, const uint32_t* attr_per_group, double reg0,
+                            const double* w_lambda, const double* v_lambda) {
   NEED_CTX(c);
   struct DropRelations {  // relations set before apply to this call only, whichever way it ends
     fmb200_ctx* c;
     ~DropRelations() { c->mcmc_rel.clear(); }
   } drop{c};
-  if (need_slot(c, train_slot) || need_slot(c, test_slot)) return 1;
+  if ((!train_xt && need_slot(c, train_slot)) || (!test_xt && need_slot(c, test_slot))) return 1;
   if (bind(c)) return 1;
   if (need_fp64(c, "MCMC / ALS run on the fp64 state: set INORDER or ORDERED mode first")) return 1;
   if (!w_lambda || (!v_lambda && c->k > 0)) return fail("null w_lambda / v_lambda");
   if (c->peer_world > 1) return fail("MCMC / ALS run on one GPU: this context is attached to a multi-GPU peer world");
+  if ((train_xt || test_xt) && c->copy_stream == nullptr)
+    CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
   return guarded([&]() {
     const std::string e = mcmc_begin(c, train_slot, test_slot, do_sample, do_multilevel, n_groups, attr_group,
-                                      attr_per_group, reg0, w_lambda, v_lambda);
+                                      attr_per_group, reg0, w_lambda, v_lambda, train_xt, test_xt);
     if (!e.empty()) {
       c->mcmc.reset();
-      return fail("fmb200_mcmc_begin: %s", e.c_str());
+      return fail("%s: %s", fn, e.c_str());
     }
     return 0;
   });
+}
+
+int fmb200_mcmc_begin(fmb200_ctx* c, int train_slot, int test_slot, int do_sample, int do_multilevel,
+                      uint32_t n_groups, const uint32_t* attr_group, const uint32_t* attr_per_group, double reg0,
+                      const double* w_lambda, const double* v_lambda) {
+  return mcmc_begin_entry("fmb200_mcmc_begin", c, train_slot, nullptr, test_slot, nullptr, do_sample, do_multilevel,
+                          n_groups, attr_group, attr_per_group, reg0, w_lambda, v_lambda);
 }
 
 int fmb200_mcmc_set_relations(fmb200_ctx* c, int train_slot, int test_slot, uint32_t n_rel,
@@ -905,22 +916,8 @@ int fmb200_mcmc_begin_xt(fmb200_ctx* c, int train_slot, const fmb200_xt_blocks* 
     c->mcmc_rel.clear();
     return fail("fmb200_mcmc_begin_xt: relations are not streamed: call fmb200_mcmc_begin for relational data");
   }
-  if ((!train_xt && need_slot(c, train_slot)) || (!test_xt && need_slot(c, test_slot))) return 1;
-  if (bind(c)) return 1;
-  if (need_fp64(c, "MCMC / ALS run on the fp64 state: set INORDER or ORDERED mode first")) return 1;
-  if (!w_lambda || (!v_lambda && c->k > 0)) return fail("null w_lambda / v_lambda");
-  if (c->peer_world > 1) return fail("MCMC / ALS run on one GPU: this context is attached to a multi-GPU peer world");
-  if ((train_xt || test_xt) && c->copy_stream == nullptr)
-    CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
-  return guarded([&]() {
-    const std::string e = mcmc_begin(c, train_slot, test_slot, do_sample, do_multilevel, n_groups, attr_group,
-                                      attr_per_group, reg0, w_lambda, v_lambda, train_xt, test_xt);
-    if (!e.empty()) {
-      c->mcmc.reset();
-      return fail("fmb200_mcmc_begin_xt: %s", e.c_str());
-    }
-    return 0;
-  });
+  return mcmc_begin_entry("fmb200_mcmc_begin_xt", c, train_slot, train_xt, test_slot, test_xt, do_sample, do_multilevel,
+                          n_groups, attr_group, attr_per_group, reg0, w_lambda, v_lambda);
 }
 
 int fmb200_mcmc_iteration(fmb200_ctx* c, double* train_metric, uint32_t* counters) {

@@ -1,6 +1,6 @@
 // fm_roworder.cuh -- a case's entries in (feature id, position) order, the order in which the
 // MCMC / ALS learner reaches them through the transposed data (reference Data.h:292-341).
-// Shared by the e-term pass (fm_inorder.cu) and the q rebuild of the Gibbs sweep (fm_mcmc.cu), with
+// Used by the e-term pass and the q rebuild of the Gibbs sweep (fm_mcmc.cu), with
 // row_of, the entry -> case lookup of the index builds (fm_ordered.cu, fm_mcmc.cu).
 #pragma once
 #include <stdint.h>
