@@ -245,12 +245,27 @@ int fmb200_mcmc_runs(fmb200_ctx* ctx, uint32_t* n_runs);
  *          Sequential semantics, fp64, bit-identical to the reference (one warp; for num_factor <= 8
  *          and rows of at most 4 entries a wavefront of conflict-free steps, fmb200_set_tuning
  *          variant 1 forcing the one-warp kernel).
+ *  _epoch_x: the out-of-core form of _epoch (the reference's -cache_size over binary .x data).  A set given
+ *          as fmb200_xt_blocks (non-NULL) is not held on the device: its .x blocks are fetched in file order
+ *          through its two slots and decoded on the device like fmb200_upload_xblock, the copy of the next block
+ *          overlapping the work on the current one; a NULL blocks pointer takes the set from its slot as _epoch
+ *          does.  The struct describes a .x exactly as it describes a .xt, with rows in place of columns: n_cases
+ *          = the rows (= targets), col_lo[b] = the first row of block b, col_lo[n_blocks] = n_cases, fetch hands
+ *          out block b's words and its rows' sizes.  The training set is passed once per epoch.  The validation
+ *          set is read only by lambda-steps, from the cursor's row: a pass over it starts at block 0 once every
+ *          block fetched before has been released (the cursor restarts), and may end early (the epoch ends).
+ *          Parameters, regularisation values and moments after every epoch are bit-identical to _epoch on the
+ *          same data resident.  Limits: one GPU, the fp64 modes, fewer than 2^32 rows and fewer than 2^32
+ *          entries per block.
  *  _get_reg: reg_w[n_groups], reg_v[n_groups][num_factor].
  *  _get_moments: var_w and var_v[num_factor] of the last epoch's last update_means (:250-274), taken
  *          at the epoch's start or, when the validation cursor restarts, before the last restart's
- *          lambda-step; the means the reference logs with them are always 0 (:270-273). */
+ *          lambda-step; the means the reference logs with them are always 0 (:270-273).
+ *  _get_reg and _get_moments serve _epoch and _epoch_x alike. */
 int fmb200_sgda_begin(fmb200_ctx* ctx, uint32_t n_groups, const uint32_t* attr_group);
 int fmb200_sgda_epoch(fmb200_ctx* ctx, int train_slot, int val_slot, int lambda_steps, double* device_seconds);
+int fmb200_sgda_epoch_x(fmb200_ctx* ctx, int train_slot, const fmb200_xt_blocks* train, int val_slot,
+                        const fmb200_xt_blocks* val, int lambda_steps, double* device_seconds);
 int fmb200_sgda_get_reg(fmb200_ctx* ctx, double* reg_w, double* reg_v);
 int fmb200_sgda_get_moments(fmb200_ctx* ctx, double* var_w, double* var_v);
 

@@ -63,6 +63,8 @@ SYMBOLS = {
     "fmb200_predict": (C.c_int, [_ctx, C.c_int, C.c_int, _f64p]),
     "fmb200_sgda_begin": (C.c_int, [_ctx, C.c_uint32, _u32p]),
     "fmb200_sgda_epoch": (C.c_int, [_ctx, C.c_int, C.c_int, C.c_int, _f64p]),
+    "fmb200_sgda_epoch_x": (C.c_int, [_ctx, C.c_int, C.POINTER(XtBlocksC), C.c_int, C.POINTER(XtBlocksC), C.c_int,
+                                      _f64p]),
     "fmb200_sgda_get_reg": (C.c_int, [_ctx, _f64p, _f64p]),
     "fmb200_sgda_get_moments": (C.c_int, [_ctx, _f64p, _f64p]),
     "fmb200_mcmc_eterms": (C.c_int, [_ctx, C.c_int, _f64p]),

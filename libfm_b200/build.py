@@ -41,7 +41,7 @@ CU_SOURCES = {
     "fm_mcmc.cu": ["--fmad=false"],
 }
 CU_HEADERS = ["fm_device.cuh", "fm_rowgroup.cuh", "fm_hogwild_common.cuh", "fmb200_internal.h",
-              "fm_inorder_wavefront.cuh", "fm_sgda_wavefront.cuh", "fm_loss.cuh", "fm_ordered.cuh", "fm_roworder.cuh", "ref_random.h"]
+              "fm_inorder_wavefront.cuh", "fm_sgda_wavefront.cuh", "fm_sgda_plan.h", "fm_loss.cuh", "fm_ordered.cuh", "fm_roworder.cuh", "ref_random.h"]
 
 
 def _newer(target: str, deps: list[str]) -> bool:

@@ -801,17 +801,147 @@ int fmb200_sgda_begin(fmb200_ctx* c, uint32_t n_groups, const uint32_t* attr_gro
   return 0;
 }
 
-int fmb200_sgda_epoch(fmb200_ctx* c, int train_slot, int val_slot, int lambda_steps, double* device_seconds) {
+}  // extern "C"
+
+namespace {
+
+// A data set of an SGDA epoch: resident in `slot`, or streamed from the .x blocks `src` through src->slot[0] and
+// src->slot[1].  order: the blocks the epoch's launches read, in turn (a block read by consecutive launches once);
+// order[j] passes through src->slot[j % 2], so the next block's copy overlaps the launches on this one.
+struct SgdaSet {
+  const char* name;
+  int slot = -1;
+  const fmb200_xt_blocks* src = nullptr;
+  uint64_t rows = 0;
+  std::vector<int64_t> order;
+  size_t pos = 0;  // order[pos] is in use (once started)
+  bool started = false;
+
+  const uint32_t* lo() const { return src ? src->col_lo : nullptr; }
+  uint64_t n_blocks() const { return src ? src->n_blocks : 0; }
+  int slot_of(size_t j) const { return src->slot[j % 2]; }
+  uint64_t row0() const { return started ? src->col_lo[order[pos]] : 0; }
+};
+
+// the checks of a streamed .x set: its block plan must cover its rows in order
+int sgda_check_blocks(const SgdaSet& s) {
+  const fmb200_xt_blocks& x = *s.src;
+  if (x.n_blocks == 0 || !x.col_lo || !x.nnz || !x.fetch || !x.release)
+    return fail("the %s .x blocks: no blocks or a null pointer", s.name);
+  if (x.n_cases && !x.target) return fail("the %s .x blocks: null target", s.name);
+  if (x.n_cases >= 0xffffffffull) return fail("the %s .x blocks: 2^32 rows and more are not supported", s.name);
+  for (int i = 0; i < 2; i++)
+    if (x.slot[i] < 0 || x.slot[i] >= FMB200_MAX_SLOTS) return fail("the %s .x blocks: slot out of range", s.name);
+  if (x.slot[0] == x.slot[1]) return fail("the %s .x blocks: the two slots must differ", s.name);
+  if (x.col_lo[0] != 0 || x.col_lo[x.n_blocks] != x.n_cases)
+    return fail("the %s .x blocks: the rows must start at 0 and end at n_cases", s.name);
+  for (uint64_t b = 0; b < x.n_blocks; b++) {
+    if (x.col_lo[b + 1] < x.col_lo[b]) return fail("the %s .x blocks: row ranges out of order", s.name);
+    if (x.nnz[b] >= 0xffffffffull) return fail("the %s .x blocks: a block of 2^32 entries and more", s.name);
+  }
+  return 0;
+}
+
+// Enqueue the copy and the decoding of order[j] into its slot on the copy stream
+int sgda_enqueue(fmb200_ctx* c, SgdaSet& s, size_t j) {
+  const uint64_t b = (uint64_t)s.order[j];
+  const void* words = nullptr;
+  const uint32_t* sizes = nullptr;
+  if (s.src->fetch(s.src->user, b, &words, &sizes) != 0)
+    return fail("fetching block %llu of the %s .x failed", (unsigned long long)b, s.name);
+  const uint32_t lo = s.src->col_lo[b];
+  return upload_xblock_enqueue(c, s.slot_of(j), s.src->col_lo[b + 1] - lo, s.src->nnz[b], words, sizes,
+                               s.src->target + lo, c->copy_stream);
+}
+
+// Make block b the one the next launches read: wait for its copy, release it, and start the copy of the block
+// after it into the other slot once the launches on that slot's block have run.
+int sgda_advance(fmb200_ctx* c, SgdaSet& s, int64_t b) {
+  if (b < 0 || (s.started && s.order[s.pos] == b)) return 0;
+  const size_t j = s.started ? s.pos + 1 : 0;
+  if (!s.started && sgda_enqueue(c, s, 0)) return 1;
+  s.started = true;
+  s.pos = j;
+  if (upload_finish(c, s.slot_of(j))) {
+    const std::string e = g_err;
+    return fail("block %lld of the %s .x: %s", (long long)b, s.name, e.c_str());
+  }
+  s.src->release(s.src->user, (uint64_t)b);
+  if (j + 1 < s.order.size()) {
+    CK(cudaStreamSynchronize(c->stream));  // order[j - 1], whose slot the next block takes, is done with
+    if (sgda_enqueue(c, s, j + 1)) return 1;
+  }
+  return 0;
+}
+
+// The epoch as sgda_plan cuts it, each streamed set's blocks fetched in the order its launches read them
+int sgda_run(fmb200_ctx* c, SgdaSet& tr, SgdaSet& va, int lambda_steps) {
+  const std::vector<SgdaLaunch> plan =
+      sgda_plan(tr.rows, va.rows, lambda_steps != 0, tr.lo(), tr.n_blocks(), va.lo(), va.n_blocks());
+  for (const SgdaLaunch& l : plan) {
+    if (tr.src && l.train_block >= 0 && (tr.order.empty() || tr.order.back() != l.train_block))
+      tr.order.push_back(l.train_block);
+    if (va.src && l.val_block >= 0 && (va.order.empty() || va.order.back() != l.val_block))
+      va.order.push_back(l.val_block);
+  }
+  for (const SgdaLaunch& l : plan) {
+    if (sgda_advance(c, tr, l.train_block) || sgda_advance(c, va, l.val_block)) return 1;
+    const DataSlot& ts = c->slots[tr.src ? tr.slot_of(tr.pos) : tr.slot];
+    // a streamed validation set no launch has read yet stands in as the training block (no lambda-steps read it)
+    const DataSlot& vs = va.src ? (va.started ? c->slots[va.slot_of(va.pos)] : ts) : c->slots[va.slot];
+    CK(launch_sgda(c, l, lambda_steps, ts, tr.row0(), tr.rows, vs, va.row0(), va.rows));
+  }
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int fmb200_sgda_epoch_x(fmb200_ctx* c, int train_slot, const fmb200_xt_blocks* train, int val_slot,
+                        const fmb200_xt_blocks* val, int lambda_steps, double* device_seconds) {
   NEED_CTX(c);
-  if (need_slot(c, train_slot) || need_slot(c, val_slot)) return 1;
+  if ((!train && need_slot(c, train_slot)) || (!val && need_slot(c, val_slot))) return 1;
   if (bind(c)) return 1;
   if (need_fp64(c, "SGDA runs on the fp64 state: set INORDER or ORDERED mode first")) return 1;
   if (c->sgda_groups == 0) return fail("call fmb200_sgda_begin first");
-  return timed(c, device_seconds, [&]() -> int {
-    CK(launch_sgda_epoch(c, c->slots[train_slot], c->slots[val_slot], lambda_steps));
-    c->sgda_moments_ready = true;
-    return 0;
+  SgdaSet tr{"training", train_slot, train}, va{"validation", val_slot, val};
+  for (SgdaSet* s : {&tr, &va}) {
+    if (!s->src) {
+      s->rows = c->slots[s->slot].n_rows;
+      continue;
+    }
+    if (c->peer_world > 1) return fail("a streamed SGDA epoch runs on one GPU: this context has peers");
+    if (sgda_check_blocks(*s)) return 1;
+    s->rows = s->src->n_cases;
+  }
+  {  // a streamed set's slots serve it alone
+    std::vector<int> res, str;
+    for (SgdaSet* s : {&tr, &va})
+      if (s->src) str.insert(str.end(), {s->src->slot[0], s->src->slot[1]});
+      else res.push_back(s->slot);
+    for (size_t i = 0; i < str.size(); i++) {
+      for (size_t j = 0; j < i; j++)
+        if (str[i] == str[j]) return fail("a streamed set's slots must differ from every other slot in use");
+      for (int r : res)
+        if (str[i] == r) return fail("a streamed set's slots must differ from every other slot in use");
+    }
+  }
+  if ((train || val) && c->copy_stream == nullptr) CK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
+  return guarded([&]() -> int {
+    return timed(c, device_seconds, [&]() -> int {
+      if (sgda_run(c, tr, va, lambda_steps)) {
+        if (train || val) cudaStreamSynchronize(c->copy_stream);  // no copy may still read a fetched block
+        return 1;
+      }
+      c->sgda_moments_ready = true;
+      return 0;
+    });
   });
+}
+
+int fmb200_sgda_epoch(fmb200_ctx* c, int train_slot, int val_slot, int lambda_steps, double* device_seconds) {
+  return fmb200_sgda_epoch_x(c, train_slot, nullptr, val_slot, nullptr, lambda_steps, device_seconds);
 }
 
 int fmb200_sgda_get_moments(fmb200_ctx* c, double* var_w, double* var_v) {

@@ -288,11 +288,12 @@ __global__ void __launch_bounds__(32, 1) fm_sgda_epoch_kernel(const SgdaArgs a) 
   uint64_t vc = a.vc0;
   for (uint64_t r = a.h_begin / 2; 2 * r < a.h_end; r++) {
     if (2 * r >= a.h_begin) {  // ---- sgd_theta_step, :136-169 ----
-      const uint64_t beg = a.row_ptr[r];
-      const uint32_t size = (uint32_t)(a.row_ptr[r + 1] - beg);
+      const uint64_t rb = r - a.train_row0;
+      const uint64_t beg = a.row_ptr[rb];
+      const uint32_t size = (uint32_t)(a.row_ptr[rb + 1] - beg);
       const uint32_t* c = a.col + beg;
       const float* x = a.val + beg;
-      const float target = a.target[r];
+      const float target = a.target[rb];
       const double mult = sgda_grad_loss(a.hp, predict_row_exact<KF>(m, w0, c, x, size, sum, lane), target);
       if (m.k0) w0 -= lr * (mult + 2 * 0.0 * w0);  // reg_0 stays 0 (:60,79)
       if (m.k1 && lane == 0) {
@@ -326,11 +327,12 @@ __global__ void __launch_bounds__(32, 1) fm_sgda_epoch_kernel(const SgdaArgs a) 
     }
     if (a.lambda_steps && a.v_rows > 0 && 2 * r + 1 < a.h_end) {  // ---- sgd_lambda_step, :201-248 ----
       if (vc == a.v_rows) vc = 0;  // :302-305
-      const uint64_t beg = a.v_row_ptr[vc];
-      const uint32_t size = (uint32_t)(a.v_row_ptr[vc + 1] - beg);
+      const uint64_t sb = vc - a.val_row0;
+      const uint64_t beg = a.v_row_ptr[sb];
+      const uint32_t size = (uint32_t)(a.v_row_ptr[sb + 1] - beg);
       const uint32_t* c = a.v_col + beg;
       const float* x = a.v_val + beg;
-      const float target = a.v_target[vc];
+      const float target = a.v_target[sb];
       vc++;
       const double grad_loss =
           sgda_grad_loss(a.hp, predict_row_exact<KF, false>(m, w0, c, x, size, sum, lane, w_dash, v_dash), target);
@@ -408,7 +410,15 @@ __global__ void fm_sgda_moments_kernel(Params64 p, uint32_t n, int k, double* __
   out[i] = var / n - mean * mean;
 }
 
-cudaError_t launch_sgda_epoch(fmb200_ctx* c, const DataSlot& tr, const DataSlot& va, int lambda_steps) {
+cudaError_t launch_sgda(fmb200_ctx* c, const SgdaLaunch& l, int lambda_steps, const DataSlot& tr, uint64_t tr_row0,
+                        uint64_t n_train, const DataSlot& va, uint64_t va_row0, uint64_t n_val) {
+  if (l.moments) {  // update_means (:298, :304-307)
+    fm_sgda_moments_kernel<<<(c->k + 32) / 32, 32, 0, c->stream>>>(c->p64, c->n, c->k, c->sgda_moments.get());
+    c->launches++;
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+  }
+  if (l.h_begin >= l.h_end) return cudaSuccess;
   SgdaArgs a;
   a.p = c->p64;
   a.grad_w = c->sgda_grad_w.get();
@@ -422,67 +432,50 @@ cudaError_t launch_sgda_epoch(fmb200_ctx* c, const DataSlot& tr, const DataSlot&
   a.use_w = c->k1;
   a.lambda_steps = lambda_steps;
   a.hp = c->hp;
-  a.n_rows = tr.n_rows;
+  a.n_rows = n_train;
+  a.v_rows = n_val;
+  a.h_begin = l.h_begin;
+  a.h_end = l.h_end;
+  a.vc0 = l.vc0;
+  a.train_row0 = tr_row0;
+  a.val_row0 = va_row0;
   a.row_ptr = tr.row_ptr.get();
   a.col = tr.col.get();
   a.val = tr.val.get();
   a.target = tr.target.get();
-  a.v_rows = va.n_rows;
   a.v_row_ptr = va.row_ptr.get();
   a.v_col = va.col.get();
   a.v_val = va.val.get();
   a.v_target = va.target.get();
   // The wavefront schedule is the default for eligible shapes (bit-identical to the one-warp kernel,
-  // tests/test_sgda_wavefront_gpu.py); variant 1 forces the one-warp kernel.
-  const bool lam = lambda_steps && va.n_rows > 0;
+  // tests/test_sgda_wavefront_gpu.py), chosen per launch from the blocks it reads; variant 1 forces the
+  // one-warp kernel.
+  const bool lam = lambda_steps && n_val > 0;
   const size_t wf_smem = sizeof(double) * (size_t)c->sgda_groups * (1 + (size_t)c->k);
   const bool wavefront = c->tune_variant != 1 &&
                          wavefront_fits(c->k, tr.max_row_nnz) && (!lam || wavefront_fits(c->k, va.max_row_nnz)) &&
                          sizeof(SgdaWindow) + wf_smem <= (size_t)c->max_smem_optin;
   const size_t smem = wavefront ? wf_smem : sgda_smem_bytes(c->sgda_groups, c->k);
   if (smem > (size_t)c->max_smem_optin) return cudaErrorInvalidConfiguration;  // fmb200_sgda_begin refuses it
-  auto run = [&](uint64_t h_begin, uint64_t h_end, uint64_t vc0) -> cudaError_t {
-    if (h_begin >= h_end) return cudaSuccess;
-    a.h_begin = h_begin;
-    a.h_end = h_end;
-    a.vc0 = vc0;
-    if (wavefront) {
-      const cudaError_t e =
-          cudaFuncSetAttribute(fm_sgda_wavefront_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      if (e != cudaSuccess) return e;
-      fm_sgda_wavefront_kernel<<<1, 32, smem, c->stream>>>(a);
-    } else {
-      const cudaError_t e = with_kf(c->k, [&](auto kf) {
-        auto kernel = fm_sgda_epoch_kernel<decltype(kf)::value>;
-        const cudaError_t e_ = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e_ != cudaSuccess) return e_;
-        kernel<<<1, 32, smem, c->stream>>>(a);
-        return cudaSuccess;
-      });
-      if (e != cudaSuccess) return e;
-    }
-    c->launches++;
-    return cudaGetLastError();
-  };
-  auto moments = [&]() -> cudaError_t {
-    fm_sgda_moments_kernel<<<(c->k + 32) / 32, 32, 0, c->stream>>>(c->p64, c->n, c->k, c->sgda_moments.get());
-    c->launches++;
-    return cudaGetLastError();
-  };
-  // The epoch's last update_means (:298, :304-307) comes at its start, or, when the validation cursor
-  // wraps, between theta-step t* = floor((N - 1) / V) * V and its lambda-step: the launch is cut there.
-  const uint64_t N = tr.n_rows, V = va.n_rows;
-  const uint64_t t_star = sgda_last_moments_step(N, V, lam);
-  cudaError_t e = cudaSuccess;
-  if (t_star == 0) {
-    if ((e = moments()) != cudaSuccess || (e = run(0, 2 * N, 0)) != cudaSuccess) return e;
-  } else if ((e = run(0, 2 * t_star + 1, 0)) != cudaSuccess || (e = moments()) != cudaSuccess ||
-             (e = run(2 * t_star + 1, 2 * N, V)) != cudaSuccess) {
-    return e;
+  if (wavefront) {
+    const cudaError_t e =
+        cudaFuncSetAttribute(fm_sgda_wavefront_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    fm_sgda_wavefront_kernel<<<1, 32, smem, c->stream>>>(a);
+  } else {
+    const cudaError_t e = with_kf(c->k, [&](auto kf) {
+      auto kernel = fm_sgda_epoch_kernel<decltype(kf)::value>;
+      const cudaError_t e_ = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      if (e_ != cudaSuccess) return e_;
+      kernel<<<1, 32, smem, c->stream>>>(a);
+      return cudaSuccess;
+    });
+    if (e != cudaSuccess) return e;
   }
+  c->launches++;
   c->last_cfg =
       wavefront ? wavefront_config((int)(sizeof(SgdaWindow) + smem)) : EpochConfig{32, 1, 1, 1, 32, (int)smem, 0};
-  return cudaSuccess;
+  return cudaGetLastError();
 }
 
 cudaError_t launch_sgd_inorder(fmb200_ctx* c, const DataSlot& d) {

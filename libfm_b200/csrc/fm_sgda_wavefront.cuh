@@ -13,6 +13,8 @@ namespace fmb {
 // training row t, 2t + 1 the lambda-step that follows it (skipped when lambda_steps == 0).  The
 // epoch is cut in two where the reference takes its last moments (update_means, :304-307), between
 // a theta-step and its lambda-step.  vc0 is the validation cursor at h_begin (v_rows = at the end).
+// Rows keep their global numbers t and s: the training arrays hold rows [train_row0, ...), the validation arrays
+// rows [val_row0, ...) (a streamed block; 0 when the set is resident).  A launch on a validation block never wraps.
 struct SgdaArgs {
   Params64 p;
   double* grad_w;        // [n]
@@ -25,6 +27,7 @@ struct SgdaArgs {
   HParams hp;
   uint64_t n_rows, v_rows;
   uint64_t h_begin, h_end, vc0;
+  uint64_t train_row0, val_row0;
   const uint64_t *row_ptr, *v_row_ptr;
   const uint32_t *col, *v_col;
   const float *val, *v_val, *target, *v_target;
@@ -103,15 +106,16 @@ __global__ void __launch_bounds__(32, 1) fm_sgda_wavefront_kernel(const SgdaArgs
     uint64_t beg = 0, end = 0;
     float ty = 0.f, ly = 0.f;
     if (has_theta) {
-      beg = a.row_ptr[p];
-      end = a.row_ptr[p + 1];
-      ty = a.target[p];
+      const uint64_t r = p - a.train_row0;
+      beg = a.row_ptr[r];
+      end = a.row_ptr[r + 1];
+      ty = a.target[r];
     }
     WfRow trow;
     trow.load(a.col, a.val, beg, end);
     beg = end = 0;
     if (has_lambda) {
-      const uint64_t s_row = (vstart + (p - p_first)) % a.v_rows;  // :302-305
+      const uint64_t s_row = (vstart + (p - p_first)) % a.v_rows - a.val_row0;  // :302-305
       beg = a.v_row_ptr[s_row];
       end = a.v_row_ptr[s_row + 1];
       ly = a.v_target[s_row];

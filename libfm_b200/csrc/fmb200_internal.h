@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "../../include/fmb200.h"
+#include "fm_sgda_plan.h"
 
 namespace fmb {
 
@@ -343,14 +344,10 @@ bool mcmc_get(const fmb200_ctx* c, double* alpha, double* w_mu, double* w_lambda
 inline size_t sgda_smem_bytes(uint32_t n_groups, int k) {
   return sizeof(double) * ((size_t)n_groups * (2 + 3 * (size_t)k));
 }
-// The step t* whose lambda-step follows the epoch's last update_means (:298, :302-307), 0 when that call
-// is the one at the epoch's start: the cursor over V validation rows restarts before the lambda-steps
-// t = V, 2V, ... of an epoch of N theta-steps.
-inline uint64_t sgda_last_moments_step(uint64_t n_train, uint64_t n_val, bool lambda_steps) {
-  if (!lambda_steps || n_val == 0 || n_train <= n_val) return 0;
-  return (n_train - 1) / n_val * n_val;
-}
-cudaError_t launch_sgda_epoch(fmb200_ctx* c, const DataSlot& tr, const DataSlot& va, int lambda_steps);
+// One launch of an SGDA epoch (fm_sgda_plan.h), after the moments kernel when l.moments.  tr holds training rows
+// [tr_row0, tr_row0 + tr.n_rows) of n_train, va validation rows [va_row0, ...) of n_val.
+cudaError_t launch_sgda(fmb200_ctx* c, const SgdaLaunch& l, int lambda_steps, const DataSlot& tr, uint64_t tr_row0,
+                        uint64_t n_train, const DataSlot& va, uint64_t va_row0, uint64_t n_val);
 // fm_hogwild.cu: throughput epoch
 cudaError_t launch_sgd_hogwild(fmb200_ctx* c, DataSlot& d);
 // fm_hogwild.cu: a fresh state clears the divergence flag of the row-lane epoch's accumulator

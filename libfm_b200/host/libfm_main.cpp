@@ -7,7 +7,8 @@
 // fp64 state, and so does `-method sgda` with its -validation set; in -mode hogwild sgda is refused with a
 // clear error instead of silently doing something else.
 // -cache_size streams a binary data set larger than it through the GPU block by block (one GPU): -method sgd
-// its .x, -method mcmc|als its transposed .xt (as the reference's data_t); text input loads the data whole.
+// and sgda its .x (sgda its validation set too), -method mcmc|als its transposed .xt (as the reference's
+// data_t); text input loads the data whole.
 //
 // New, optional flags (old command lines are unaffected):
 //   -mode hogwild|ordered|inorder   throughput (default); sequentially consistent fp64 (parallel over
@@ -67,17 +68,17 @@ static int run(const CmdLine& cmd, const std::string& method, std::chrono::stead
   };
 
   // (1) data, libfm.cpp:141-157.  -cache_size (bytes; 0 or absent: everything resident, the reference's
-  // unlimited), on one GPU: with -method sgd, a binary data set whose rows exceed one block of cache_size / 2
-  // bytes is read and trained on block by block (BinaryBlocks); with -method mcmc | als, one whose transposed
-  // file <file>.xt exists and whose columns exceed such a block is streamed from .xt and .y alone, .x unread
-  // (BinaryBlocks::open_xt; MCMC and ALS run in -mode inorder | ordered on one GPU, checked before loading).
-  // Train and test decide independently.  Text input ignores the flag, as in the reference; SGDA loads its
-  // data whole.
-  const long long cache_size = cmd.integer("gpus", 1) == 1 && !sgda ? cmd.integer64("cache_size", 0) : 0;
+  // unlimited), on one GPU: with -method sgd or sgda, a binary data set whose rows exceed one block of
+  // cache_size / 2 bytes is read and trained on block by block (BinaryBlocks; SGDA's validation set too); with
+  // -method mcmc | als, one whose transposed file <file>.xt exists and whose columns exceed such a block is
+  // streamed from .xt and .y alone, .x unread (BinaryBlocks::open_xt; SGDA, MCMC and ALS run in -mode inorder |
+  // ordered on one GPU, checked before loading).  Train, test and validation decide independently.  Text input
+  // ignores the flag, as in the reference.
+  const long long cache_size = cmd.integer("gpus", 1) == 1 ? cmd.integer64("cache_size", 0) : 0;
   auto load = [&](const std::string& file, SparseData& d) {
     std::unique_ptr<BinaryBlocks> b;
     if (cache_size > 0)
-      b = sgd ? BinaryBlocks::open(file, (uint64_t)cache_size) : BinaryBlocks::open_xt(file, (uint64_t)cache_size);
+      b = mcmc ? BinaryBlocks::open_xt(file, (uint64_t)cache_size) : BinaryBlocks::open(file, (uint64_t)cache_size);
     if (b) b->print();
     else d.load(file);
     return b;
@@ -89,17 +90,19 @@ static int run(const CmdLine& cmd, const std::string& method, std::chrono::stead
   SparseData test;
   const std::unique_ptr<BinaryBlocks> test_blocks = load(cmd.str("test"), test);
   SparseData validation;  // libfm.cpp:159-173
+  std::unique_ptr<BinaryBlocks> validation_blocks;
   if (cmd.has("validation") && !sgda)
     std::cout << "WARNING: Validation data is only used for SGDA. The data is ignored." << std::endl;
   if (sgda) {
     std::cout << "Loading validation set...\t" << std::endl;
-    validation.load(cmd.str("validation"));
+    validation_blocks = load(cmd.str("validation"), validation);
   }
   std::cout << "#relations: " << 0 << std::endl;
   std::cout << "Loading meta data...\t" << std::endl;
   uint32_t n = (uint32_t)std::max(train_blocks ? train_blocks->num_feature : train.num_feature,
                                   test_blocks ? test_blocks->num_feature : test.num_feature);  // :203
-  if (sgda) n = std::max(n, (uint32_t)validation.num_feature);  // :204-206
+  if (sgda)  // :204-206
+    n = std::max(n, (uint32_t)(validation_blocks ? validation_blocks->num_feature : validation.num_feature));
 
   HostModel fm;
   Learner fml;
@@ -164,6 +167,7 @@ static int run(const CmdLine& cmd, const std::string& method, std::chrono::stead
     validation.binarize_targets();  // :304-305
     if (train_blocks) train_blocks->binarize_targets();
     if (test_blocks) test_blocks->binarize_targets();
+    if (validation_blocks) validation_blocks->binarize_targets();
   } else {
     throw "unknown task";
   }
@@ -246,7 +250,7 @@ static int run(const CmdLine& cmd, const std::string& method, std::chrono::stead
 
   // learn, libfm.cpp:414-420
   fml.attach(train, test, train_blocks.get(), test_blocks.get());
-  if constexpr (sgda) fml.attach_validation(validation);
+  if constexpr (sgda) fml.attach_validation(validation, validation_blocks.get());
   const double t_attached = since_start();
   if constexpr (!mcmc) {
     fml.learn();

@@ -157,11 +157,14 @@ def write_transposed(data: Data, path_xt: str) -> None:
 class XtBlocks:
     """A data set streamed from its transposed file <file>.xt in the blocks the command line plans under
     -cache_size (read_xblocks: rows are features, ids are cases), for FmLearnSgdElement.mcmc_begin_xt.
-    `slots`: the two device slots its blocks pass through.  `fetches` counts the blocks handed to the library."""
+    `slots`: the two device slots its blocks pass through.  `fetches` counts the blocks handed to the library.
+    transposed=False reads a .x instead, in blocks of rows (cases), for FmLearnSgdElement.sgda_epoch_x."""
 
-    def __init__(self, path_xt: str, target, cache_size: int, slots=(2, 4)):
+    def __init__(self, path_xt: str, target, cache_size: int, slots=(2, 4), transposed: bool = True):
         head = np.fromfile(path_xt, dtype=np.uint32, count=6)
         self.num_feature, self.num_cases = int(head[4]), int(head[5])
+        if not transposed:
+            self.num_cases, self.num_feature = self.num_feature, self.num_cases
         self.target = np.ascontiguousarray(target, dtype=np.float32)
         if self.target.size != self.num_cases:
             raise FmError("case count of %s and its targets differ" % path_xt)
@@ -593,6 +596,21 @@ class FmLearnSgdElement:
         sec = C.c_double()
         self._check(self.lib.fmb200_sgda_epoch(self._ctx, self._slot_of(train), self._slot_of(validation),
                                                int(lambda_steps), C.byref(sec)))
+        return sec.value
+
+    def sgda_epoch_x(self, train, validation, lambda_steps: bool) -> float:
+        """fmb200_sgda_epoch_x: as sgda_epoch, each of train / validation either a Data (resident in a slot) or an
+        XtBlocks over its .x (transposed=False; streamed in its blocks).  Returns device seconds."""
+        keep, args = [], []
+        for d in (train, validation):
+            if isinstance(d, XtBlocks):
+                st, cb = d._struct()
+                keep.append((st, cb))
+                args += [-1, C.pointer(st)]
+            else:
+                args += [self._slot_of(d), None]
+        sec = C.c_double()
+        self._check(self.lib.fmb200_sgda_epoch_x(self._ctx, *args, int(lambda_steps), C.byref(sec)))
         return sec.value
 
     def sgda_reg(self):
