@@ -261,7 +261,21 @@ int fmb200_mcmc_runs(fmb200_ctx* ctx, uint32_t* n_runs);
  *  _get_moments: var_w and var_v[num_factor] of the last epoch's last update_means (:250-274), taken
  *          at the epoch's start or, when the validation cursor restarts, before the last restart's
  *          lambda-step; the means the reference logs with them are always 0 (:270-273).
- *  _get_reg and _get_moments serve _epoch and _epoch_x alike. */
+ *  _get_reg and _get_moments serve _epoch and _epoch_x alike.
+ *
+ * In HOGWILD mode the same entry points run SGDA as a windowed fp32 epoch (fm_sgda_hogwild.cu), for
+ * throughput.  The epoch is cut into windows of W consecutive training rows, the first at row 0 (W = 4096; for
+ * tests fmb200_set_tuning's rows_per_tile overrides it).  In each window every training row is scored from the
+ * state as the window found it and takes the reference's theta-step with reg as the previous window left it, its
+ * steps damped by the mean-field scale of the HOGWILD epoch (damp = -1 turns that off), rounded to 2^-32 and
+ * summed exactly; the window's stored gradient of every feature it names becomes the sum of its rows' gradients.
+ * Then, with lambda_steps, one lambda-step per theta-step reads the folded state, those gradients and the same
+ * reg, and reg <- max(0, reg + the window's summed lambda terms).  With W = 1 and no damping this is the
+ * reference's SGDA.  The moments are those of the state the lambda-steps read in the window holding the last
+ * cursor restart (the epoch's start without one).  Every sum is exact or in a fixed order, so an epoch computes
+ * the same bits on every run and at every grid size.  _begin also zeroes the fp32 w.  Limits: num_factor <= 128,
+ * n_groups * (num_factor + 1) <= 8192, one GPU, resident data sets (_epoch_x with blocks is refused); a step or
+ * gradient that is not finite or not below 2^11 turns the state into NaN. */
 int fmb200_sgda_begin(fmb200_ctx* ctx, uint32_t n_groups, const uint32_t* attr_group);
 int fmb200_sgda_epoch(fmb200_ctx* ctx, int train_slot, int val_slot, int lambda_steps, double* device_seconds);
 int fmb200_sgda_epoch_x(fmb200_ctx* ctx, int train_slot, const fmb200_xt_blocks* train, int val_slot,
@@ -322,7 +336,9 @@ int fmb200_last_epoch_dealt(fmb200_ctx* ctx, int* dealt);
  * of the epoch kernel, 1 = sub-warp row-group kernel, 2 = one-lane-per-row kernel
  * (k <= 8, rows of <= 4 entries; ignored when not applicable), 3 = its warp-specialised
  * form (producer warp + mbarrier hand-offs; bias read three tiles ahead), 5 = the one-lane-per-row
- * kernel on rows in file order (no deal; see fmb200_last_epoch_dealt).
+ * kernel on rows in file order (no deal; see fmb200_last_epoch_dealt).  rows_per_tile (1 .. 2^20): the SGD epochs
+ * take the tile of 32 .. 512 rows nearest below it; HOGWILD SGDA (fmb200_sgda_epoch) takes it as its window W,
+ * for tests, and damps unless damp = -1.
  * INORDER mode runs the wavefront schedule of the sequential epoch for k <= 8 and rows of <= 4
  * entries (conflict-free runs of examples gather and scatter in parallel, only the bias chain
  * stays serial; bit-identical to the row-at-a-time kernel, verified on the device); variant 1

@@ -763,10 +763,16 @@ int fmb200_predict(fmb200_ctx* c, int slot, int transform, double* out) {
 int fmb200_sgda_begin(fmb200_ctx* c, uint32_t n_groups, const uint32_t* attr_group) {
   NEED_CTX(c);
   if (bind(c)) return 1;
-  if (need_fp64(c, "SGDA runs on the fp64 state: set INORDER or ORDERED mode first")) return 1;
+  const bool hogwild = c->mode == FMB200_MODE_HOGWILD;
   if (n_groups == 0 || n_groups > 1024) return fail("n_groups must be in [1,1024]");
   if (n_groups > 1 && !attr_group) return fail("attr_group is required for more than one group");
-  if (sgda_smem_bytes(n_groups, c->k) > (size_t)c->max_smem_optin)
+  if (hogwild && c->k > 128) return fail("SGDA in HOGWILD mode supports num_factor <= 128 (got %d)", c->k);
+  if (hogwild && (uint64_t)n_groups * (c->k + 1) > kSgdaMaxTerms)
+    return fail("SGDA in HOGWILD mode with %u groups at num_factor = %d keeps %llu lambda terms per validation row "
+                "(groups * (num_factor + 1)); at most %llu: use at most %llu groups",
+                n_groups, c->k, (unsigned long long)n_groups * (c->k + 1), (unsigned long long)kSgdaMaxTerms,
+                (unsigned long long)(kSgdaMaxTerms / (c->k + 1)));
+  if (!hogwild && sgda_smem_bytes(n_groups, c->k) > (size_t)c->max_smem_optin)
     return fail("SGDA with %u groups at num_factor = %d needs %zu bytes of shared memory per block (8 * groups * "
                 "(2 + 3 * num_factor)); this device allows %d: use at most %zu groups",
                 n_groups, c->k, sgda_smem_bytes(n_groups, c->k), c->max_smem_optin,
@@ -794,7 +800,22 @@ int fmb200_sgda_begin(fmb200_ctx* c, uint32_t n_groups, const uint32_t* attr_gro
   CK(cudaMemsetAsync(c->sgda_grad_v.get(), 0, nk * sizeof(double), c->stream));
   CK(cudaMemsetAsync(c->sgda_reg_w.get(), 0, n_groups * sizeof(double), c->stream));
   CK(cudaMemsetAsync(c->sgda_reg_v.get(), 0, gk * sizeof(double), c->stream));
-  CK(cudaMemsetAsync(c->p64.w(), 0, n1 * sizeof(double), c->stream));
+  if (hogwild) {  // the fp32 stored gradients, their window sums and the stamps, beside the packed state
+    const uint64_t nf = c->p32.n_floats;
+    if (!c->sgda_grad32) {
+      CK(alloc(c->sgda_grad32, nf));
+      CK(alloc(c->sgda_gacc, nf));
+      CK(alloc(c->sgda_stamp, n1));
+    }
+    CK(cudaMemsetAsync(c->sgda_grad32.get(), 0, nf * sizeof(float), c->stream));
+    CK(cudaMemsetAsync(c->sgda_gacc.get(), 0, nf * sizeof(unsigned long long), c->stream));
+    CK(cudaMemsetAsync(c->sgda_stamp.get(), 0, n1 * sizeof(uint32_t), c->stream));
+    c->sgda_stamp_next = 1;
+    CK(cudaMemsetAsync(c->p32.w(), 0, (size_t)c->n * c->p32.ws * sizeof(float), c->stream));
+    CK(clear_acc_flag(c));
+  } else {
+    CK(cudaMemsetAsync(c->p64.w(), 0, n1 * sizeof(double), c->stream));
+  }
   if (attr_group) CK(cudaMemcpyAsync(c->sgda_group.get(), attr_group, c->n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
   else CK(cudaMemsetAsync(c->sgda_group.get(), 0, n1 * sizeof(uint32_t), c->stream));
   CK(cudaStreamSynchronize(c->stream));
@@ -903,8 +924,19 @@ int fmb200_sgda_epoch_x(fmb200_ctx* c, int train_slot, const fmb200_xt_blocks* t
   NEED_CTX(c);
   if ((!train && need_slot(c, train_slot)) || (!val && need_slot(c, val_slot))) return 1;
   if (bind(c)) return 1;
-  if (need_fp64(c, "SGDA runs on the fp64 state: set INORDER or ORDERED mode first")) return 1;
   if (c->sgda_groups == 0) return fail("call fmb200_sgda_begin first");
+  if (c->mode == FMB200_MODE_HOGWILD) {
+    if (train || val)
+      return fail("SGDA in HOGWILD mode takes resident data sets: streamed (.x block) SGDA runs in INORDER or "
+                  "ORDERED mode");
+    if (c->peer_world > 1) return fail("SGDA in HOGWILD mode runs on one GPU: this context has peers");
+    if (!c->sgda_grad32) return fail("call fmb200_sgda_begin in HOGWILD mode first");
+    return timed(c, device_seconds, [&]() -> int {
+      CK(launch_sgda_hogwild(c, c->slots[train_slot], c->slots[val_slot], lambda_steps));
+      c->sgda_moments_ready = true;
+      return 0;
+    });
+  }
   SgdaSet tr{"training", train_slot, train}, va{"validation", val_slot, val};
   for (SgdaSet* s : {&tr, &va}) {
     if (!s->src) {
@@ -1273,8 +1305,10 @@ int fmb200_set_tuning(fmb200_ctx* c, int ctas_per_sm, int rows_per_tile, int thr
   NEED_CTX(c);
   if (threads && (threads % 32 != 0 || threads < 32 || threads > 1024))
     return fail("threads must be a multiple of 32 in [32,1024]");
-  if (rows_per_tile && (rows_per_tile < 32 || rows_per_tile > 512))
-    return fail("rows_per_tile must be in [32,512]");
+  // the SGD epochs take the tile of 32 .. 512 rows nearest below it; HOGWILD SGDA takes it as its window, whose
+  // fixed-point sums hold up to 2^20 rows
+  if (rows_per_tile && (rows_per_tile < 1 || rows_per_tile > (1 << 20)))
+    return fail("rows_per_tile must be in [1,2^20]");
   c->tune_ctas_per_sm = ctas_per_sm;
   c->tune_rows_per_tile = rows_per_tile;
   c->tune_threads = threads;

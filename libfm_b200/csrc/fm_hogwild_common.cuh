@@ -186,10 +186,10 @@ __device__ __forceinline__ uint64_t ring_init(unsigned char* smem, int tid) {
 struct LossStep {
   float mult, curv;
 };
-__device__ __forceinline__ LossStep loss_step(const HogwildArgs& a, float p, float y) {
+__device__ __forceinline__ LossStep loss_step(int task, float min_target, float max_target, float p, float y) {
   LossStep l;
-  if (a.task == FMB200_TASK_REGRESSION) {
-    const float pc = fmaxf(a.min_target, fminf(a.max_target, p));
+  if (task == FMB200_TASK_REGRESSION) {
+    const float pc = fmaxf(min_target, fminf(max_target, p));
     l.mult = pc - y;
     const float den = p - y;
     l.curv = (pc == p) ? 1.f : (fabsf(den) > 1e-12f ? fminf(fmaxf(l.mult / den, 0.f), 1.f) : 0.f);
@@ -199,6 +199,9 @@ __device__ __forceinline__ LossStep loss_step(const HogwildArgs& a, float p, flo
     l.curv = sg * (1.f - sg);
   }
   return l;
+}
+__device__ __forceinline__ LossStep loss_step(const HogwildArgs& a, float p, float y) {
+  return loss_step(a.task, a.min_target, a.max_target, p, y);
 }
 
 // gamma(c, u) = (1 - (1-u)^c) / (c*u): scale of each of c concurrent steps whose

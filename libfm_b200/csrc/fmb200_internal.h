@@ -279,6 +279,15 @@ struct fmb200_ctx {
   bool sgda_moments_ready = false;   // an epoch has run since fmb200_sgda_begin
   fmb::DevPtr<uint32_t> sgda_group;
   uint32_t sgda_groups = 0;
+  // HOGWILD SGDA (fm_sgda_hogwild.cu): fp32 stored gradients and their window sums, beside the packed state
+  // element for element; the window stamp of every feature and the next epoch's first stamp; the lambda-steps'
+  // per-group terms of a window [W][groups * (k + 1)]
+  fmb::DevPtr<float> sgda_grad32;
+  fmb::DevPtr<unsigned long long> sgda_gacc;
+  fmb::DevPtr<uint32_t> sgda_stamp;
+  uint32_t sgda_stamp_next = 1;
+  fmb::DevPtr<double> sgda_part;
+  uint64_t sgda_part_cap = 0;
   int tune_damp = 0;  // 0 auto, 1 force on, -1 force off
   int tune_variant = 0;  // 0 auto, 1 row-group kernel, 2 row-lane kernel when eligible
   std::unique_ptr<fmb::McmcState, fmb::McmcDelete> mcmc;  // MCMC / ALS learner state (fm_mcmc.cu)
@@ -348,6 +357,13 @@ inline size_t sgda_smem_bytes(uint32_t n_groups, int k) {
 // [tr_row0, tr_row0 + tr.n_rows) of n_train, va validation rows [va_row0, ...) of n_val.
 cudaError_t launch_sgda(fmb200_ctx* c, const SgdaLaunch& l, int lambda_steps, const DataSlot& tr, uint64_t tr_row0,
                         uint64_t n_train, const DataSlot& va, uint64_t va_row0, uint64_t n_val);
+// fm_sgda_hogwild.cu: the windowed SGDA epoch of HOGWILD mode.  Its windows are kSgdaWindowRows training rows, or
+// fmb200_set_tuning's rows_per_tile when that is set; a window's lambda-steps keep groups * (k + 1) doubles each,
+// at most kSgdaMaxTerms.
+constexpr uint64_t kSgdaWindowRows = 4096;
+constexpr uint64_t kSgdaMaxTerms = 8192;
+uint64_t sgda_hogwild_window(const fmb200_ctx* c);
+cudaError_t launch_sgda_hogwild(fmb200_ctx* c, const DataSlot& tr, const DataSlot& va, int lambda_steps);
 // fm_hogwild.cu: throughput epoch
 cudaError_t launch_sgd_hogwild(fmb200_ctx* c, DataSlot& d);
 // fm_hogwild.cu: a fresh state clears the divergence flag of the row-lane epoch's accumulator

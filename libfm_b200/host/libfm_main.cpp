@@ -4,8 +4,8 @@
 // (reference src/libfm/libfm.cpp:62-441) and swaps the learner for one whose
 // passes over the data run in libfmb200 (include/fmb200.h).  `-method sgd` runs in every mode;
 // `-method mcmc|als` (data sets without relations, one GPU) run with -mode inorder or ordered, the
-// fp64 state, and so does `-method sgda` with its -validation set; in -mode hogwild sgda is refused with a
-// clear error instead of silently doing something else.
+// fp64 state, and so does `-method sgda` with its -validation set, which also runs in -mode hogwild as the
+// windowed fp32 epoch (resident data, one GPU).
 // -cache_size streams a binary data set larger than it through the GPU block by block (one GPU): -method sgd
 // and sgda its .x (sgda its validation set too), -method mcmc|als its transposed .xt (as the reference's
 // data_t); text input loads the data whole.
@@ -47,7 +47,8 @@ static Exec exec_of(const CmdLine& cmd, const std::string& method) {
     if (mode < 0) throw std::string("unknown -mode " + name);
     if (num_gpus < 1) throw "-gpus must be >= 1";
   } else {
-    if (mode != FMB200_MODE_INORDER && mode != FMB200_MODE_ORDERED)
+    // SGDA also runs in -mode hogwild, as the windowed fp32 epoch (fm_sgda_hogwild.cu)
+    if (mode != FMB200_MODE_INORDER && mode != FMB200_MODE_ORDERED && !(method == "sgda" && mode == FMB200_MODE_HOGWILD))
       throw std::string("method '" + method + "' is outside the libfm_b200 scope in -mode " + name +
                         " (the fp32 SGD path); use -mode inorder");
     if (num_gpus != 1) throw std::string("-method " + method + " runs on one GPU: -gpus must be 1");
@@ -342,12 +343,19 @@ int main(int argc, char** argv) {
       std::cout << "WARNING: -load_model enabled only for SGD and ALS." << std::endl;
       return 0;
     }
-    if (method == "sgda") {  // the fp64 modes only: SGDA is one chain of regularisation updates
+    if (method == "sgda") {  // the fp64 modes, and -mode hogwild with a validation set (the windowed epoch)
       const std::string mode = cmd.str("mode", "hogwild");
-      if (mode != "inorder" && mode != "ordered")
+      if (mode != "inorder" && mode != "ordered" && !(mode == "hogwild" && cmd.has("validation")))
         throw std::string("method '" + method + "' is outside the libfm_b200 scope (SGD hot path only); use -method sgd");
       if (!cmd.has("validation"))  // the reference asserts (libfm.cpp:277)
         throw "-method sgda needs a validation set (-validation) to learn the regularisation values on";
+      if (mode == "hogwild" && cmd.integer64("cache_size", 0) > 0) {  // checked before loading
+        std::string fx, fy;
+        for (const char* f : {"train", "test", "validation"})
+          if (SparseData::binary_pair(cmd.str(f), &fx, &fy))
+            throw "-method sgda in -mode hogwild trains on resident data: -cache_size streams binary data in -mode "
+                  "inorder or ordered; use -mode inorder";
+      }
     }
     if (method != "sgd" && method != "sgda" && method != "mcmc" && method != "als")
       throw "unknown method";  // libfm.cpp:291-293
