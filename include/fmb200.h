@@ -345,6 +345,30 @@ int fmb200_last_epoch_dealt(fmb200_ctx* ctx, int* dealt);
  * forces the row-at-a-time kernel. */
 int fmb200_set_tuning(fmb200_ctx* ctx, int ctas_per_sm, int rows_per_tile, int threads, int damp,
                       int variant);
+/* Reproducible HOGWILD SGD (on != 0): every fmb200_sgd_epoch[_async] in HOGWILD mode runs the windowed epoch
+ * (fm_sgd_window.cu), whatever k (<= 128) and row length.  Tiles are tile_rows consecutive rows in file order,
+ * windows window_tiles tiles, the first at row 0, the last tile and window what is left; 0 takes the default
+ * (256 rows, 64 tiles: windows of 16 384 rows).  Limits: tile_rows 1 .. 1024, window_tiles 1 .. 65 536.  In the
+ * first epoch after fmb200_set_params, with a bias, unless damp = -1, on more than 32 tiles, the first 4 windows
+ * are one tile each (the bias ramp).  Every row of a window is scored from the state as the window found it and
+ * takes the reference's SGD step (fm_sgd.h:38-50) -- a feature the row names twice takes two steps from that
+ * state --, damped by gamma(c_i, lr (h_joint + reg)) with c_i = count_i * min(N, flight) / N (flight = the window's
+ * rows, one tile in a ramp window), rounded to 2^-32 and summed exactly; the bias takes one damped step per tile
+ * from the tile's summed loss multipliers and curvatures, added in a fixed order; the sums are folded into the fp32
+ * state after the window.  Damping is on when the hottest feature's concurrency over a window matters
+ * (fmb200_set_tuning's damp forces it on or off).  The parameters after an epoch are a function of the state, the
+ * data, the hyperparameters and (tile_rows, window_tiles, damping) only: the same bits on every run, for every
+ * grid size, CTAs per SM, threads per CTA and SM count.  fmb200_set_tuning's ctas_per_sm and threads still pick
+ * the launch and change no result; its rows_per_tile and variant are ignored (variant 132
+ * prints the kernel's phase timers, a development aid).  fmb200_last_epoch_config reports
+ * the launch's grid and block and tile_rows as rows_per_tile.  Limits of exactness: a window adds at most
+ * S = min(window rows * longest row, nnz) steps to an element, and a step that is not finite or not below
+ * min(2^11, 2^31 / S) (so every sum stays below 2^63) turns the state into NaN.  A data set streamed in blocks
+ * (fmb200_upload_xblock) runs one epoch call per block, so windows restart at every block; with several GPUs each
+ * shard's epoch is reproducible, the exchange is not part of the claim.  INORDER and ORDERED epochs are
+ * deterministic already and HOGWILD SGDA is windowed already: the switch leaves them alone.  on = 0 restores
+ * the default dispatch. */
+int fmb200_set_reproducible(fmb200_ctx* ctx, int on, int tile_rows, int window_tiles);
 /* The dependency index ORDERED mode builds per data set (bit-exact index work, tested against a
  * host restatement): link[e] = e - (previous entry naming the same feature), rowdep[r] = r -
  * (nearest earlier row sharing a feature; 0 = the row names a feature twice); 0xffffffff = none.

@@ -9,7 +9,7 @@
 // prove the ABI fits (oracle/_ref/libFM_b200; exercised by tests/test_cli_gpu.py).
 //
 // FMB200_MODE=inorder|ordered|hogwild (environment; default hogwild) picks the execution mode,
-// FMB200_DEVICE the CUDA ordinal.
+// FMB200_DEVICE the CUDA ordinal, FMB200_REPRODUCIBLE=1 the windowed HOGWILD epoch (fmb200_set_reproducible).
 #ifndef FM_LEARN_SGD_B200_H_
 #define FM_LEARN_SGD_B200_H_
 
@@ -40,6 +40,8 @@ class fm_learn_sgd_b200 : public fm_learn_sgd {
     ck(fmb200_set_mode(ctx, (mode && !strcmp(mode, "inorder")) ? FMB200_MODE_INORDER
                             : (mode && !strcmp(mode, "ordered")) ? FMB200_MODE_ORDERED
                                                                  : FMB200_MODE_HOGWILD));
+    const char* repro = getenv("FMB200_REPRODUCIBLE");
+    if (repro && !strcmp(repro, "1")) ck(fmb200_set_reproducible(ctx, 1, 0, 0));
   }
 
   // the row loop of fm_learn_sgd_element::learn (fm_learn_sgd_element.h:48-78), one

@@ -92,6 +92,7 @@ SYMBOLS = {
     "fmb200_last_epoch_config": (C.c_int, [_ctx] + [_intp] * 7),
     "fmb200_last_epoch_dealt": (C.c_int, [_ctx, _intp]),
     "fmb200_set_tuning": (C.c_int, [_ctx, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "fmb200_set_reproducible": (C.c_int, [_ctx, C.c_int, C.c_int, C.c_int]),
     "fmb200_ordered_index": (C.c_int, [_ctx, C.c_int, _u32p, _u32p]),
 }
 

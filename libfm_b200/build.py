@@ -39,6 +39,7 @@ CU_SOURCES = {
     "fm_upload.cu": [],
     "fm_deal.cu": [],
     "fm_sgda_hogwild.cu": [],
+    "fm_sgd_window.cu": [],
     "fm_mcmc.cu": ["--fmad=false"],
 }
 CU_HEADERS = ["fm_device.cuh", "fm_rowgroup.cuh", "fm_hogwild_common.cuh", "fmb200_internal.h",

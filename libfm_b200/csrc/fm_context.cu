@@ -1317,4 +1317,15 @@ int fmb200_set_tuning(fmb200_ctx* c, int ctas_per_sm, int rows_per_tile, int thr
   return 0;
 }
 
+int fmb200_set_reproducible(fmb200_ctx* c, int on, int tile_rows, int window_tiles) {
+  NEED_CTX(c);
+  if (tile_rows < 0 || tile_rows > fmb::kWindowMaxTileRows) return fail("tile_rows must be in [1,1024] (0: 256)");
+  if (window_tiles < 0 || window_tiles > fmb::kWindowMaxTiles)
+    return fail("window_tiles must be in [1,65536] (0: 64)");
+  c->win_on = on != 0;
+  c->win_tile_rows = tile_rows ? tile_rows : (int)fmb::kWindowTileRows;
+  c->win_tiles = window_tiles ? window_tiles : (int)fmb::kWindowTiles;
+  return 0;
+}
+
 }  // extern "C"

@@ -570,6 +570,7 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, DataSlot& d, bool* handled) {
 cudaError_t launch_sgd_hogwild(fmb200_ctx* c, DataSlot& d) {
   if (c->kp / 4 > 32) return cudaErrorInvalidValue;  // num_factor <= 128 in this mode
   if (d.n_rows == 0) return cudaSuccess;
+  if (c->win_on) return launch_sgd_window(c, d);
   {
     bool handled = false;
     cudaError_t e = launch_rowlane(c, d, &handled);

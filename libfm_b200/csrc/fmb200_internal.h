@@ -224,6 +224,13 @@ struct EpochConfig {
   int dealt = 0;  // the row-lane epoch ran the dealt schedule
 };
 
+// The reproducible HOGWILD SGD epoch (fm_sgd_window.cu): tiles of kWindowTileRows rows, windows of kWindowTiles
+// tiles (W = 16 384 rows; scripts/sgd_window_study.py, DESIGN.md section 3.3) unless fmb200_set_reproducible sets
+// them, within the limits below; the first
+// kWindowRampTiles windows of the bias ramp are one tile each
+constexpr uint64_t kWindowTileRows = 256, kWindowTiles = 64, kWindowRampTiles = 4;
+constexpr int kWindowMaxTileRows = 1024, kWindowMaxTiles = 65536;
+
 }  // namespace fmb
 
 struct fmb200_ctx {
@@ -290,6 +297,16 @@ struct fmb200_ctx {
   uint64_t sgda_part_cap = 0;
   int tune_damp = 0;  // 0 auto, 1 force on, -1 force off
   int tune_variant = 0;  // 0 auto, 1 row-group kernel, 2 row-lane kernel when eligible
+  // the reproducible HOGWILD SGD epoch (fmb200_set_reproducible, fm_sgd_window.cu): on, its tile and window
+  // geometry; every feature's window stamp and the next epoch's first stamp, a window's touched features, its
+  // bias accumulators and list lengths, its rows' (mult, h_joint)
+  bool win_on = false;
+  int win_tile_rows = (int)fmb::kWindowTileRows, win_tiles = (int)fmb::kWindowTiles;
+  fmb::DevPtr<uint32_t> win_stamp, win_list;
+  uint32_t win_stamp_next = 1;
+  fmb::DevPtr<unsigned long long> win_aux;
+  fmb::DevPtr<float2> win_rows;
+  uint64_t win_rows_cap = 0;
   std::unique_ptr<fmb::McmcState, fmb::McmcDelete> mcmc;  // MCMC / ALS learner state (fm_mcmc.cu)
   // relation blocks for the next fmb200_mcmc_begin on these slots (fmb200_mcmc_set_relations), consumed by it
   std::vector<fmb::RelationHost> mcmc_rel;
@@ -366,6 +383,8 @@ uint64_t sgda_hogwild_window(const fmb200_ctx* c);
 cudaError_t launch_sgda_hogwild(fmb200_ctx* c, const DataSlot& tr, const DataSlot& va, int lambda_steps);
 // fm_hogwild.cu: throughput epoch
 cudaError_t launch_sgd_hogwild(fmb200_ctx* c, DataSlot& d);
+// fm_sgd_window.cu: the reproducible HOGWILD SGD epoch, windows of win_tiles tiles of win_tile_rows rows
+cudaError_t launch_sgd_window(fmb200_ctx* c, DataSlot& d);
 // fm_hogwild.cu: a fresh state clears the divergence flag of the row-lane epoch's accumulator
 cudaError_t clear_acc_flag(fmb200_ctx* c);
 // fm_hogwild.cu: build the dealt copy the row-lane epoch would run on this data set, if it would deal

@@ -8,6 +8,7 @@
 #include <chrono>
 #include <cmath>
 #include <cstdlib>
+#include <cstring>
 #include <fstream>
 #include <iomanip>
 #include <iostream>
@@ -377,6 +378,11 @@ class GpuSgdLearner : public GpuLearner {
     if (num_gpus > 1 && mode != FMB200_MODE_HOGWILD)
       throw std::string("-gpus > 1 requires -mode hogwild (the ordered / in-order epoch is one dependency chain)");
     create_contexts();
+    // FMB200_REPRODUCIBLE=1: HOGWILD epochs as windows of a constant number of rows, the same model on every run
+    // (per block with -cache_size, per shard with -gpus)
+    const char* repro = getenv("FMB200_REPRODUCIBLE");
+    if (repro && !strcmp(repro, "1"))
+      for (auto c : ctx_) ck(fmb200_set_reproducible(c, 1, 0, 0));
     // per-epoch exchange: NVLink peer-memory averaging when the devices can map each
     // other, NCCL otherwise (or when FMB200_CLI_NCCL is set)
     if (num_gpus > 1 && getenv("FMB200_CLI_NCCL") == nullptr) {

@@ -461,6 +461,11 @@ class FmLearnSgdElement:
         self._check(self.lib.fmb200_set_tuning(self._ctx, ctas_per_sm, rows_per_tile, threads, damp,
                                                variant))
 
+    def set_reproducible(self, on=True, tile_rows=0, window_tiles=0) -> None:
+        """HOGWILD SGD epochs as windows of tile_rows x window_tiles rows (0: 256 and 64): the same bits on every run
+        and grid (include/fmb200.h, fmb200_set_reproducible)."""
+        self._check(self.lib.fmb200_set_reproducible(self._ctx, int(bool(on)), tile_rows, window_tiles))
+
     def push_hparams(self) -> None:
         self._check(self.lib.fmb200_set_hparams(self._ctx, self.task, self.learn_rate, self.fm.reg0,
                                                 self.fm.regw, self.fm.regv, self.min_target,
