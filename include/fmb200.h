@@ -342,7 +342,11 @@ int fmb200_last_epoch_dealt(fmb200_ctx* ctx, int* dealt);
  * INORDER mode runs the wavefront schedule of the sequential epoch for k <= 8 and rows of <= 4
  * entries (conflict-free runs of examples gather and scatter in parallel, only the bias chain
  * stays serial; bit-identical to the row-at-a-time kernel, verified on the device); variant 1
- * forces the row-at-a-time kernel. */
+ * forces the row-at-a-time kernel.
+ * MCMC / ALS, read by fmb200_mcmc_begin: the sweeps over segments (relation blocks, streamed .xt blocks) sweep each
+ * stretch of narrow feature runs (no more features than the CTA has warps) with one CTA of `threads` threads
+ * (0: 256) and a CTA barrier between runs, and wide runs with the cooperative grid; variant 1 sweeps every run
+ * with the grid.  The results are the same bits either way. */
 int fmb200_set_tuning(fmb200_ctx* ctx, int ctas_per_sm, int rows_per_tile, int threads, int damp,
                       int variant);
 /* Reproducible HOGWILD SGD (on != 0): every fmb200_sgd_epoch[_async] in HOGWILD mode runs the windowed epoch

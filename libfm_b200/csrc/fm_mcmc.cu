@@ -50,6 +50,18 @@ constexpr double kAlpha0 = 1.0, kGamma0 = 1.0, kBeta0 = 1.0, kMu0 = 0.0, kW0Mean
 // device flag words
 enum { F_NAN_W = 0, F_INF_W, F_NAN_V, F_INF_V, F_SKIP, F_WORDS = 8 };
 
+// The CTA that sweeps narrow runs (mcmc_cta_sweep_kernel): kCtaSweepThreads threads by default, any multiple of 32
+// up to kCtaSweepMaxThreads through fmb200_set_tuning's threads; a run is narrow when it has at most as many
+// features as that CTA has warps (DESIGN §3.8)
+constexpr int kCtaSweepThreads = 256, kCtaSweepMaxThreads = 1024;
+
+// A stretch of consecutive runs [r_lo, r_hi) of one segment, swept by one launch: one CTA when they are all narrow,
+// the cooperative grid otherwise
+struct Stretch {
+  uint32_t r_lo, r_hi;
+  bool narrow;
+};
+
 // A data set streamed from blocks of its .xt (fmb200_mcmc_begin_xt)
 struct XtSet {
   fmb200_xt_blocks src{};
@@ -135,6 +147,9 @@ struct McmcState {
   // The id space in segments, each swept by its own launches: a streamed training set's blocks, or the main table
   // and then each relation block.  Segment i sweeps the runs [seg_run[i], seg_run[i + 1]).
   std::vector<uint32_t> seg_run;
+  // the launch plan: segment i's runs as maximal stretches of narrow and of wide runs, in order (plan_sweeps)
+  std::vector<std::vector<Stretch>> plan;
+  int cta_threads = kCtaSweepThreads;
   uint32_t iter = 0;
   uint32_t counters[16] = {0};
   // device
@@ -337,14 +352,14 @@ __device__ void draw_feature(const SweepArgs& a, uint32_t j, int f, int lane) {
   }
 }
 
-// runs [r_lo, r_hi)
-template <bool V, bool REL = false>
-__device__ void sweep_runs(const SweepArgs& a, cg::grid_group& grid, int f, uint32_t r_lo, uint32_t r_hi, uint32_t warp,
+// runs [r_lo, r_hi), sync() after each: a grid barrier, or a CTA barrier when one CTA sweeps them
+template <bool V, bool REL = false, class Sync>
+__device__ void sweep_runs(const SweepArgs& a, Sync sync, int f, uint32_t r_lo, uint32_t r_hi, uint32_t warp,
                            uint32_t nwarp, int lane) {
   for (uint32_t r = r_lo; r < r_hi; r++) {
     const uint32_t j1 = a.runs[r + 1];
     for (uint32_t j = a.runs[r] + warp; j < j1; j += nwarp) draw_feature<V, REL>(a, j, f, lane);
-    grid.sync();
+    sync();
   }
 }
 
@@ -366,11 +381,12 @@ __global__ void __launch_bounds__(256) mcmc_sweep_kernel(const SweepArgs a) {
     for (uint64_t c = tid; c < a.n_rows; c += nth) a.e[c] -= a.e_shift;
     grid.sync();
   }
-  if (a.use_w) sweep_runs<false>(a, grid, 0, 0, a.n_runs, warp, nwarp, lane);
+  auto sync = [&] { grid.sync(); };
+  if (a.use_w) sweep_runs<false>(a, sync, 0, 0, a.n_runs, warp, nwarp, lane);
   for (int f = 0; f < a.k; f++) {
     for (uint64_t c = tid; c < a.n_rows; c += nth) a.q[c] = main_q(a, c, f);  // the q rebuild
     grid.sync();
-    sweep_runs<true>(a, grid, f, 0, a.n_runs, warp, nwarp, lane);
+    sweep_runs<true>(a, sync, f, 0, a.n_runs, warp, nwarp, lane);
   }
 }
 
@@ -381,7 +397,19 @@ __global__ void __launch_bounds__(256) mcmc_block_sweep_kernel(const SweepArgs a
   cg::grid_group grid = cg::this_grid();
   const uint64_t tid = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
   const uint64_t nth = (uint64_t)gridDim.x * blockDim.x;
-  sweep_runs<V, REL>(a, grid, f, r_lo, r_hi, (uint32_t)(tid >> 5), (uint32_t)(nth >> 5), threadIdx.x & 31);
+  sweep_runs<V, REL>(a, [&] { grid.sync(); }, f, r_lo, r_hi, (uint32_t)(tid >> 5), (uint32_t)(nth >> 5),
+                     threadIdx.x & 31);
+}
+
+// The same sweep over narrow runs (no wider than the CTA has warps), by one CTA launched normally: a run's features
+// get a warp each, as in the grid, and __syncthreads() between runs stands for the grid barrier.  It orders and
+// makes visible every global write of the CTA's threads before the next run's reads, so each draw reads what it
+// reads in mcmc_block_sweep_kernel and the results are the same bits.  (One CTA per launch: the bound's 1 lets
+// ptxas use up to 64 registers, and it spills none.)
+template <bool V, bool REL = false>
+__global__ void __launch_bounds__(kCtaSweepMaxThreads, 1) mcmc_cta_sweep_kernel(const SweepArgs a, uint32_t r_lo,
+                                                                               uint32_t r_hi, int f) {
+  sweep_runs<V, REL>(a, [] { __syncthreads(); }, f, r_lo, r_hi, threadIdx.x >> 5, blockDim.x >> 5, threadIdx.x & 31);
 }
 
 // What a case adds from one block, in column order (the block's entries stably sorted by case):
@@ -763,14 +791,23 @@ const void* const kBlockSweep[2][2] = {
     {(const void*)mcmc_block_sweep_kernel<false, false>, (const void*)mcmc_block_sweep_kernel<false, true>},
     {(const void*)mcmc_block_sweep_kernel<true, false>, (const void*)mcmc_block_sweep_kernel<true, true>}};
 
-// The sweep of w (v = false) or of factor f over the runs [r_lo, r_hi) of one segment (rel: of a relation block),
-// one cooperative launch; nothing when there are no runs
-std::string launch_block_sweep(fmb200_ctx* c, const McmcState& s, const SweepArgs& a, bool v, bool rel, uint32_t r_lo,
-                               uint32_t r_hi, int f) {
-  if (r_lo >= r_hi) return "";
-  void* args[] = {(void*)&a, (void*)&r_lo, (void*)&r_hi, (void*)&f};
-  MK(cudaLaunchCooperativeKernel(kBlockSweep[v][rel], dim3(s.grid), dim3(256), args, 0, c->stream));
-  c->launches++;
+// mcmc_cta_sweep_kernel<V, REL> by [V][REL]
+const void* const kCtaSweep[2][2] = {
+    {(const void*)mcmc_cta_sweep_kernel<false, false>, (const void*)mcmc_cta_sweep_kernel<false, true>},
+    {(const void*)mcmc_cta_sweep_kernel<true, false>, (const void*)mcmc_cta_sweep_kernel<true, true>}};
+
+// The sweep of w (v = false) or of factor f over the runs of segment seg (rel: of a relation block), stretch by
+// stretch of the plan: a stretch of narrow runs is one launch of one CTA, a stretch of wide runs one cooperative
+// launch; nothing when the segment has no runs
+std::string launch_block_sweep(fmb200_ctx* c, const McmcState& s, const SweepArgs& a, bool v, bool rel, size_t seg,
+                               int f) {
+  for (const Stretch& st : s.plan[seg]) {
+    uint32_t r_lo = st.r_lo, r_hi = st.r_hi;
+    void* args[] = {(void*)&a, (void*)&r_lo, (void*)&r_hi, (void*)&f};
+    if (st.narrow) MK(cudaLaunchKernel(kCtaSweep[v][rel], dim3(1), dim3(s.cta_threads), args, 0, c->stream));
+    else MK(cudaLaunchCooperativeKernel(kBlockSweep[v][rel], dim3(s.grid), dim3(256), args, 0, c->stream));
+    c->launches++;
+  }
   return "";
 }
 
@@ -798,7 +835,7 @@ std::string xt_sweep(fmb200_ctx* c, McmcState& s, SweepArgs a) {
       }
       if (!sweep) return "";
       a.cols = Cols{d.row_ptr.get(), x.col_lo[b], x.col_lo[b + 1], d.col.get(), d.val.get()};
-      return launch_block_sweep(c, s, a, p >= 0, false, s.seg_run[b], s.seg_run[b + 1], p < 0 ? 0 : p);
+      return launch_block_sweep(c, s, a, p >= 0, false, b, p < 0 ? 0 : p);
     });
     if (!err.empty()) return err;
   }
@@ -941,14 +978,14 @@ std::string rel_upload(fmb200_ctx* c, McmcState& s, const RelationHost& h, RelDe
 std::string rel_sweep(fmb200_ctx* c, McmcState& s, const SweepArgs& a) {
   const uint64_t N = s.set[0].n;
   auto sweep = [&](bool v, int f) -> std::string {
-    std::string err = launch_block_sweep(c, s, a, v, false, s.seg_run[0], s.seg_run[1], f);
+    std::string err = launch_block_sweep(c, s, a, v, false, 0, f);
     for (uint32_t r = 0; err.empty() && r < s.rel.size(); r++) {
       SweepArgs b = a;
       b.rel = s.rel[r].view();
       b.cols = s.rel[r].cols();
       b.q = b.rel.q;
       MK(launch_for(c, b.rel.rows, v ? rel_unsync_kernel<true> : rel_unsync_kernel<false>, b.rel, a.e, a.q));
-      err = launch_block_sweep(c, s, b, v, true, s.seg_run[r + 1], s.seg_run[r + 2], f);
+      err = launch_block_sweep(c, s, b, v, true, r + 1, f);
       if (err.empty()) MK(launch_for(c, N, v ? rel_resync_kernel<true> : rel_resync_kernel<false>, b.rel, a.e, a.q, N));
     }
     return err;
@@ -1121,6 +1158,22 @@ std::string cut_runs(fmb200_ctx* c, McmcState& s, const std::vector<uint32_t>& p
   s.seg_run.push_back((uint32_t)s.runs.size() - 1);
   MK(to_device(c, s.runs_d, s.runs.data(), s.runs.size()));
   return "";
+}
+
+// The launch plan of the segmented sweeps: each segment's runs in maximal stretches of narrow runs (at most as many
+// features as the sweeping CTA has warps) and of wide runs.  fmb200_set_tuning's threads sets the CTA's width, and
+// its variant 1 makes every run wide (the cooperative kernel alone, for comparison).
+void plan_sweeps(const fmb200_ctx* c, McmcState& s) {
+  s.cta_threads = c->tune_threads ? c->tune_threads : kCtaSweepThreads;
+  const uint32_t warps = (uint32_t)s.cta_threads / 32;
+  s.plan.assign(s.seg_run.size() - 1, {});
+  for (size_t i = 0; i + 1 < s.seg_run.size(); i++)
+    for (uint32_t r = s.seg_run[i]; r < s.seg_run[i + 1]; r++) {
+      const bool narrow = c->tune_variant != 1 && s.runs[r + 1] - s.runs[r] <= warps;
+      std::vector<Stretch>& p = s.plan[i];
+      if (!p.empty() && p.back().narrow == narrow) p.back().r_hi = r + 1;
+      else p.push_back(Stretch{r, r + 1, narrow});
+    }
 }
 
 // The cooperative grid: as many blocks per SM as every sweep kernel the iteration launches fits
@@ -1436,6 +1489,7 @@ std::string mcmc_begin(fmb200_ctx* c, int train, int test, int do_sample, int do
   err = cut_runs(c, s, prev, seg);
   if (err.empty()) err = size_grid(c, s);
   if (!err.empty()) return err;
+  plan_sweeps(c, s);
 
   // fm_learn_mcmc_simultaneous.h:69-86: predict, then e := prediction - target (both tasks)
   err = repredict(c, s);

@@ -3,7 +3,7 @@
 // Keeps the reference's flags, defaults, stdout lines and file formats
 // (reference src/libfm/libfm.cpp:62-441) and swaps the learner for one whose
 // passes over the data run in libfmb200 (include/fmb200.h).  `-method sgd` runs in every mode;
-// `-method mcmc|als` (data sets without relations, one GPU) run with -mode inorder or ordered, the
+// `-method mcmc|als` (one GPU, with -relation blocks on resident data) run with -mode inorder or ordered, the
 // fp64 state, and so does `-method sgda` with its -validation set, which also runs in -mode hogwild as the
 // windowed fp32 epoch (resident data, one GPU).
 // -cache_size streams a binary data set larger than it through the GPU block by block (one GPU): -method sgd
@@ -98,7 +98,16 @@ static int run(const CmdLine& cmd, const std::string& method, std::chrono::stead
     std::cout << "Loading validation set...\t" << std::endl;
     validation_blocks = load(cmd.str("validation"), validation);
   }
-  std::cout << "#relations: " << 0 << std::endl;
+  // relation blocks (MCMC and ALS; the others have refused -relation), libfm.cpp:176-197: each block's .xt and
+  // .groups, then its joins of the train and test cases
+  const std::vector<std::string> rel_stems = cmd.list("relation");
+  std::cout << "#relations: " << rel_stems.size() << std::endl;
+  std::vector<GpuMcmcLearner::Relation> rel(rel_stems.size());
+  for (size_t r = 0; r < rel.size(); r++) {
+    rel[r].data.load(rel_stems[r]);
+    rel[r].join[0].load(rel_stems[r] + ".train", train.num_cases());
+    rel[r].join[1].load(rel_stems[r] + ".test", test.num_cases());
+  }
   std::cout << "Loading meta data...\t" << std::endl;
   uint32_t n = (uint32_t)std::max(train_blocks ? train_blocks->num_feature : train.num_feature,
                                   test_blocks ? test_blocks->num_feature : test.num_feature);  // :203
@@ -114,22 +123,21 @@ static int run(const CmdLine& cmd, const std::string& method, std::chrono::stead
     // counted in group 0
     fml.attr_group.assign(n, 0u);
     uint32_t G = 1;
-    if (cmd.has("meta")) {
-      std::ifstream in(cmd.str("meta").c_str());
-      if (!in.is_open()) throw "Unable to open file " + cmd.str("meta");
-      G = 0;
-      for (uint32_t i = 0; i < n; i++) {
-        unsigned int v = 0;
-        in >> v;
-        fml.attr_group[i] = v;
-        G = std::max(G, v + 1);
-      }
-    }
+    if (cmd.has("meta")) G = read_groups(cmd.str("meta"), n, fml.attr_group);
     if constexpr (sgda) {
       fml.n_groups = G;
     } else {
+      // the joined meta table, libfm.cpp:212-241: the blocks' attributes follow the main table's, each block's
+      // groups follow the groups before it
+      for (GpuMcmcLearner::Relation& b : rel) {
+        b.data.attr_offset = n;
+        n += b.data.num_feature;
+        for (uint32_t g : b.data.attr_group) fml.attr_group.push_back(G + g);
+        G += b.data.num_groups;
+      }
       fml.attr_per_group.assign(G, 0u);
       for (uint32_t i = 0; i < n; i++) fml.attr_per_group[fml.attr_group[i]]++;
+      fml.relations = std::move(rel);
     }
   }
 
@@ -361,9 +369,18 @@ int main(int argc, char** argv) {
       throw "unknown method";  // libfm.cpp:291-293
     // SGDA, MCMC and ALS refuse an out-of-scope -mode or -gpus before loading anything; SGD checks them after its model
     if (method != "sgd") exec_of(cmd, method);
-    if (!cmd.list("relation").empty()) {
+    if (!cmd.list("relation").empty()) {  // MCMC and ALS: resident relation blocks, -mode inorder | ordered, one GPU
       if (method == "sgd") throw "relations are not supported with SGD";  // fm_learn_sgd.h:61-63
-      throw std::string("relations (-relation) are not supported with -method " + method);
+      if (method == "sgda") throw std::string("relations (-relation) are not supported with -method " + method);
+      if (cmd.integer64("cache_size", 0) > 0)
+        throw "relations (-relation) are not supported with -cache_size: the relation blocks and the data sets are "
+              "held on the GPU whole; drop -cache_size";
+      // a block is read from its transposed binary file <stem>.xt alone (RelationData); a stem without one is
+      // refused as before, before the data sets are read.  The other files of a block are checked as they load,
+      // each error naming its file.
+      for (const std::string& stem : cmd.list("relation"))
+        if (!SparseData::file_exists(stem + ".xt"))
+          throw std::string("relations (-relation) are not supported with -method " + method);
     }
     if (method == "sgd") return run<GpuSgdLearner>(cmd, method, t_start);
     if (method == "sgda") return run<GpuSgdaLearner>(cmd, method, t_start);

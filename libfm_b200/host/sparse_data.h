@@ -13,6 +13,7 @@
 // larger than -cache_size is not loaded whole: BinaryBlocks plans its blocks and
 // BlockReader reads them, one pass at a time.
 #pragma once
+#include <algorithm>
 #include <condition_variable>
 #include <cstdint>
 #include <cstdio>
@@ -226,15 +227,15 @@ struct SparseData {
     return t;
   }
 
-  // The header of fx, checked against the n_rows targets of fy; leaves `in` at the first row.  transposed: fx is
-  // a .xt, whose columns are the cases.
+  // The header of fx, checked against the n_rows targets of fy (no check when fy is empty); leaves `in` at the
+  // first row.  transposed: fx is a .xt, whose columns are the cases.
   static XHeader read_header(std::ifstream& in, const std::string& fx, const std::string& fy, uint64_t n_rows,
                              bool transposed = false) {
     if (!in.is_open()) throw "could not open " + fx;
     XHeader fh;
     in.read(reinterpret_cast<char*>(&fh), sizeof(fh));
     if (!in || fh.id != 2 || fh.float_size != sizeof(float)) throw "could not read " + fx;
-    if ((transposed ? fh.num_cols : fh.num_rows) != n_rows)
+    if (!fy.empty() && (transposed ? fh.num_cols : fh.num_rows) != n_rows)
       throw std::string(transposed ? "case count of " : "row count of ") + fx + " and " + fy + " differ";
     // a truncated / corrupt header must not size the arrays: bound num_values by the file
     in.seekg(0, std::ios::end);
@@ -261,36 +262,42 @@ struct SparseData {
   static constexpr const char* data_target_[2] = {".data", ".target"};
   static constexpr const char* x_y_[2] = {".x", ".y"};
 
+ public:
+  // The binary matrix fx -- file_header (24 B), then per row {uint size; size x {uint id; float value}} -- into
+  // row_ptr, col and val (a .x, or a .xt whose rows are the features); fy and n_rows as in read_header
+  static XHeader read_matrix(const std::string& fx, const std::string& fy, uint64_t n_rows, bool transposed,
+                             std::vector<uint64_t>& row_ptr, std::vector<uint32_t>& col, std::vector<float>& val) {
+    std::ifstream in(fx.c_str(), std::ios::binary);
+    const XHeader fh = read_header(in, fx, fy, n_rows, transposed);
+    col.resize(fh.num_values);
+    val.resize(fh.num_values);
+    row_ptr.assign(1, 0);
+    row_ptr.reserve((size_t)fh.num_rows + 1);
+    std::vector<char> buf;
+    uint64_t pos = 0;
+    for (uint32_t r = 0; r < fh.num_rows; r++) {
+      uint32_t size = 0;
+      in.read(reinterpret_cast<char*>(&size), sizeof(size));
+      if (!in || pos + size > fh.num_values) throw "could not read " + fx;
+      buf.resize((size_t)size * 8);
+      in.read(buf.data(), buf.size());
+      if (!in) throw "could not read " + fx;
+      for (uint32_t j = 0; j < size; j++) {
+        memcpy(&col[pos + j], buf.data() + 8 * (size_t)j, 4);
+        memcpy(&val[pos + j], buf.data() + 8 * (size_t)j + 4, 4);
+      }
+      pos += size;
+      row_ptr.push_back(pos);
+    }
+    if (pos != fh.num_values) throw "could not read " + fx;
+    return fh;
+  }
+
+ private:
   void load_binary(const std::string& fx, const std::string& fy) {
     target = read_targets(fy);
-    // matrix: file_header (24 B) then per row {uint size; size x {uint id; float value}}
-    {
-      std::cout << "data... ";
-      std::ifstream in(fx.c_str(), std::ios::binary);
-      const XHeader fh = read_header(in, fx, fy, target.size());
-      col.resize(fh.num_values);
-      val.resize(fh.num_values);
-      row_ptr.assign(1, 0);
-      row_ptr.reserve((size_t)fh.num_rows + 1);
-      std::vector<char> buf;
-      uint64_t pos = 0;
-      for (uint32_t r = 0; r < fh.num_rows; r++) {
-        uint32_t size = 0;
-        in.read(reinterpret_cast<char*>(&size), sizeof(size));
-        if (!in || pos + size > fh.num_values) throw "could not read " + fx;
-        buf.resize((size_t)size * 8);
-        in.read(buf.data(), buf.size());
-        if (!in) throw "could not read " + fx;
-        for (uint32_t j = 0; j < size; j++) {
-          memcpy(&col[pos + j], buf.data() + 8 * (size_t)j, 4);
-          memcpy(&val[pos + j], buf.data() + 8 * (size_t)j + 4, 4);
-        }
-        pos += size;
-        row_ptr.push_back(pos);
-      }
-      if (pos != fh.num_values) throw "could not read " + fx;
-      num_feature = (int)fh.num_cols;
-    }
+    std::cout << "data... ";
+    num_feature = (int)read_matrix(fx, fy, target.size(), false, row_ptr, col, val).num_cols;
     for (float y : target) {  // Data.h:166-171
       if (y < min_target) min_target = y;
       if (y > max_target) max_target = y;
@@ -298,6 +305,92 @@ struct SparseData {
     std::cout << "num_cases=" << num_cases() << "\tnum_values=" << num_values()
               << "\tnum_features=" << num_feature << "\tmin_target=" << min_target
               << "\tmax_target=" << max_target << std::endl;
+  }
+};
+
+// DataMetaInfo::loadGroupsFromFile (Data.h:84-96), the rules of -meta and of a relation block's .groups: one group
+// id per attribute, read with >>, where a value the file lacks reads as 0.  group holds the n attributes' groups on
+// return; the result is the group count, 1 + the largest id.
+inline uint32_t read_groups(const std::string& file, uint32_t n, std::vector<uint32_t>& group) {
+  std::ifstream in(file.c_str());
+  if (!in.is_open()) throw "Unable to open file " + file;
+  group.assign(n, 0u);
+  uint32_t G = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    unsigned int v = 0;
+    in >> v;
+    group[i] = v;
+    G = std::max(G, v + 1);
+  }
+  return G;
+}
+
+// A relation block (block structure, BS) as the reference reads it for MCMC and ALS (relation.h:70-114): only its
+// transposed matrix <stem>.xt, whose rows are the block's features and whose columns are its rows, and its optional
+// <stem>.groups.  Every error names the file and starts with "relations: ".
+struct RelationData {
+  uint32_t num_cases = 0, num_feature = 0;
+  uint32_t attr_offset = 0;  // model id of feature 0, set after the main table's attributes (libfm.cpp:213-216)
+  std::vector<uint64_t> col_ptr{0};  // the .xt: feature j's entries at [col_ptr[j], col_ptr[j + 1])
+  std::vector<uint32_t> row;
+  std::vector<float> val;
+  std::vector<uint32_t> attr_group;  // [num_feature]: its DataMetaInfo, all 0 without a .groups file
+  uint32_t num_groups = 1;
+
+  void load(const std::string& stem) {
+    std::cout << "has x = " << 0 << std::endl;
+    std::cout << "has xt = " << 1 << std::endl;
+    std::cout << "data transpose... ";
+    try {
+      const SparseData::XHeader fh = SparseData::read_matrix(stem + ".xt", "", 0, true, col_ptr, row, val);
+      num_feature = fh.num_rows;
+      num_cases = fh.num_cols;
+      std::cout << "num_cases=" << num_cases << "\tnum_values=" << fh.num_values << "\tnum_features=" << num_feature
+                << std::endl;
+      attr_group.assign(num_feature, 0u);
+      num_groups = 1;
+      if (SparseData::file_exists(stem + ".groups")) num_groups = read_groups(stem + ".groups", num_feature, attr_group);
+    } catch (const std::string& e) {
+      throw "relations: " + e;
+    }
+  }
+};
+
+// RelationJoin::load (relation.h:127-150): a data set's case -> block row map, binary when the file starts with a
+// DVector<uint> header {1, 4}, else expected_rows whitespace-separated numbers.  Its length must be the data set's
+// case count.
+struct RelationJoin {
+  std::vector<uint32_t> rows;
+
+  void load(const std::string& file, uint64_t expected_rows) {
+    std::ifstream in(file.c_str(), std::ios::binary);
+    if (!in.is_open()) throw "relations: could not open " + file;
+    uint32_t hdr[3] = {0, 0, 0};
+    in.read(reinterpret_cast<char*>(hdr), 2 * sizeof(uint32_t));
+    const bool binary = in && hdr[0] == 1 && hdr[1] == sizeof(uint32_t);
+    uint64_t n = 0;
+    if (binary) {
+      in.read(reinterpret_cast<char*>(hdr + 2), sizeof(uint32_t));
+      if (!in) throw "relations: could not read " + file;
+      n = hdr[2];
+      if (n == expected_rows) {
+        rows.resize(n);
+        in.read(reinterpret_cast<char*>(rows.data()), sizeof(uint32_t) * n);
+        if (!in) throw "relations: could not read " + file;
+      }
+    } else {
+      in.clear();
+      in.close();
+      std::ifstream txt(file.c_str());
+      rows.clear();
+      rows.reserve(expected_rows);
+      unsigned int v;
+      while (rows.size() < expected_rows && txt >> v) rows.push_back(v);
+      n = rows.size();
+    }
+    if (n != expected_rows)
+      throw "relations: " + file + " maps " + std::to_string(n) + " cases, its data set has " +
+          std::to_string(expected_rows);
   }
 };
 

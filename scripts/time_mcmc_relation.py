@@ -1,12 +1,17 @@
 """Time one MCMC iteration on the full-size BS shape (make_relation_golden.bs_case) two ways.
 
-  python scripts/time_mcmc_relation.py [--reps 3] [--out FILE]
+  python scripts/time_mcmc_relation.py [--reps 3] [--phases] [--threads T] [--no-reference] [--out FILE]
 
   gpu        fmb200_mcmc_iteration with the two relation blocks (-mode inorder), host wall clock around the call,
              which returns after the iteration's last device work and host step; iterations 2 .. reps + 1 of one
              learner (the first warms up), median reported
   reference  the stock reference's time_learn (user time of its iteration on one host core) for the second
              iteration of oracle/_ref/libFM -method mcmc -relation user,item on the same files, from its -rlog
+  phases     (--phases) one more GPU iteration under torch.profiler: the device time of its kernels by phase (block
+             sweeps, unsync / resync, q rebuild, e-terms, the rest), from CUDA activity records; the iteration's wall
+             time less their sum is host work and launch gaps
+
+FMB200_LIB selects the library (_capi.py), so two builds can be timed in turn.
 
 Data: 1 000 209 train and 100 000 test ratings of MovieLens-1M shape with Zipf(1) popularity and empty main rows; a
 user block (6040 rows: the user's id and the items the user rated, 1/sqrt(#items)) and an item block (3706 rows),
@@ -45,7 +50,40 @@ def write_files(c, d: str) -> dict:
     return paths
 
 
-def gpu_ms(c, d: str, reps: int) -> list[float]:
+# phase -> substrings of the kernel names it takes (fm_mcmc.cu); REL_Q = 0, REL_ETERM = 1
+PHASES = (("block sweeps", ("mcmc_block_sweep_kernel", "mcmc_cta_sweep_kernel")),
+          ("unsync / resync", ("rel_unsync_kernel", "rel_resync_kernel")),
+          ("q rebuild", ("rel_row_kernel<0>", "rel_case_q_kernel")),
+          ("e-terms", ("rel_row_kernel<1>", "fm_eterm64_kernel")))
+
+
+def phase_ms(l) -> tuple[dict, float]:
+    """one iteration under torch.profiler: {phase: device ms} (kernels only) and the iteration's wall ms"""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.init()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        t0 = time.perf_counter()
+        l.mcmc_iteration()
+        wall = (time.perf_counter() - t0) * 1e3
+    out = {name: 0.0 for name, _ in PHASES}
+    out["other kernels"] = 0.0
+    n = 0
+    for e in prof.events():
+        us = getattr(e, "device_time_total", None)
+        if us is None:
+            us = e.cuda_time_total
+        if not us or e.name.startswith("cuda") or "Memcpy" in e.name or "Memset" in e.name:
+            continue  # kernels only
+        n += 1
+        name = next((p for p, keys in PHASES if any(k in e.name for k in keys)), "other kernels")
+        out[name] += us / 1e3
+    if n == 0:
+        raise RuntimeError("torch.profiler recorded no kernels of the iteration")
+    return out, wall
+
+
+def gpu_ms(c, d: str, reps: int, phases: bool = False, threads: int = 0):
     tr, te, k = c["train"], c["test"], c["k"]
     rel = []
     for stem in STEMS:
@@ -54,6 +92,8 @@ def gpu_ms(c, d: str, reps: int) -> list[float]:
                     RelationJoin.load(os.path.join(d, stem + ".test"), te.num_cases, b)))
     n = sum(b.num_feature for b, _, _ in rel)
     l = FmLearnSgdElement(FmModel(n, k), mode=MODE_INORDER)
+    if threads:
+        l.set_tuning(threads=threads)  # the width of the CTA that sweeps narrow runs
     l.upload(tr, 0)
     l.upload(te, 1)
     l.fm.init(42)
@@ -67,8 +107,9 @@ def gpu_ms(c, d: str, reps: int) -> list[float]:
         t0 = time.perf_counter()
         l.mcmc_iteration()
         out.append((time.perf_counter() - t0) * 1e3)
+    ph = phase_ms(l) if phases else None
     l.close()
-    return out
+    return out, ph
 
 
 def reference_ms(paths: dict, d: str, k: int) -> float | None:
@@ -100,12 +141,15 @@ def main() -> None:
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--out", help="also write the report to this file")
     ap.add_argument("--reference-only", action="store_true", help="skip the GPU (checks the reference command)")
+    ap.add_argument("--no-reference", action="store_true", help="skip the reference run")
+    ap.add_argument("--phases", action="store_true", help="also time one iteration's kernels by phase")
+    ap.add_argument("--threads", type=int, default=0, help="width of the narrow-run CTA (0: the library's)")
     a = ap.parse_args()
     c = bs_case()
     with tempfile.TemporaryDirectory() as d:
         paths = write_files(c, d)
-        g = [] if a.reference_only else gpu_ms(c, d, a.reps)
-        ref = reference_ms(paths, d, c["k"])
+        g, ph = ([], None) if a.reference_only else gpu_ms(c, d, a.reps, a.phases, a.threads)
+        ref = None if a.no_reference else reference_ms(paths, d, c["k"])
     nnz = [b["data"].num_values for b in c["blocks"]]
     lines = ["MCMC iteration, full-size BS shape: %d train / %d test cases, empty main rows, user block %d entries, "
              "item block %d entries, k = %d" % (c["train"].num_cases, c["test"].num_cases, nnz[0], nnz[1], c["k"]),
@@ -113,7 +157,14 @@ def main() -> None:
              "gpu        %10s ms  (runs: %s)" % ("%.1f" % sorted(g)[len(g) // 2] if g else "n/a",
                                                   ", ".join("%.1f" % x for x in g)),
              "reference  %10s ms  (stock libFM -method mcmc -relation, time_learn of iteration 1, one host core)"
-             % ("%.1f" % ref if ref is not None else "n/a")]
+             % ("%.1f" % ref if ref is not None else "n/a"),
+             "library    %s%s" % (os.environ.get("FMB200_LIB", "libfm_b200/lib/libfmb200.so"),
+                                 ", narrow-run CTA of %d threads" % a.threads if a.threads else "")]
+    if ph:
+        out, wall = ph
+        lines.append("phases of one profiled iteration (device ms of its kernels; wall %.1f ms):" % wall)
+        lines += ["  %-16s %8.1f ms" % (name, ms) for name, ms in out.items()]
+        lines.append("  %-16s %8.1f ms" % ("host and gaps", wall - sum(out.values())))
     text = "\n".join(lines) + "\n"
     sys.stdout.write(text)
     if a.out:
