@@ -764,14 +764,16 @@ int fmb200_sgda_begin(fmb200_ctx* c, uint32_t n_groups, const uint32_t* attr_gro
   NEED_CTX(c);
   if (bind(c)) return 1;
   const bool hogwild = c->mode == FMB200_MODE_HOGWILD;
-  if (n_groups == 0 || n_groups > 1024) return fail("n_groups must be in [1,1024]");
-  if (n_groups > 1 && !attr_group) return fail("attr_group is required for more than one group");
+  if (n_groups == 0) return fail("n_groups must be in [1,1024]");
   if (hogwild && c->k > 128) return fail("SGDA in HOGWILD mode supports num_factor <= 128 (got %d)", c->k);
+  // before the group cap: at num_factor = 7 both allow 1024 groups, and the refusal of 1025 names both
   if (hogwild && (uint64_t)n_groups * (c->k + 1) > kSgdaMaxTerms)
     return fail("SGDA in HOGWILD mode with %u groups at num_factor = %d keeps %llu lambda terms per validation row "
                 "(groups * (num_factor + 1)); at most %llu: use at most %llu groups",
                 n_groups, c->k, (unsigned long long)n_groups * (c->k + 1), (unsigned long long)kSgdaMaxTerms,
-                (unsigned long long)(kSgdaMaxTerms / (c->k + 1)));
+                (unsigned long long)std::min<uint64_t>(1024, kSgdaMaxTerms / (c->k + 1)));
+  if (n_groups > 1024) return fail("n_groups must be in [1,1024]");
+  if (n_groups > 1 && !attr_group) return fail("attr_group is required for more than one group");
   if (!hogwild && sgda_smem_bytes(n_groups, c->k) > (size_t)c->max_smem_optin)
     return fail("SGDA with %u groups at num_factor = %d needs %zu bytes of shared memory per block (8 * groups * "
                 "(2 + 3 * num_factor)); this device allows %d: use at most %zu groups",

@@ -107,6 +107,31 @@ def ragged(n_rows: int, num_feature: int, max_nnz: int, seed: int, empty_frac: f
     return Data(row_ptr, col, val, y, num_feature)
 
 
+def long_rows(n_rows: int, num_feature: int, max_nnz: int, seed: int, zipf: float = 0.0, twice: float = 0.05,
+              thrice: float = 0.05) -> Data:
+    """Long-row generator: 0 .. max_nnz entries (5 % of the rows empty), x in [0.5, 1.5], y in 1..5.  A
+    fraction `twice` of the rows names its first feature again at a later entry, a fraction `thrice` at two later
+    entries.  Ids are uniform, or Zipf(zipf) with feature 0 the hottest."""
+    r = np.random.default_rng(seed)
+    lens = r.integers(0, max_nnz + 1, size=n_rows)
+    lens[r.random(n_rows) < 0.05] = 0
+    row_ptr = np.zeros(n_rows + 1, dtype=np.uint64)
+    row_ptr[1:] = np.cumsum(lens)
+    nnz = int(row_ptr[-1])
+    if zipf > 0:
+        p = 1.0 / np.arange(1, num_feature + 1) ** zipf
+        col = r.choice(num_feature, size=nnz, p=p / p.sum()).astype(np.uint32)
+    else:
+        col = r.integers(0, num_feature, size=nnz).astype(np.uint32)
+    for times, frac in ((2, twice), (3, thrice)):
+        for row in np.flatnonzero((lens >= times) & (r.random(n_rows) < frac)):
+            a = int(row_ptr[row])
+            col[a + r.choice(np.arange(1, lens[row]), size=times - 1, replace=False)] = col[a]
+    val = r.uniform(0.5, 1.5, size=nnz).astype(np.float32)
+    y = r.integers(1, 6, size=n_rows).astype(np.float32)
+    return Data(row_ptr, col, val, y, num_feature)
+
+
 def to_libfm_text(data: Data, path: str) -> None:
     """Write `target id:value ...` lines (the format Data::load parses)."""
     with open(path, "w") as f:

@@ -33,6 +33,10 @@ EPS_M = 2e-6      # relative error of a step's fp32 products and of a tile's fp3
 EPS_GAMMA = 2e-4  # relative error of gamma: the exponent c log(1 - u) carries c times the error of __logf
 KAPPA = 0.1       # feed-forward of earlier windows' differences, per window
 GAMMA_CUT_JUMP = 5e-4  # gamma drops from 1 to 1 - q/2 at its q < 1e-3 cut; fp32 may put c u on the other side
+# The windowed epochs' warp-per-row score (tests/window_model.py, oracle/sgda_window_model.py): each lane adds
+# n ceil(k / 32) terms in sequence, then a shuffle tree; the row-lane calibration above never saw such rows.
+EPS_SEQ = 2.0 ** -22  # error of an fp32 sum per term it adds in sequence, relative to the terms' magnitudes
+SEQ_EXTRA = 6         # the shuffle tree over 32 lanes (5 levels) and the bias add
 
 ACC_SCALE = 2.0 ** 32
 CLAMP_EDGE = 1e-5

@@ -23,6 +23,13 @@ With W = 1, no damping, no quantisation and fp64 state this is the reference's S
 (tests/test_sgda_window_model.py holds it to oracle/fm_oracle_sgda.c).  Beside the state the model carries the
 row-lane model's per-element budget (rowlane_model.Budget; the same constants) with two more terms: the steps a
 difference in reg moves (2 lr |reg - reg'| |theta|) and, for reg itself, REG_REL of every lambda contribution.
+
+eps_seq > 0 (EPS_SEQ) adds the term tests/window_model.py states for the windowed SGD epoch's warp-per-row score,
+which the row-lane calibration never saw: a lane adds n ceil(k / 32) terms in sequence before a 5-level shuffle
+tree, so with L = eps_seq (n ceil(k / 32) + SEQ_EXTRA) the score carries scale L (|w0| + sum_i |w_i x_i| +
+sum_f (sum_i |v_if x_i|)^2 + sum_i,f (v_if x_i)^2) more, each per-factor sum s_f (and so each V gradient) L sum_i
+|v_if x_i|, and h_row, which damped steps read, L (xx + 3 |xx - 2| sum_f (sum_i |v_if x_i|)^2 + sq) relative.  Only
+the theta-phase is fp32; the lambda-phase is fp64.  eps_seq = 0 (the default) leaves the budget as it was.
 """
 from __future__ import annotations
 
@@ -30,8 +37,8 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from .rowlane_model import (ACC_SCALE, EPS_GAMMA, EPS_M, EPS_P, KAPPA, Budget, HParams, State, gamma,
-                            gamma_cut_edge, loss_step, quantise, row_curvature, ulp32)
+from .rowlane_model import (ACC_SCALE, EPS_GAMMA, EPS_M, EPS_P, EPS_SEQ, KAPPA, SEQ_EXTRA, Budget, HParams,
+                            State, gamma, gamma_cut_edge, loss_step, quantise, row_curvature, ulp32)
 
 REG_REL = 2e-3  # relative difference of a lambda contribution: it is read from fp32 state within the budget
 
@@ -133,10 +140,11 @@ def _window_sum(idx, d, n, quant, fp32):
 
 def sgda_window_epoch(state: State, sg: Sgda, train, val, hp: HParams, W: int, lambda_steps: bool,
                       damp: bool = True, quant: bool = True, fp32: bool = True, budget: Budget | None = None,
-                      reg_budget: RegBudget | None = None, trace: list | None = None):
+                      reg_budget: RegBudget | None = None, trace: list | None = None, eps_seq: float = 0.0):
     """One windowed SGDA epoch over train (row_ptr, col, val, target) with validation set val.
     Returns (state, sgda, (var_w, var_v), budget, reg_budget); pass the budgets back to carry them on.
-    trace: a list that receives the state after each window's fold."""
+    trace: a list that receives the state after each window's fold.
+    eps_seq: the budget's term for the lanes' serial sums (EPS_SEQ; 0 leaves it out, see the module's notes)."""
     n, k = state.w.shape[0], state.v.shape[0]
     N, V = int(train.row_ptr.shape[0] - 1), int(val.row_ptr.shape[0] - 1)
     G = sg.reg_w.shape[0]
@@ -151,6 +159,8 @@ def sgda_window_epoch(state: State, sg: Sgda, train, val, hp: HParams, W: int, l
     conc_scale = np.float32(min(W, N) / N) if N else np.float32(1.0)
     cb = float(np.float32(min(W, N)))
     scale = 2.0 if hp.task == 0 else 1.0  # SGDA's regression loss is (p - y)^2: twice SGD's multiplier
+    lanes_seq = -(-k // 32)  # factors per lane
+    row_len = np.diff(train.row_ptr.astype(np.int64)).astype(np.float64)
     t_star = last_moments_step(N, V, lam)
     j_star = t_star // W if t_star > 0 else -1
     mom = mom_b = None
@@ -187,6 +197,13 @@ def sgda_window_epoch(state: State, sg: Sgda, train, val, hp: HParams, W: int, l
         p_abs = (abs(st.w0) if hp.k0 else 0.0) + np.bincount(er, weights=np.abs(wv * x), minlength=R) \
             + 0.5 * (abs_s ** 2).sum(0) + 0.5 * sq
         row_err = scale * EPS_P * (1.0 + p_abs) + EPS_M * np.abs(mult)
+        if eps_seq:  # the lanes' serial sums: the score, each per-factor sum s_f and h_row
+            seq = eps_seq * (row_len[r0:r1] * lanes_seq + SEQ_EXTRA)  # L of the module's notes, per row
+            abs_s2 = (abs_s * abs_s).sum(0)
+            row_err = row_err + scale * seq * ((abs(st.w0) if hp.k0 else 0.0) +
+                                             np.bincount(er, weights=np.abs(wv * x), minlength=R) + abs_s2 + sq)
+            rel_h = np.minimum(1.0, seq * (xx + 3.0 * np.abs(xx - 2.0) * abs_s2 + sq) / np.maximum(hrow, 1e-300)) \
+                * (hrow > 0)
 
         # a row steps a feature it names twice twice: the second step starts where the first one ended
         prev, last = _occurrences(er, ids)
@@ -221,6 +238,8 @@ def sgda_window_epoch(state: State, sg: Sgda, train, val, hp: HParams, W: int, l
         bv = sv * (lr * gv_abs * row_err[er] + EPS_M * lr * np.abs(me * x) * abs_s[:, er] + EPS_M * 2 * lr * rv * np.abs(vv)
                    + 2 * lr * rb.reg_v[g].T * np.abs(vv)) + 1.0 / ACC_SCALE \
             + np.abs(dv) * (EPS_GAMMA * damped + damped * gamma_cut_edge(c[None, :], uv) + edge[er])
+        if eps_seq:
+            bv = bv + sv * lr * np.abs(me * x) * (seq * abs_s)[:, er] + np.abs(dv) * damped * rel_h[er]
         for f in range(k):
             st.v[f] = _fold_sum(st.v[f], ids, dv[f], n, quant, fp32)
             bud.v[f] += grow * np.bincount(ids, weights=bv[f], minlength=n)
@@ -232,6 +251,8 @@ def sgda_window_epoch(state: State, sg: Sgda, train, val, hp: HParams, W: int, l
             bw = sw * (lr * np.abs(x) * row_err[er] + EPS_M * 2 * lr * rw * np.abs(wv)
                        + 2 * lr * rb.reg_w[g] * np.abs(wv)) + 1.0 / ACC_SCALE \
                 + np.abs(dw) * (EPS_GAMMA * damped + damped * gamma_cut_edge(c, uw) + edge[er])
+            if eps_seq:
+                bw = bw + np.abs(dw) * damped * rel_h[er]
             st.w = _fold_sum(st.w, ids, dw, n, quant, fp32)
             bud.w += grow * np.bincount(ids, weights=bw, minlength=n)
             sg.grad_w = np.where(touched, _window_sum(ids[keep], (me * x)[keep], n, quant, fp32), sg.grad_w)
@@ -242,6 +263,8 @@ def sgda_window_epoch(state: State, sg: Sgda, train, val, hp: HParams, W: int, l
             h_edge = edge * ((1.0 if damp else 0.0) * hrow + 1.0)
             b0 = gb * lr * row_err + 1.0 / ACC_SCALE + np.abs(db) * (
                 EPS_GAMMA * on + (gamma_cut_edge(cb, lr * hjoint) if on else 0.0) + np.minimum(1.0, h_edge))
+            if eps_seq and on:
+                b0 = b0 + np.abs(db) * rel_h
             st.w0 = float(_fold_sum(np.array([st.w0]), np.zeros(R, dtype=np.int64), db, 1, quant, fp32)[0])
             bud.w0 += grow * float(b0.sum())
         bud.windows += 1

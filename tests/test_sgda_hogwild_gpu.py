@@ -19,9 +19,9 @@ pytestmark = pytest.mark.gpu
 def _cls(d):
     return Data(d.row_ptr, d.col, d.val, np.where(d.target > 3, 1.0, -1.0).astype(np.float32), d.num_feature)
 
-def _learner(n, k, task, lr, tuning, k0=True, k1=True):
+def _learner(n, k, task, lr, tuning, k0=True, k1=True, stdev=0.1):
     fm = FmModel(n, k, k0, k1)
-    fm.init_stdev = 0.1
+    fm.init_stdev = stdev
     fm.init_numpy(42)
     l = FmLearnSgdElement(fm, device=0, mode=MODE_HOGWILD)
     l.task, l.learn_rate = task, lr
@@ -34,12 +34,16 @@ def _pull(l):
     l.pull_params()
     return State(float(l.fm.w0), l.fm.w.copy(), l.fm.v.copy())
 
-def run_case(name, train, val, k=8, task=0, G=1, W=None, damp=1, epochs=3, lr=0.01, k0=True, k1=True):
+def run_case(name, train, val, k=8, task=0, G=1, W=None, damp=1, epochs=3, lr=0.01, k0=True, k1=True, stdev=0.1,
+             eps_seq=0.0, ctas_per_sm=0):
+    """Hold `epochs` epochs to the model; eps_seq goes to its budget (sm.EPS_SEQ for long rows and wide k).
+    Returns the worst (theta / budget, reg / bound, moments / bound) over the epochs."""
     n = train.num_feature
     group = np.arange(n) % G
-    tuning = dict(rows_per_tile=W or 0, damp=damp)
-    l = _learner(n, k, task, lr, tuning, k0, k1)
+    tuning = dict(rows_per_tile=W or 0, damp=damp, ctas_per_sm=ctas_per_sm)
+    l = _learner(n, k, task, lr, tuning, k0, k1, stdev)
     hp = HParams(task, lr, min_target=1.0, max_target=5.0, k0=k0, k1=k1)
+    worst = np.zeros(3)
     try:
         l.upload(train, 0)
         l.upload(val, 1)
@@ -50,11 +54,12 @@ def run_case(name, train, val, k=8, task=0, G=1, W=None, damp=1, epochs=3, lr=0.
         for e in range(epochs):
             l.sgda_epoch(train, val, e > 0)
             want, sg, mom, bud, rb = sm.sgda_window_epoch(want, sg, train, val, hp, W or sm.DEFAULT_W, e > 0,
-                                                          damp=damp >= 0, budget=bud, reg_budget=rb)
+                                                          damp=damp >= 0, budget=bud, reg_budget=rb,
+                                                          eps_seq=eps_seq)
             got = _pull(l)
             b0, bw, bv = bud.bound(want)
             ratio = max(abs(got.w0 - want.w0) / b0, np.max(np.abs(got.w - want.w) / bw),
-                        np.max(np.abs(got.v - want.v) / bv))
+                        np.max(np.abs(got.v - want.v) / bv, initial=0.0))
             reg_w, reg_v = l.sgda_reg()
             tiny = 1e-300
             rr = max(np.max(np.abs(reg_w - sg.reg_w) / (rb.reg_w + tiny)),
@@ -68,8 +73,10 @@ def run_case(name, train, val, k=8, task=0, G=1, W=None, damp=1, epochs=3, lr=0.
             assert mr < 1.0, "epoch %d: the moments are %.2f bounds away from the model" % (e, mr)
             if e > 0 and lr > 0:
                 assert np.any(reg_v > 0) or np.any(reg_w > 0), "the lambda-steps did not move reg"
+            worst = np.maximum(worst, [ratio, rr, mr])
     finally:
         l.close()
+    return worst
 
 def _two_field(n_train, n_val, seed=3):
     return synth.split_rows(synth.two_field(n_train + n_val, 300, 200, seed=seed), n_train)

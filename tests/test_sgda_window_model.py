@@ -3,8 +3,15 @@
 tests/test_sgda_hogwild_gpu.py holds the HOGWILD SGDA kernel to this model, so the model is tied down first: to
 the reference's SGDA (oracle/fm_oracle_sgda.c) where the two must agree -- windows of one row, no damping, no
 quantisation, fp64 state --, to update_means at the window the moments rule names, to a two-window case worked
-out by hand, and, at the default window, to the reference's test RMSE on planted C2-shaped data.
+out by hand, and, at the default window, to the reference's test RMSE on planted C2-shaped data.  The budget's
+term for the kernel's serial sums (eps_seq) is checked too: left out, the model computes what it computed before
+the term existed, bit for bit; put in, it widens the budget and nothing else, by what a case worked out by hand
+gives.
 """
+import json
+import os
+from importlib import util
+
 import numpy as np
 import pytest
 
@@ -12,10 +19,19 @@ from libfm_b200 import Data, synth
 from oracle import HParams, Port, State
 from oracle import sgda_window_model as sm
 
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
-def _init(n, k, seed):
+
+def _script(name):
+    spec = util.spec_from_file_location(name, os.path.join(ROOT, "scripts", name + ".py"))
+    mod = util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    return mod
+
+
+def _init(n, k, seed, stdev=0.1):
     r = np.random.default_rng(seed)
-    v = np.asarray(0.1 * r.standard_normal((k, n)), dtype=np.float32).astype(np.float64)
+    v = np.asarray(stdev * r.standard_normal((k, n)), dtype=np.float32).astype(np.float64)
     return State(0.0, np.zeros(n), v)
 
 
@@ -23,10 +39,10 @@ def _cls(d):
     return Data(d.row_ptr, d.col, d.val, np.where(d.target > 3, 1.0, -1.0).astype(np.float32), d.num_feature)
 
 
-def _compare_w1(train, val, k, G, task, epochs=3, k0=True, k1=True, lr=0.01):
+def _compare_w1(train, val, k, G, task, epochs=3, k0=True, k1=True, lr=0.01, stdev=0.1):
     n = train.num_feature
     group = np.arange(n) % G
-    st = _init(n, k, 3)
+    st = _init(n, k, 3, stdev)
     hp = HParams(task, lr, min_target=1.0, max_target=5.0, k0=k0, k1=k1)
     o = Port(n, k, k0, k1)
     o.set_params(st.w0, st.w, st.v)
@@ -39,6 +55,7 @@ def _compare_w1(train, val, k, G, task, epochs=3, k0=True, k1=True, lr=0.01):
         for got, want in [(st.w0, o.w0.value), (st.w, o.w), (st.v, o.v), (sg.grad_w, o.grad_w),
                           (sg.grad_v, o.grad_v), (sg.reg_w, o.reg_w), (sg.reg_v, o.reg_v)]:
             np.testing.assert_allclose(got, want, rtol=0, atol=1e-12)
+    assert np.isfinite(st.v).all() and np.isfinite(sg.reg_v).all()
     assert e == 0 or np.any(sg.reg_v > 0)  # the lambda-steps moved reg
 
 
@@ -66,6 +83,89 @@ def test_windows_of_one_row_ragged_rows():
     train, val = synth.split_rows(d, 300)
     _compare_w1(train, val, 5, 3, 0)
     _compare_w1(_cls(train), _cls(val), 5, 3, 1)
+
+
+@pytest.mark.parametrize("k", [33, 100])
+def test_windows_of_one_row_long_rows_wide_k(k):
+    """Rows of 0-60 entries that name a feature two and three times, x in [0.5, 1.5], at k = 33 (a lane's second
+    factor) and k = 100, three groups, both tasks."""
+    d = synth.long_rows(300, 120, 60, seed=k)
+    train, val = synth.split_rows(d, 220)
+    _compare_w1(train, val, k, 3, 0, lr=0.002, stdev=0.02)
+    _compare_w1(_cls(train), _cls(val), k, 3, 1, epochs=2, lr=0.002, stdev=0.02)
+
+
+# ---- the budget's term for the lanes' serial sums (eps_seq) ----
+
+def test_default_eps_seq_is_the_recorded_model():
+    """eps_seq = 0, and leaving it out, compute what the model computed before the term existed, bit for bit:
+    state, stored gradients, reg, moments and both budgets (scripts/make_sgda_model_digests.py)."""
+    mk = _script("make_sgda_model_digests")
+    with open(os.path.join(ROOT, "tests", "golden", "sgda_window_model_digests.json")) as f:
+        want = json.load(f)
+    assert sorted(want) == sorted(mk.CASES)
+    for name in mk.CASES:
+        for kw in ({}, dict(eps_seq=0.0)):
+            got = mk.model_digests(name, **kw)
+            for e, (g, w) in enumerate(zip(got, want[name])):
+                bad = sorted(q for q in w if g[q] != w[q])
+                assert not bad, "%s %s epoch %d: %s differ" % (name, kw, e, bad)
+
+
+def test_eps_seq_widens_the_budget_only():
+    """eps_seq > 0 leaves the state, the SGDA state and the moments as they were, and makes no budget element
+    smaller; the V budget of every feature a row stepped grows, and grows more at larger k."""
+    mk = _script("make_sgda_model_digests")
+    for name in mk.CASES:
+        train, val, st0, sg0, hp, W, damp = mk.long_case(name)
+        runs = {}
+        for eps in (0.0, sm.EPS_SEQ):
+            st, sg, bud, rb = st0, sg0, None, None
+            for e in range(2):
+                st, sg, mom, bud, rb = sm.sgda_window_epoch(st, sg, train, val, hp, W, e > 0, damp=damp,
+                                                            budget=bud, reg_budget=rb, eps_seq=eps)
+            runs[eps] = (st, sg, mom, bud, rb)
+        (st, sg, mom, bud, rb), (st1, sg1, mom1, bud1, rb1) = runs[0.0], runs[sm.EPS_SEQ]
+        same = [(st.w0, st1.w0), (st.w, st1.w), (st.v, st1.v), (sg.grad_w, sg1.grad_w), (sg.grad_v, sg1.grad_v),
+                (sg.reg_w, sg1.reg_w), (sg.reg_v, sg1.reg_v), (mom[0], mom1[0]), (mom[1], mom1[1])]
+        for a, b in same:
+            assert np.array_equal(np.float64(a).view(np.uint64), np.float64(b).view(np.uint64)), name
+        for a, b in [(bud.w0, bud1.w0), (bud.w, bud1.w), (bud.v, bud1.v), (rb.reg_w, rb1.reg_w),
+                     (rb.reg_v, rb1.reg_v), (rb.var_w, rb1.var_w), (rb.var_v, rb1.var_v)]:
+            assert np.all(np.asarray(b) >= np.asarray(a)), name
+        stepped = np.bincount(train.col.astype(np.int64), minlength=train.num_feature) > 0
+        assert np.all(bud1.v[:, stepped] > bud.v[:, stepped]) and np.all(rb1.var_v > rb.var_v), name
+        assert bud1.w0 > bud.w0 and np.all(bud1.w[stepped] >= bud.w[stepped]), name
+
+
+def test_eps_seq_term_by_hand():
+    """One row of three entries (the first feature named twice), k = 40, one window, no damping: the V budget of
+    each entry grows by lr |mult x| L sum_i |v_f,i x_i| plus what the wider score error moves, with
+    L = eps_seq (3 ceil(40 / 32) + SEQ_EXTRA) = eps_seq 12."""
+    n, k, lr = 3, 40, 0.01
+    train = Data(np.array([0, 3]), np.array([0, 1, 0]), np.array([1.0, 0.5, 1.5]), np.array([4.0]), n)
+    val = Data(np.array([0, 1]), np.array([2]), np.array([1.0]), np.array([3.0]), n)
+    st = _init(n, k, 9)
+    hp = HParams(0, lr, min_target=1.0, max_target=5.0, k0=False)
+    eps = 1e-3
+    runs = [sm.sgda_window_epoch(st, sm.Sgda.begin(n, k), train, val, hp, 1, False, damp=False, eps_seq=e)
+            for e in (0.0, eps)]
+    (_, _, _, b0, _), (_, _, _, b1, _) = runs
+    x = train.val.astype(np.float64)
+    ids = train.col.astype(np.int64)
+    vx = st.v[:, ids] * x
+    abs_s = np.abs(vx).sum(1)
+    s = vx.sum(1)
+    L = eps * 12
+    term_score = 2 * L * (np.abs(st.w[ids] * x).sum() + (abs_s ** 2).sum() + (vx ** 2).sum())
+    p = st.w[ids] @ x + 0.5 * ((s ** 2).sum() - (vx ** 2).sum())
+    mult = 2 * (np.clip(p, 1.0, 5.0) - 4.0)
+    want = np.zeros((k, n))
+    for i, (f, xi) in enumerate(zip(ids, x)):
+        want[:, f] += lr * np.abs(s - st.v[:, f] * xi) * abs(xi) * term_score + lr * abs(mult * xi) * L * abs_s
+    # the second step of feature 0 starts where the first ended: its gradient reads v + step, not v, which moves
+    # the by-hand |s - v x| by far less than the 1e-6 relative tolerance
+    np.testing.assert_allclose(b1.v - b0.v, want, rtol=1e-6, atol=0)
 
 
 def test_zero_gradient_is_stored():

@@ -18,13 +18,11 @@ from __future__ import annotations
 
 import numpy as np
 
-from oracle.rowlane_model import (ACC_SCALE, EPS_GAMMA, EPS_M, EPS_P, KAPPA, Budget, HParams, State, _exact_sums,
-                                  fold, gamma, gamma_cut_edge, loss_step, quantise, row_curvature, windows)
+from oracle.rowlane_model import (ACC_SCALE, EPS_GAMMA, EPS_M, EPS_P, EPS_SEQ, KAPPA, SEQ_EXTRA, Budget, HParams,
+                                  State, _exact_sums, fold, gamma, gamma_cut_edge, loss_step, quantise, row_curvature,
+                                  windows)
 
 __all__ = ["EPS_SEQ", "SEQ_EXTRA", "window_epoch_model", "Budget", "HParams", "State"]
-
-EPS_SEQ = 2.0 ** -22  # error of an fp32 sum per term it adds in sequence, relative to the terms' magnitudes
-SEQ_EXTRA = 6         # the shuffle tree over 32 lanes (5 levels) and the bias add
 
 
 def window_epoch_model(state: State, data, hp: HParams, T: int, B: int, damp: bool, ramp_tiles: int,
