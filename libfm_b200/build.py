@@ -42,7 +42,7 @@ CU_SOURCES = {
     "fm_sgd_window.cu": [],
     "fm_mcmc.cu": ["--fmad=false"],
 }
-CU_HEADERS = ["fm_device.cuh", "fm_rowgroup.cuh", "fm_hogwild_common.cuh", "fmb200_internal.h",
+CU_HEADERS = ["fm_device.cuh", "fm_rowgroup.cuh", "fm_hogwild_common.cuh", "fm_window.cuh", "fmb200_internal.h",
               "fm_inorder_wavefront.cuh", "fm_sgda_wavefront.cuh", "fm_sgda_plan.h", "fm_loss.cuh", "fm_ordered.cuh", "fm_roworder.cuh", "ref_random.h"]
 
 

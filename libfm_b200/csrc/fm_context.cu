@@ -802,17 +802,14 @@ int fmb200_sgda_begin(fmb200_ctx* c, uint32_t n_groups, const uint32_t* attr_gro
   CK(cudaMemsetAsync(c->sgda_grad_v.get(), 0, nk * sizeof(double), c->stream));
   CK(cudaMemsetAsync(c->sgda_reg_w.get(), 0, n_groups * sizeof(double), c->stream));
   CK(cudaMemsetAsync(c->sgda_reg_v.get(), 0, gk * sizeof(double), c->stream));
-  if (hogwild) {  // the fp32 stored gradients, their window sums and the stamps, beside the packed state
+  if (hogwild) {  // the fp32 stored gradients and their window sums, beside the packed state
     const uint64_t nf = c->p32.n_floats;
     if (!c->sgda_grad32) {
       CK(alloc(c->sgda_grad32, nf));
       CK(alloc(c->sgda_gacc, nf));
-      CK(alloc(c->sgda_stamp, n1));
     }
     CK(cudaMemsetAsync(c->sgda_grad32.get(), 0, nf * sizeof(float), c->stream));
     CK(cudaMemsetAsync(c->sgda_gacc.get(), 0, nf * sizeof(unsigned long long), c->stream));
-    CK(cudaMemsetAsync(c->sgda_stamp.get(), 0, n1 * sizeof(uint32_t), c->stream));
-    c->sgda_stamp_next = 1;
     CK(cudaMemsetAsync(c->p32.w(), 0, (size_t)c->n * c->p32.ws * sizeof(float), c->stream));
     CK(clear_acc_flag(c));
   } else {

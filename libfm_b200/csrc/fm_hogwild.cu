@@ -369,10 +369,26 @@ static HogwildArgs make_args(fmb200_ctx* c, const DataSlot& d, uint64_t n_tiles,
   return a;
 }
 
-// The fixed-point accumulator of the reproducible row-lane epoch: one u64 per float of the packed state,
-// then the flag word of acc_add (set when a step was not finite or too large for the fixed point).
-// Allocated zeroed on first use; every launch leaves the steps zero behind it.
+// The fixed-point accumulator of the reproducible epochs (the row-lane epoch here, the windowed SGD and SGDA
+// epochs of fm_window.cuh): one u64 per float of the packed state, then the flag word of acc_add (set when a step
+// was not finite or too large for the fixed point).  Allocated zeroed on first use; every launch leaves the steps
+// zero behind it.
 static unsigned long long* acc_flag(fmb200_ctx* c) { return c->d_acc.get() + c->p32.n_floats; }
+
+cudaError_t acc_ready(fmb200_ctx* c, unsigned long long** steps, unsigned long long** flag) {
+  if (!c->d_acc) {
+    const uint64_t words = c->p32.n_floats + 1;
+    cudaError_t e = alloc(c->d_acc, words);
+    if (e == cudaSuccess) e = cudaMemsetAsync(c->d_acc.get(), 0, words * sizeof(unsigned long long), c->stream);
+    if (e != cudaSuccess) {
+      c->d_acc.reset();
+      return e;
+    }
+  }
+  *steps = c->d_acc.get();
+  if (flag) *flag = acc_flag(c);
+  return cudaSuccess;
+}
 
 cudaError_t clear_acc_flag(fmb200_ctx* c) {
   return c->d_acc ? cudaMemsetAsync(acc_flag(c), 0, sizeof(unsigned long long), c->stream) : cudaSuccess;
@@ -501,17 +517,12 @@ static cudaError_t launch_rowlane(fmb200_ctx* c, DataSlot& d, bool* handled) {
     // its steps are folded in after it: the same result on every run.  A ramp window is one tile.
     const uint64_t n_acc = c->p32.n_floats;
     if (n_acc % 4 != 0) return cudaErrorInvalidValue;  // the fold takes float4s (Params32: blocks of 4 floats)
-    if (!c->d_acc) {
-      if ((e = alloc(c->d_acc, n_acc + 1)) != cudaSuccess) return e;
-      e = cudaMemsetAsync(c->d_acc.get(), 0, (n_acc + 1) * sizeof(unsigned long long), c->stream);
-      if (e != cudaSuccess) return e;
-    }
-    unsigned long long* acc = c->d_acc.get();
+    unsigned long long* acc = nullptr;
+    if ((e = acc_ready(c, &acc, &a.acc_bad)) != cudaSuccess) return e;
     float* base = c->p32.base;
     a.acc_w0 = acc + (a.w0 - base);
     a.acc_w = acc + (a.w - base);
     a.acc_v = acc + (a.v - base);
-    a.acc_bad = acc_flag(c);
     a.state = base;
     a.acc = acc;
     a.n_acc = n_acc;

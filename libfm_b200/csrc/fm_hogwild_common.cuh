@@ -122,10 +122,11 @@ __device__ __forceinline__ void acc_add(unsigned long long* p, float d, unsigned
   if (fabsf(d) < kAccStepMax) red_add_u64(p, (unsigned long long)__float2ll_rn(d * kAccScale));
   else atomicOr(bad, 1ull);  // also NaN: the comparison is false
 }
-// the value acc_add adds, for a caller that adds it in bulk: a step it would not add is 0
-__device__ __forceinline__ unsigned long long acc_quantise(float d, unsigned long long* bad) {
-  if (fabsf(d) < kAccStepMax) return (unsigned long long)__float2ll_rn(d * kAccScale);
-  atomicOr(bad, 1ull);
+// the value acc_add adds, for a caller that adds it in bulk: a step it would not add is 0.  A caller whose
+// windows add more steps to one element may pass a smaller cap.
+__device__ __forceinline__ unsigned long long acc_quantise(float d, unsigned long long* bad, float cap = kAccStepMax) {
+  if (fabsf(d) < cap) return (unsigned long long)__float2ll_rn(d * kAccScale);
+  atomicOr(bad, 1ull);  // also NaN: the comparison is false
   return 0ull;
 }
 

@@ -380,18 +380,6 @@ __global__ void __launch_bounds__(32, 1) fm_sgda_epoch_kernel(const SgdaArgs a) 
   for (uint32_t i = lane; i < G * (uint32_t)k; i += 32) a.reg_v[i] = s_reg_v[i];
 }
 
-// Factors per lane of the one-warp kernels: body(kf) runs with kf.value = KF in {1, 2, 4, 8}, the
-// smallest with 32 * KF >= k.  Lane l owns factors l, l + 32, ..., so k is at most 256.
-template <class Body>
-cudaError_t with_kf(int k, Body&& body) {
-  if (k > 32 * 8) return cudaErrorInvalidValue;
-  const int kf = (k + 31) / 32;
-  if (kf <= 1) return body(std::integral_constant<int, 1>());
-  if (kf <= 2) return body(std::integral_constant<int, 2>());
-  if (kf <= 4) return body(std::integral_constant<int, 4>());
-  return body(std::integral_constant<int, 8>());
-}
-
 // update_means (fm_learn_sgd_element_adapt_reg.h:250-274) over the fp64 state: thread 0 walks w, thread
 // 1 + f factor f, each one serial chain over j = 0..n-1.  The means it returns are zeroed (:270-273), so
 // only the variances are kept: out = [var_w | var_v[k]].
@@ -463,7 +451,7 @@ cudaError_t launch_sgda(fmb200_ctx* c, const SgdaLaunch& l, int lambda_steps, co
     if (e != cudaSuccess) return e;
     fm_sgda_wavefront_kernel<<<1, 32, smem, c->stream>>>(a);
   } else {
-    const cudaError_t e = with_kf(c->k, [&](auto kf) {
+    const cudaError_t e = with_kf<8>(c->k, [&](auto kf) {
       auto kernel = fm_sgda_epoch_kernel<decltype(kf)::value>;
       const cudaError_t e_ = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e_ != cudaSuccess) return e_;
@@ -497,7 +485,7 @@ cudaError_t launch_sgd_inorder(fmb200_ctx* c, const DataSlot& d) {
     c->last_cfg = wavefront_config(0);
     return cudaGetLastError();
   }
-  const cudaError_t e = with_kf(c->k, [&](auto kf) {
+  const cudaError_t e = with_kf<8>(c->k, [&](auto kf) {
     fm_sgd_inorder_kernel<decltype(kf)::value><<<1, 32, 0, c->stream>>>(
         c->p64, c->k, c->k0, c->k1, c->hp, d.n_rows, d.row_ptr.get(), d.col.get(), d.val.get(), d.target.get());
     return cudaSuccess;
@@ -510,7 +498,7 @@ cudaError_t launch_sgd_inorder(fmb200_ctx* c, const DataSlot& d) {
 
 cudaError_t launch_predict64(fmb200_ctx* c, const DataSlot& d, int transform, double* out_pred,
                              double* partials, int n_blocks) {
-  const cudaError_t e = with_kf(c->k, [&](auto kf) {
+  const cudaError_t e = with_kf<8>(c->k, [&](auto kf) {
     fm_predict64_kernel<decltype(kf)::value><<<n_blocks, 256, 0, c->stream>>>(
         c->p64, c->k, c->k0, c->k1, c->hp, transform, d.n_rows, d.row_ptr.get(), d.col.get(), d.val.get(),
         d.target.get(), out_pred, partials);

@@ -9,25 +9,23 @@
 //          the window found it and takes the reference's SGD step (fm_sgd.h:38-50) for every entry, damped by
 //          gamma(c_i, lr (h_joint + reg)) with c_i = count_i * min(N, flight) / N, quantised to 2^-32 and added to
 //          the fixed-point accumulator (fm_hogwild_common.cuh: exact in any order).  A feature the row names twice
-//          takes two steps, both from the window's state.  The first touch of a feature in the window (its stamp)
-//          appends it to the window's list.  The row's (mult, h_joint) goes to its slot of a per-row buffer.
+//          takes two steps, both from the window's state.  The first touch of a feature in the window goes to the
+//          window's list (window_touch).  The row's (mult, h_joint) goes to its slot of a per-row buffer.
 //   fold   a warp per tile sums the tile's (mult, h_joint) in a fixed order (lane l takes rows l, l + 32, ...; then
-//          the shuffle tree) and adds the tile's damped bias step to the window's bias accumulator; the accumulated
-//          steps of every feature on the list are folded into the fp32 state and cleared.  The bias itself folds
-//          at the start of the next window (each thread folds it into a register) and into the state at the end.
+//          the shuffle tree) and adds the tile's damped bias step to the window's bias accumulator; the listed
+//          features are folded into the fp32 state (window_fold).  The bias itself folds at the start of the next
+//          window (each thread folds it into a register) and into the state at the end.
 // A step that is not finite or not below the cap sets the divergence flag, and every later fold turns the whole
-// state NaN.  Which warp takes which row or tile only decides the order in which integers are added, and the fp32
-// arithmetic of a row depends on k and the row alone, so the epoch is the same bits on every run, at every grid
-// size, CTAs per SM, threads per CTA and SM count.  It is the fp64 model of the row-lane windows with TR = T, grid = B;
-// tests/test_sgd_window_gpu.py holds the kernel to it (DESIGN.md section 3.3).
+// state NaN (nan_state).  These pieces and the cooperative launch are fm_window.cuh's; the stamp table and the
+// launch are shared with the HOGWILD SGDA epoch.  Which warp takes which row or tile only decides the order in which
+// integers are added, and the fp32 arithmetic of a row depends on k and the row alone, so the epoch is the same bits
+// on every run, at every grid size, CTAs per SM, threads per CTA and SM count.  It is the fp64 model of the row-lane
+// windows with TR = T, grid = B, its budget widened for long rows and wide k; tests/test_sgd_window_gpu.py holds the
+// kernel to it (DESIGN.md section 3.3).
 //
 // Exactness: at most S = min(W * max_row_nnz, nnz) steps land on one element per window (at most B on the bias),
 // so a per-step cap of min(2^11, 2^31 / S) keeps every u64 sum below 2^63.
-#include <algorithm>
-
-#include "fm_device.cuh"
-#include "fm_hogwild_common.cuh"
-#include "fmb200_internal.h"
+#include "fm_window.cuh"
 
 namespace fmb {
 
@@ -64,20 +62,6 @@ struct WindowArgs {
 };
 
 constexpr int kWindowProfSlots = 4;  // theta, barrier 1, fold, barrier 2
-
-__device__ __forceinline__ unsigned long long quantise(float d, float cap, unsigned long long* bad) {
-  if (fabsf(d) < cap) return (unsigned long long)__float2ll_rn(d * kAccScale);
-  atomicOr(bad, 1ull);  // also NaN: the comparison is false
-  return 0ull;
-}
-
-// after a divergence: every element of the state NaN, its accumulated steps cleared (the flag stays)
-__device__ __forceinline__ void nan_state(const WindowArgs& a, uint64_t gt, uint64_t GT) {
-  for (uint64_t e = gt; e < a.n_floats; e += GT) {
-    a.state[e] = __int_as_float(0x7fffffff);
-    a.acc[e] = 0ull;
-  }
-}
 
 // window j: its first tile and its tiles (the ramp windows are one tile each)
 __device__ __forceinline__ void window_tiles(const WindowArgs& a, uint32_t j, uint32_t* t0, uint32_t* nt) {
@@ -149,7 +133,6 @@ __device__ void window_row(const WindowArgs& a, uint64_t r, float w0, float conc
     const uint32_t m = min(32u, size - b);
     uint32_t my_id = 0;
     float my_x = 0.f, my_sv = 1.f;
-    bool first = false;
     if ((uint32_t)lane < m) {
       my_id = __ldg(a.col + beg + b + lane);
       my_x = __ldg(a.val + beg + b + lane);
@@ -160,18 +143,10 @@ __device__ void window_row(const WindowArgs& a, uint64_t r, float w0, float conc
         const uint64_t e = a.off_w + (uint64_t)my_id * a.ws;
         const float sw = damped ? gamma_scale(c, lr * (hjoint + a.regw)) : 1.f;
         const float wv = __ldcg(a.state + e);
-        red_add_u64(a.acc + e, quantise(sw * (nlr_mult * my_x + nlr_regw * wv), cap, bad));
+        red_add_u64(a.acc + e, acc_quantise(sw * (nlr_mult * my_x + nlr_regw * wv), bad, cap));
       }
-      first = __ldcg(a.stamp + my_id) != stamp && atomicExch(a.stamp + my_id, stamp) != stamp;
     }
-    // the window's first touches go to its list, one reservation per warp
-    const unsigned fm = __ballot_sync(0xffffffffu, first);
-    if (fm) {
-      unsigned long long base = 0;
-      if (lane == 0) base = atomicAdd(cnt, (unsigned long long)__popc(fm));
-      base = __shfl_sync(0xffffffffu, base, 0);
-      if (first) a.list[base + __popc(fm & ((1u << lane) - 1u))] = my_id;
-    }
+    window_touch(a, stamp, cnt, my_id, (uint32_t)lane < m, lane);
 #pragma unroll 4
     for (uint32_t i = 0; i < m; i++) {
       const uint32_t id = __shfl_sync(0xffffffffu, my_id, i);
@@ -184,7 +159,7 @@ __device__ void window_row(const WindowArgs& a, uint64_t r, float w0, float conc
         if (f < k) {
           const uint64_t e = a.off_v + (uint64_t)id * a.kp + f;
           const float vv = __ldcg(a.state + e);
-          red_add_u64(a.acc + e, quantise(sv * (nlr_mult * (s[j] * x - vv * x2) + nlr_regv * vv), cap, bad));
+          red_add_u64(a.acc + e, acc_quantise(sv * (nlr_mult * (s[j] * x - vv * x2) + nlr_regv * vv), bad, cap));
         }
       }
     }
@@ -201,7 +176,6 @@ __global__ void __launch_bounds__(kWindowMaxThreads, KF == 4 ? 3 : 4) fm_sgd_win
   unsigned long long* flag = a.acc + a.n_floats;
   unsigned long long* accb = a.aux;
   const uint32_t n_win = a.ramp_tiles + (a.n_tiles - a.ramp_tiles + a.B - 1) / a.B;
-  const uint32_t gp = (uint32_t)a.kp / 4, F = gp + 1;  // fold items of a feature: its float4s of V, then w
   float w0 = a.use_w0 ? __ldcg(a.state) : 0.f;
   long long t_prof = clock64();
   unsigned long long s_prof[kWindowProfSlots] = {0ull, 0ull, 0ull, 0ull};
@@ -246,7 +220,7 @@ __global__ void __launch_bounds__(kWindowMaxThreads, KF == 4 ? 3 : 4) fm_sgd_win
         if (lane == 0) {
           M += (float)T * a.reg0 * w0;
           const float gb = gamma_scale(fmaxf(w0c, 1.f), a.lr * (H / (float)T + a.reg0));
-          red_add_u64(accb + (j & 1), quantise(-a.lr * gb * M, a.step_cap, flag));
+          red_add_u64(accb + (j & 1), acc_quantise(-a.lr * gb * M, flag, a.step_cap));
         }
       }
     }
@@ -257,28 +231,7 @@ __global__ void __launch_bounds__(kWindowMaxThreads, KF == 4 ? 3 : 4) fm_sgd_win
     if (bad) {  // a step overflowed: the whole state turns NaN
       nan_state(a, gt, GT);
     } else {
-      const uint64_t n_items = __ldcg(a.aux + 2 + (j & 1)) * F;
-      for (uint64_t t = gt; t < n_items; t += GT) {
-        const uint32_t i = __ldcg(a.list + t / F);
-        const uint32_t c = (uint32_t)(t % F);
-        if (c < gp) {
-          const uint64_t e = a.off_v + (uint64_t)i * a.kp + 4 * c;
-          float4 x = __ldcg(reinterpret_cast<const float4*>(a.state + e));
-          ulonglong2* ap = reinterpret_cast<ulonglong2*>(a.acc + e);
-          const ulonglong2 u0 = __ldcg(ap), u1 = __ldcg(ap + 1);
-          x.x = acc_fold(x.x, u0.x, false);
-          x.y = acc_fold(x.y, u0.y, false);
-          x.z = acc_fold(x.z, u1.x, false);
-          x.w = acc_fold(x.w, u1.y, false);
-          *reinterpret_cast<float4*>(a.state + e) = x;
-          ap[0] = make_ulonglong2(0ull, 0ull);
-          ap[1] = make_ulonglong2(0ull, 0ull);
-        } else if (a.use_w) {
-          const uint64_t e = a.off_w + (uint64_t)i * a.ws;
-          a.state[e] = acc_fold(__ldcg(a.state + e), __ldcg(a.acc + e), false);
-          a.acc[e] = 0ull;
-        }
-      }
+      window_fold(a, __ldcg(a.aux + 2 + (j & 1)), gt, GT);
     }
     mark(2);
     bar.arrive(tid);
@@ -295,13 +248,6 @@ __global__ void __launch_bounds__(kWindowMaxThreads, KF == 4 ? 3 : 4) fm_sgd_win
   }
 }
 
-template <class Body>
-cudaError_t with_kf(int k, Body&& body) {
-  if (k <= 32) return body(std::integral_constant<int, 1>());
-  if (k <= 64) return body(std::integral_constant<int, 2>());
-  return body(std::integral_constant<int, 4>());
-}
-
 }  // namespace
 
 cudaError_t launch_sgd_window(fmb200_ctx* c, DataSlot& d) {
@@ -315,21 +261,7 @@ cudaError_t launch_sgd_window(fmb200_ctx* c, DataSlot& d) {
   const uint64_t n_floats = c->p32.n_floats;
   if (n_floats % 4 != 0 || c->p32.off_v % 4 != 0) return cudaErrorInvalidValue;  // the fold takes float4s
   cudaError_t e;
-  if (!c->d_acc) {
-    if ((e = alloc(c->d_acc, n_floats + 1)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d_acc.get(), 0, (n_floats + 1) * sizeof(unsigned long long), c->stream)) != cudaSuccess)
-      return e;
-  }
-  if (!c->win_stamp) {
-    const uint64_t n1 = std::max<uint64_t>(c->n, 1);
-    if ((e = alloc(c->win_stamp, n1)) != cudaSuccess) return e;
-    if ((e = alloc(c->win_list, n1)) != cudaSuccess) return e;
-    if ((e = alloc(c->win_aux, 4)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->win_stamp.get(), 0, n1 * sizeof(uint32_t), c->stream)) != cudaSuccess) return e;
-    c->win_stamp_next = 1;
-  }
   if ((e = grow(c->win_rows, c->win_rows_cap, std::min(W, N))) != cudaSuccess) return e;
-  if ((e = cudaMemsetAsync(c->win_aux.get(), 0, 4 * sizeof(unsigned long long), c->stream)) != cudaSuccess) return e;
   // The bias ramp of the row-lane epoch: the first epoch after the state was set starts the bias far from its
   // equilibrium, so its first windows are one tile each
   const bool ramp = c->hogwild_fresh && c->k0 && c->tune_damp >= 0 && n_tiles > 8 * kWindowRampTiles;
@@ -355,17 +287,12 @@ cudaError_t launch_sgd_window(fmb200_ctx* c, DataSlot& d) {
   a.ramp_conc_scale = (float)((double)TR / (double)N);
   a.ramp_w0_conc = (float)TR;
   a.state = c->p32.base;
-  a.acc = c->d_acc.get();
   a.n_floats = n_floats;
   a.off_w = c->p32.off_w;
   a.off_v = c->p32.off_v;
   a.ws = c->p32.ws;
   a.kp = c->kp;
   a.k = c->k;
-  a.stamp = c->win_stamp.get();
-  a.stamp0 = c->win_stamp_next;
-  a.list = c->win_list.get();
-  a.aux = c->win_aux.get();
   a.rows = reinterpret_cast<float2*>(c->win_rows.get());
   a.use_w0 = c->k0;
   a.use_w = c->k1;
@@ -378,28 +305,15 @@ cudaError_t launch_sgd_window(fmb200_ctx* c, DataSlot& d) {
   a.min_target = (float)c->hp.min_target;
   a.max_target = (float)c->hp.max_target;
   a.step_cap = (float)std::min((double)kAccStepMax, 2147483648.0 / steps);
-  a.gbar = c->d_gbar.get();
-  a.gbar_base = c->gbar_count;
   PhaseTimers prof;  // fmb200_set_tuning variant 132: phase timers, printed per window
   if (c->tune_variant == 132 && (e = prof.start(kWindowProfSlots, c->stream)) != cudaSuccess) return e;
   a.prof = prof.slots.get();
   const uint32_t n_win = a.ramp_tiles + (uint32_t)((n_tiles - a.ramp_tiles + B - 1) / B);
   const int threads = c->tune_threads > 0 ? std::min(c->tune_threads, kWindowMaxThreads) : kWindowMaxThreads;
-  return with_kf(c->k, [&](auto kf) -> cudaError_t {
-    auto fn = fm_sgd_window_kernel<decltype(kf)::value>;
-    int occ = 0;
-    cudaError_t e_ = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, threads, 0);
+  return with_kf<4>(c->k, [&](auto kf) -> cudaError_t {
+    int grid = 0;
+    cudaError_t e_ = launch_windows(c, fm_sgd_window_kernel<decltype(kf)::value>, a, threads, n_win, 2, &grid);
     if (e_ != cudaSuccess) return e_;
-    if (occ < 1) return cudaErrorInvalidConfiguration;
-    const int per_sm = c->tune_ctas_per_sm > 0 ? std::min(c->tune_ctas_per_sm, occ) : occ;
-    const int grid = c->sm_count * per_sm;
-    // cooperative: the grid barriers need every CTA resident (grid <= occ * SMs by construction)
-    void* args[] = {&a};
-    e_ = cudaLaunchCooperativeKernel((const void*)fn, dim3(grid), dim3(threads), args, 0, c->stream);
-    if (e_ != cudaSuccess) return e_;
-    c->launches++;
-    c->gbar_count += (uint32_t)grid * 2u * n_win;
-    c->win_stamp_next += n_win;
     c->last_cfg = EpochConfig{32, decltype(kf)::value, (int)TR, grid, threads, 0, damp ? 1 : 0, 0};
     if (a.prof) {
       static const char* name[kWindowProfSlots] = {"theta", "barrier1", "fold", "barrier2"};

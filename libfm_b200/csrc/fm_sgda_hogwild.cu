@@ -22,12 +22,10 @@
 // read in the window that holds the epoch's last cursor restart (the epoch's start when there is none).
 // Which warp takes which row only decides the order in which integers are added, so the result is the same
 // bits on every run and at every grid size.  tests/test_sgda_hogwild_gpu.py holds it to an fp64 statement of the
-// windows (DESIGN.md section 3.5).
-#include <algorithm>
-
-#include "fm_device.cuh"
-#include "fm_hogwild_common.cuh"
-#include "fmb200_internal.h"
+// windows (DESIGN.md section 3.5).  The stamp table and the cooperative launch are fm_window.cuh's,
+// shared with the reproducible SGD epoch.  Its windows are short (4096 rows): measured on an H100, the SGD epoch's
+// touched-feature list and fold (window_touch, window_fold) made this epoch 1.1-1.3 ms slower on C2, so it scans.
+#include "fm_window.cuh"
 
 namespace fmb {
 
@@ -58,6 +56,8 @@ struct SgdaHwArgs {
   uint32_t n;
   uint32_t* stamp;  // [n]: the stamp of the last window that named the feature
   uint32_t stamp0;  // stamp of this epoch's window 0
+  uint32_t* list;           // the SGD epoch's list and count words: set by launch_windows, not used here
+  unsigned long long* aux;
   double* reg_w;    // [G]
   double* reg_v;    // [G][k]
   const uint32_t* group;
@@ -75,9 +75,8 @@ struct SgdaHwArgs {
 __device__ __forceinline__ float ldf(const float* p) { return __ldcg(p); }
 __device__ __forceinline__ double ldd(const double* p) { return __ldcg(p); }
 
-// the gradient an accumulated element stores: its sum, or NaN after a divergence
-__device__ __forceinline__ float acc_value(unsigned long long u, bool bad) {
-  if (bad) return __int_as_float(0x7fffffff);
+// the gradient sum an accumulated element stores
+__device__ __forceinline__ float acc_value(unsigned long long u) {
   return (float)((double)(long long)u * (1.0 / (double)kAccScale));
 }
 
@@ -314,7 +313,7 @@ __global__ void __launch_bounds__(kSgdaThreads) fm_sgda_hogwild_kernel(const Sgd
         e = a.off_v + (uint64_t)i * a.kp + f;
       }
       a.state[e] = acc_fold(a.state[e], __ldcg(a.acc + e), bad);
-      a.grad[e] = acc_value(__ldcg(a.gacc + e), bad);
+      a.grad[e] = bad ? __int_as_float(0x7fffffff) : acc_value(__ldcg(a.gacc + e));
       a.acc[e] = 0ull;
       a.gacc[e] = 0ull;
     }
@@ -343,13 +342,6 @@ __global__ void __launch_bounds__(kSgdaThreads) fm_sgda_hogwild_kernel(const Sgd
   }
 }
 
-template <class Body>
-cudaError_t with_kf128(int k, Body&& body) {
-  if (k <= 32) return body(std::integral_constant<int, 1>());
-  if (k <= 64) return body(std::integral_constant<int, 2>());
-  return body(std::integral_constant<int, 4>());
-}
-
 }  // namespace
 
 uint64_t sgda_hogwild_window(const fmb200_ctx* c) {
@@ -363,12 +355,6 @@ cudaError_t launch_sgda_hogwild(fmb200_ctx* c, const DataSlot& tr, const DataSlo
   const bool lam = lambda_steps && V > 0;
   const uint32_t E = c->sgda_groups * (uint32_t)(c->k + 1);
   cudaError_t e;
-  const uint64_t n_floats = c->p32.n_floats;
-  if (!c->d_acc) {
-    if ((e = alloc(c->d_acc, n_floats + 1)) != cudaSuccess) return e;
-    if ((e = cudaMemsetAsync(c->d_acc.get(), 0, (n_floats + 1) * sizeof(unsigned long long), c->stream)) != cudaSuccess)
-      return e;
-  }
   if (lam && (e = grow(c->sgda_part, c->sgda_part_cap, std::min(W, N) * E)) != cudaSuccess) return e;
   SgdaHwArgs a;
   a.row_ptr = tr.row_ptr.get();
@@ -386,17 +372,14 @@ cudaError_t launch_sgda_hogwild(fmb200_ctx* c, const DataSlot& tr, const DataSlo
   a.w0_conc = (float)std::min(W, N);
   a.state = c->p32.base;
   a.grad = c->sgda_grad32.get();
-  a.acc = c->d_acc.get();
   a.gacc = c->sgda_gacc.get();
-  a.n_floats = n_floats;
+  a.n_floats = c->p32.n_floats;
   a.off_w = c->p32.off_w;
   a.off_v = c->p32.off_v;
   a.ws = c->p32.ws;
   a.kp = c->kp;
   a.k = c->k;
   a.n = c->n;
-  a.stamp = c->sgda_stamp.get();
-  a.stamp0 = c->sgda_stamp_next;
   a.reg_w = c->sgda_reg_w.get();
   a.reg_v = c->sgda_reg_v.get();
   a.group = c->sgda_group.get();
@@ -414,24 +397,12 @@ cudaError_t launch_sgda_hogwild(fmb200_ctx* c, const DataSlot& tr, const DataSlo
   a.lr = (float)c->hp.lr;
   a.min_target = (float)c->hp.min_target;
   a.max_target = (float)c->hp.max_target;
-  a.gbar = c->d_gbar.get();
-  a.gbar_base = c->gbar_count;
-  const uint64_t n_win = (N + W - 1) / W;
-  return with_kf128(c->k, [&](auto kf) -> cudaError_t {
-    auto fn = fm_sgda_hogwild_kernel<decltype(kf)::value>;
-    int occ = 0;
-    cudaError_t e_ = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, kSgdaThreads, 0);
+  const uint32_t n_win = (uint32_t)((N + W - 1) / W);
+  return with_kf<4>(c->k, [&](auto kf) -> cudaError_t {
+    int grid = 0;
+    const cudaError_t e_ =
+        launch_windows(c, fm_sgda_hogwild_kernel<decltype(kf)::value>, a, kSgdaThreads, n_win, lam ? 4 : 2, &grid);
     if (e_ != cudaSuccess) return e_;
-    if (occ < 1) return cudaErrorInvalidConfiguration;
-    const int per_sm = c->tune_ctas_per_sm > 0 ? std::min(c->tune_ctas_per_sm, occ) : occ;
-    const int grid = c->sm_count * per_sm;
-    // cooperative: the grid barriers need every CTA resident (grid <= occ * SMs by construction)
-    void* args[] = {&a};
-    e_ = cudaLaunchCooperativeKernel((const void*)fn, dim3(grid), dim3(kSgdaThreads), args, 0, c->stream);
-    if (e_ != cudaSuccess) return e_;
-    c->launches++;
-    c->gbar_count += (uint32_t)grid * (uint32_t)(n_win * (lam ? 4 : 2));
-    c->sgda_stamp_next += (uint32_t)n_win;
     c->last_cfg = EpochConfig{32, 1, (int)std::min<uint64_t>(W, 0x7fffffff), grid, kSgdaThreads, 0, a.damp, 0};
     return cudaGetLastError();
   });

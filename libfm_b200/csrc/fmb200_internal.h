@@ -231,6 +231,17 @@ struct EpochConfig {
 constexpr uint64_t kWindowTileRows = 256, kWindowTiles = 64, kWindowRampTiles = 4;
 constexpr int kWindowMaxTileRows = 1024, kWindowMaxTiles = 65536;
 
+// The bookkeeping of the windowed epochs (fm_window.cuh): the stamps for the reproducible SGD and the HOGWILD SGDA
+// epoch, the list and count words for the SGD epoch.
+// A window's stamp comes from `next`, which only grows, and stamps are only compared for equality with the current
+// window's, so no epoch needs the table reset.
+struct WindowBook {
+  DevPtr<uint32_t> stamp;          // [n]: the stamp of the last window that touched each feature (zero at first)
+  DevPtr<uint32_t> list;           // [n]: the features the running window touched, in no particular order
+  DevPtr<unsigned long long> aux;  // by window parity: [0, 1] the SGD epoch's bias steps, [2, 3] the list's length
+  uint32_t next = 1;               // the stamp of the next launch's window 0
+};
+
 }  // namespace fmb
 
 struct fmb200_ctx {
@@ -255,7 +266,8 @@ struct fmb200_ctx {
   fmb::DevPtr<double> d_pred;  // predict output staging
   uint64_t pred_cap = 0;
   fmb::DevPtr<unsigned int> d_sched;   // hogwild tile scheduler: [next tile, CTAs run dry]
-  fmb::DevPtr<unsigned long long> d_acc;  // fixed-point accumulator of the row-lane epoch (fm_hogwild.cu)
+  fmb::DevPtr<unsigned long long> d_acc;  // the reproducible epochs' fixed-point accumulator (acc_ready)
+  fmb::WindowBook window;                 // the windowed SGD and SGDA epochs' stamps, the SGD epoch's list
   // its dealt schedule: the bias step of a window by window parity [2], then the rows' (mult, hjoint) pairs
   fmb::DevPtr<unsigned long long> d_deal_bias;
   uint64_t deal_bias_cap = 0;  // u64 words
@@ -287,24 +299,17 @@ struct fmb200_ctx {
   fmb::DevPtr<uint32_t> sgda_group;
   uint32_t sgda_groups = 0;
   // HOGWILD SGDA (fm_sgda_hogwild.cu): fp32 stored gradients and their window sums, beside the packed state
-  // element for element; the window stamp of every feature and the next epoch's first stamp; the lambda-steps'
-  // per-group terms of a window [W][groups * (k + 1)]
+  // element for element; the lambda-steps' per-group terms of a window [W][groups * (k + 1)]
   fmb::DevPtr<float> sgda_grad32;
   fmb::DevPtr<unsigned long long> sgda_gacc;
-  fmb::DevPtr<uint32_t> sgda_stamp;
-  uint32_t sgda_stamp_next = 1;
   fmb::DevPtr<double> sgda_part;
   uint64_t sgda_part_cap = 0;
   int tune_damp = 0;  // 0 auto, 1 force on, -1 force off
   int tune_variant = 0;  // 0 auto, 1 row-group kernel, 2 row-lane kernel when eligible
   // the reproducible HOGWILD SGD epoch (fmb200_set_reproducible, fm_sgd_window.cu): on, its tile and window
-  // geometry; every feature's window stamp and the next epoch's first stamp, a window's touched features, its
-  // bias accumulators and list lengths, its rows' (mult, h_joint)
+  // geometry, a window's rows' (mult, h_joint)
   bool win_on = false;
   int win_tile_rows = (int)fmb::kWindowTileRows, win_tiles = (int)fmb::kWindowTiles;
-  fmb::DevPtr<uint32_t> win_stamp, win_list;
-  uint32_t win_stamp_next = 1;
-  fmb::DevPtr<unsigned long long> win_aux;
   fmb::DevPtr<float2> win_rows;
   uint64_t win_rows_cap = 0;
   std::unique_ptr<fmb::McmcState, fmb::McmcDelete> mcmc;  // MCMC / ALS learner state (fm_mcmc.cu)
@@ -385,7 +390,10 @@ cudaError_t launch_sgda_hogwild(fmb200_ctx* c, const DataSlot& tr, const DataSlo
 cudaError_t launch_sgd_hogwild(fmb200_ctx* c, DataSlot& d);
 // fm_sgd_window.cu: the reproducible HOGWILD SGD epoch, windows of win_tiles tiles of win_tile_rows rows
 cudaError_t launch_sgd_window(fmb200_ctx* c, DataSlot& d);
-// fm_hogwild.cu: a fresh state clears the divergence flag of the row-lane epoch's accumulator
+// fm_hogwild.cu: the fixed-point accumulator of the reproducible epochs (row-lane, windowed SGD, SGDA), zeroed on
+// first use: *steps := its n_floats step words, *flag (when not null) := the divergence flag behind them
+cudaError_t acc_ready(fmb200_ctx* c, unsigned long long** steps, unsigned long long** flag);
+// fm_hogwild.cu: a fresh state clears the accumulator's divergence flag
 cudaError_t clear_acc_flag(fmb200_ctx* c);
 // fm_hogwild.cu: build the dealt copy the row-lane epoch would run on this data set, if it would deal
 cudaError_t prepare_rowlane_deal(fmb200_ctx* c, DataSlot& d);
@@ -467,6 +475,20 @@ constexpr int row_class_ctas(int R, int U) { return R * U <= 4 ? 3 : (R > 20 ? 1
 // exist for every G of pick_geometry and every power of two S <= 8 with G * S <= 32.
 template <int V>
 using Int = std::integral_constant<int, V>;
+
+// Factors per lane of a warp whose lane l owns factors l, l + 32, ...: body(Int<KF>{}) for the smallest KF in
+// {1, 2, 4, 8} with 32 * KF >= k, up to MAX_KF (4 or 8); cudaErrorInvalidValue when k > 32 * MAX_KF
+template <int MAX_KF, class Body>
+cudaError_t with_kf(int k, Body&& body) {
+  static_assert(MAX_KF == 4 || MAX_KF == 8, "KF is 1, 2, 4 or 8");
+  if (k > 32 * MAX_KF) return cudaErrorInvalidValue;
+  if (k <= 32) return body(Int<1>{});
+  if (k <= 64) return body(Int<2>{});
+  if constexpr (MAX_KF == 8) {
+    if (k > 128) return body(Int<8>{});
+  }
+  return body(Int<4>{});
+}
 template <int G, class F>
 auto dispatch_s(int S, F& f) {
   if constexpr (G <= 4) {

@@ -33,8 +33,8 @@ EPS_M = 2e-6      # relative error of a step's fp32 products and of a tile's fp3
 EPS_GAMMA = 2e-4  # relative error of gamma: the exponent c log(1 - u) carries c times the error of __logf
 KAPPA = 0.1       # feed-forward of earlier windows' differences, per window
 GAMMA_CUT_JUMP = 5e-4  # gamma drops from 1 to 1 - q/2 at its q < 1e-3 cut; fp32 may put c u on the other side
-# The windowed epochs' warp-per-row score (tests/window_model.py, oracle/sgda_window_model.py): each lane adds
-# n ceil(k / 32) terms in sequence, then a shuffle tree; the row-lane calibration above never saw such rows.
+# The windowed epochs' warp-per-row score (rowlane_epoch_model's eps_seq, oracle/sgda_window_model.py): each lane
+# adds n ceil(k / 32) terms in sequence, then a shuffle tree; the row-lane calibration above never saw such rows.
 EPS_SEQ = 2.0 ** -22  # error of an fp32 sum per term it adds in sequence, relative to the terms' magnitudes
 SEQ_EXTRA = 6         # the shuffle tree over 32 lanes (5 levels) and the bias add
 
@@ -162,9 +162,22 @@ def _exact_sums(idx, q, n):
 
 
 def rowlane_epoch_model(state: State, data, hp: HParams, TR: int, grid: int, damp: bool, ramp_tiles: int,
-                        budget: Budget | None = None):
+                        budget: Budget | None = None, eps_seq: float = 0.0):
     """One epoch over `data` (row_ptr, col, val, target) in tiles of TR rows and windows of `grid` tiles.
-    Returns (state, budget); pass the budget of the previous epoch to carry it on."""
+    Returns (state, budget); pass the budget of the previous epoch to carry it on.
+
+    It is also the windowed HOGWILD SGD epoch (fmb200_set_reproducible, fm_sgd_window.cu) with TR = its tile rows
+    and grid = its window tiles.  eps_seq > 0 (EPS_SEQ) adds to the budget a term for what the row-lane calibration
+    did not cover there: rows of tens of entries and k up to 128.  A warp scores a row with its lanes over factors,
+    each lane summing n * ceil(k / 32) terms in sequence before a 5-level shuffle tree, so with
+    L = eps_seq (n ceil(k / 32) + SEQ_EXTRA)
+
+        the score carries      L (|w0| + sum_i |w_i x_i| + sum_f (sum_i |v_if x_i|)^2 + sum_i,f (v_if x_i)^2) more,
+        each per-factor sum    L sum_i |v_if x_i|,
+        h_row (damped steps)   L (xx + 3 |xx - 2| sum_f (sum_i |v_if x_i|)^2 + sq) relative to h_row,
+
+    as oracle/rowgroup_model.py bounds its sub-warp rows with EPS_S = 2^-22.  The term widens the budget and never
+    changes the state; eps_seq = 0 leaves it out."""
     n = state.w.shape[0]
     k = state.v.shape[0]
     N = int(data.row_ptr.shape[0] - 1)
@@ -176,6 +189,7 @@ def rowlane_epoch_model(state: State, data, hp: HParams, TR: int, grid: int, dam
     count = np.bincount(col, minlength=n).astype(np.float32)
     n_tiles = (N + TR - 1) // TR
     lr = hp.lr
+    lanes_seq = -(-k // 32)  # factors per lane of the windowed epoch's warp
 
     st = state.copy()
     bud = Budget.zero(st) if budget is None else Budget(budget.w0, budget.w.copy(), budget.v.copy(), budget.windows)
@@ -205,6 +219,15 @@ def rowlane_epoch_model(state: State, data, hp: HParams, TR: int, grid: int, dam
         xx = np.bincount(er, weights=x * x, minlength=R)
         hrow, hjoint = row_curvature(hp, curv, xx, s2, sq, damp)
         row_err = EPS_P * (1.0 + np.abs(p)) + EPS_M * np.abs(mult)
+        if eps_seq:  # the lanes' sequences (L of the notes above, per row)
+            L = eps_seq * (np.diff(rp[r0:r1 + 1]).astype(np.float64) * lanes_seq + SEQ_EXTRA)
+            abs_s = np.stack([np.bincount(er, weights=np.abs(vx[f]), minlength=R) for f in range(k)]) if k \
+                else np.zeros((0, R))
+            abs_s2 = (abs_s * abs_s).sum(0)
+            row_err = row_err + L * ((abs(st.w0) if hp.k0 else 0.0) +
+                                     np.bincount(er, weights=np.abs(wv * x), minlength=R) + abs_s2 + sq)
+            rel_h = np.minimum(1.0, L * (xx + 3.0 * np.abs(xx - 2.0) * abs_s2 + sq) / np.maximum(hrow, 1e-300)) \
+                * (hrow > 0)
 
         # ---- per entry: concurrency, damping, steps ----
         c = (count[ids] * conc_scale).astype(np.float64)
@@ -218,6 +241,8 @@ def rowlane_epoch_model(state: State, data, hp: HParams, TR: int, grid: int, dam
         cut_w = damped * gamma_cut_edge(c, lr * (hjoint[er] + hp.regw))
         bv = sv * (lr * np.abs(grad) * row_err[er] + EPS_M * lr * hp.regv * np.abs(vv)) + 1.0 / ACC_SCALE \
             + np.abs(dv) * (EPS_GAMMA * damped + cut_v + edge[er])
+        if eps_seq:
+            bv = bv + sv * lr * np.abs(mult[er] * x) * (L * abs_s)[:, er] + np.abs(dv) * damped * rel_h[er]
         for f in range(k):
             st.v[f] = fold(st.v[f], _exact_sums(ids, quantise(dv[f]), n))
             bud.v[f] += grow * np.bincount(ids, weights=bv[f], minlength=n)
@@ -225,6 +250,8 @@ def rowlane_epoch_model(state: State, data, hp: HParams, TR: int, grid: int, dam
             dw = sw * (-lr * mult[er] * x - lr * hp.regw * wv)
             bw = sw * (lr * np.abs(x) * row_err[er] + EPS_M * lr * hp.regw * np.abs(wv)) + 1.0 / ACC_SCALE \
                 + np.abs(dw) * (EPS_GAMMA * damped + cut_w + edge[er])
+            if eps_seq:
+                bw = bw + np.abs(dw) * damped * rel_h[er]
             st.w = fold(st.w, _exact_sums(ids, quantise(dw), n))
             bud.w += grow * np.bincount(ids, weights=bw, minlength=n)
 

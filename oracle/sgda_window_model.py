@@ -24,8 +24,8 @@ With W = 1, no damping, no quantisation and fp64 state this is the reference's S
 row-lane model's per-element budget (rowlane_model.Budget; the same constants) with two more terms: the steps a
 difference in reg moves (2 lr |reg - reg'| |theta|) and, for reg itself, REG_REL of every lambda contribution.
 
-eps_seq > 0 (EPS_SEQ) adds the term tests/window_model.py states for the windowed SGD epoch's warp-per-row score,
-which the row-lane calibration never saw: a lane adds n ceil(k / 32) terms in sequence before a 5-level shuffle
+eps_seq > 0 (EPS_SEQ) adds the term rowlane_epoch_model's eps_seq states for the windowed SGD epoch's warp-per-row
+score, which the row-lane calibration never saw: a lane adds n ceil(k / 32) terms in sequence before a 5-level shuffle
 tree, so with L = eps_seq (n ceil(k / 32) + SEQ_EXTRA) the score carries scale L (|w0| + sum_i |w_i x_i| +
 sum_f (sum_i |v_if x_i|)^2 + sum_i,f (v_if x_i)^2) more, each per-factor sum s_f (and so each V gradient) L sum_i
 |v_if x_i|, and h_row, which damped steps read, L (xx + 3 |xx - 2| sum_f (sum_i |v_if x_i|)^2 + sq) relative.  Only

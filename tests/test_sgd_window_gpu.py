@@ -1,17 +1,17 @@
 """GPU: the reproducible HOGWILD SGD epoch (fmb200_set_reproducible, fm_sgd_window.cu).
 
 The windowed epoch is oracle/rowlane_model.py's rowlane_epoch_model with TR = the tile rows and grid = the window
-tiles, at any k <= 128 and any row length; tests/window_model.py restates it with a budget widened for long rows
-and wide k.  After every epoch each parameter must lie within that budget plus one fp32 ulp, and each of w0, w and v
-within a small relative distance of what the run moved it.  The same bits on every run, grid, CTAs per SM and
+tiles, at any k <= 128 and any row length, with its budget widened for long rows and wide k (eps_seq = EPS_SEQ).
+After every epoch each parameter must lie within that budget plus one fp32 ulp, and each of w0, w and v within a
+small relative distance of what the run moved it.  The same bits on every run, grid, CTAs per SM and
 threads per CTA; a held-out RMSE at C3 shape as close to the sequential oracle's as the free-running kernel's.
 """
 import numpy as np
 import pytest
 
 from libfm_b200 import Data, FmError, FmLearnSgdElement, FmModel, MODE_HOGWILD, synth
-from oracle import HParams, Port, State
-from window_model import window_epoch_model
+from oracle import HParams, Port, State, rowlane_epoch_model
+from oracle.rowlane_model import EPS_SEQ
 
 pytestmark = pytest.mark.gpu
 
@@ -58,7 +58,8 @@ def run_case(name, d, k, T, B, task=0, regs=(0.0, 0.0, 0.0), k0=True, k1=True, d
             cfg = l.epoch_config()
             assert cfg["rows_per_tile"] == T and cfg["lanes_per_row"] == 32, "the windowed epoch did not run"
             ramp = RAMP_TILES if e == 0 and k0 and damp >= 0 and n_tiles > 8 * RAMP_TILES else 0
-            want, bud = window_epoch_model(want, d, hp, T, B, bool(cfg["damp"]), ramp, budget=bud)
+            want, bud = rowlane_epoch_model(want, d, hp, TR=T, grid=B, damp=bool(cfg["damp"]), ramp_tiles=ramp,
+                                            budget=bud, eps_seq=EPS_SEQ)
             got = _pull(l)
             b0, bw, bv = bud.bound(want)
             ratio = max(abs(got.w0 - want.w0) / b0, np.max(np.abs(got.w - want.w) / bw),

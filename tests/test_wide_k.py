@@ -6,9 +6,10 @@ over 3 attribute groups, the MCMC e-terms, and 4 iterations of MCMC and of ALS. 
 fm_oracle_sgda.c) must reproduce every SGD, SGDA and e-term record bit for bit; that makes it a valid yardstick for
 tests/test_wide_k_gpu.py at those widths, which also replays the MCMC / ALS records on the GPU.
 
-The second half restates the kernels' width classes -- `with_kf` (fm_inorder.cu: KF factors per lane of the
-one-warp kernels) and `ordered_shape` (fm_ordered.cu: GL lanes x KF consecutive factors per example) -- and checks
-that GPU_WIDTHS reaches every class with odd and even k, a partially filled and an empty factor slot.
+The second half restates the kernels' width classes -- `with_kf` (fmb200_internal.h: KF factors per lane of
+fm_inorder.cu's one-warp kernels) and `ordered_shape` (fm_ordered.cu: GL lanes x KF consecutive factors per
+example) -- and checks that GPU_WIDTHS reaches every class with odd and even k, a partially filled and an empty
+factor slot.
 """
 import hashlib
 import os
@@ -184,7 +185,7 @@ def test_mcmc_records_are_complete(wide):
 # ---- the kernels' width classes -------------------------------------------------------------------------------
 
 def with_kf(k):
-    """fm_inorder.cu::with_kf: factors per lane of the one-warp kernels (lane l owns l, l + 32, ...)"""
+    """with_kf<8> (fmb200_internal.h): factors per lane of the one-warp kernels (lane l owns l, l + 32, ...)"""
     assert 0 <= k <= 256
     kf = (k + 31) // 32
     return 1 if kf <= 1 else 2 if kf <= 2 else 4 if kf <= 4 else 8

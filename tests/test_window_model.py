@@ -1,12 +1,12 @@
-"""CPU: tests/window_model.py, the model of the windowed HOGWILD SGD epoch.  With eps_seq = 0 it computes what
-oracle/rowlane_model.py's rowlane_epoch_model computes, state and budget bit for bit; its sequence term widens the
-budget and never changes the state; a one-row window checked by hand shows what the term adds."""
+"""CPU: the model of the windowed HOGWILD SGD epoch, oracle/rowlane_model.py's rowlane_epoch_model with the budget's
+sequence term (eps_seq).  The term widens the budget and never changes the state; a one-row window checked by hand
+shows what the term adds."""
 import numpy as np
 import pytest
 
 from libfm_b200 import Data, synth
 from oracle import HParams, State, rowlane_epoch_model
-from window_model import EPS_SEQ, SEQ_EXTRA, window_epoch_model
+from oracle.rowlane_model import EPS_SEQ, SEQ_EXTRA
 
 
 def _state(n, k, seed):
@@ -22,23 +22,21 @@ def _same(a, b):
 
 @pytest.mark.parametrize("k,task,damp,ramp,k0,k1", [(5, 0, True, 4, True, True), (40, 0, False, 0, True, False),
                                                      (3, 1, True, 0, False, True)])
-def test_without_the_term_it_is_the_row_lane_model(k, task, damp, ramp, k0, k1):
+def test_the_term_widens_the_budget_only(k, task, damp, ramp, k0, k1):
     d = synth.ragged(3000, 200, 12, seed=4)
     if task == 1:
         d = Data(d.row_ptr, d.col, d.val, np.where(d.target > 3, 1.0, -1.0), d.num_feature)
     hp = HParams(task, 0.01, 0.01, 0.02, 0.03, float(d.target.min()), float(d.target.max()), k0, k1)
     st = _state(200, k, 1)
     a, ba = rowlane_epoch_model(st, d, hp, TR=32, grid=4, damp=damp, ramp_tiles=ramp)
-    b, bb = window_epoch_model(st, d, hp, T=32, B=4, damp=damp, ramp_tiles=ramp, eps_seq=0.0)
-    assert _same(a, b) and _same(ba, bb) and ba.windows == bb.windows
+    c, bc = rowlane_epoch_model(st, d, hp, TR=32, grid=4, damp=damp, ramp_tiles=ramp, eps_seq=EPS_SEQ)
+    assert _same(a, c) and ba.windows == bc.windows
+    assert bc.w0 >= ba.w0 and np.all(bc.w >= ba.w) and np.all(bc.v >= ba.v) and np.any(bc.v > ba.v)
     # a second epoch carries the budget on alike
     a2, ba2 = rowlane_epoch_model(a, d, hp, TR=32, grid=4, damp=damp, ramp_tiles=0, budget=ba)
-    b2, bb2 = window_epoch_model(b, d, hp, T=32, B=4, damp=damp, ramp_tiles=0, budget=bb, eps_seq=0.0)
-    assert _same(a2, b2) and _same(ba2, bb2)
-    # the term widens the budget, never the state
-    c, bc = window_epoch_model(st, d, hp, T=32, B=4, damp=damp, ramp_tiles=ramp)
-    assert _same(a, c)
-    assert bc.w0 >= ba.w0 and np.all(bc.w >= ba.w) and np.all(bc.v >= ba.v) and np.any(bc.v > ba.v)
+    c2, bc2 = rowlane_epoch_model(c, d, hp, TR=32, grid=4, damp=damp, ramp_tiles=0, budget=bc, eps_seq=EPS_SEQ)
+    assert _same(a2, c2)
+    assert bc2.w0 >= ba2.w0 and np.all(bc2.w >= ba2.w) and np.all(bc2.v >= ba2.v)
 
 
 def test_one_row_by_hand():
@@ -50,8 +48,8 @@ def test_one_row_by_hand():
              np.array([1.0], np.float32), 2)
     hp = HParams(0, 0.1, min_target=0.0, max_target=5.0, k0=False, k1=False)
     st = State(0.0, np.zeros(2), np.array([[0.5, 0.25]]))
-    _, b0 = window_epoch_model(st, d, hp, T=1, B=1, damp=False, ramp_tiles=0, eps_seq=0.0)
-    _, b1 = window_epoch_model(st, d, hp, T=1, B=1, damp=False, ramp_tiles=0)
+    _, b0 = rowlane_epoch_model(st, d, hp, TR=1, grid=1, damp=False, ramp_tiles=0)
+    _, b1 = rowlane_epoch_model(st, d, hp, TR=1, grid=1, damp=False, ramp_tiles=0, eps_seq=EPS_SEQ)
     L = EPS_SEQ * (2 + SEQ_EXTRA)
     lr, mult = 0.1, 0.75
     grad = np.array([1.0 * 1 - 0.5 * 1, 1.0 * 2 - 0.25 * 4])  # s x - v x^2
@@ -70,8 +68,8 @@ def test_wide_rows_count_each_lanes_factors():
     extra = {}
     for k in (32, 64):
         st = State(0.0, np.zeros(3), r.uniform(0.1, 0.2, (k, 3)).round(6))
-        _, b0 = window_epoch_model(st, d, hp, T=1, B=1, damp=False, ramp_tiles=0, eps_seq=0.0)
-        _, b1 = window_epoch_model(st, d, hp, T=1, B=1, damp=False, ramp_tiles=0, eps_seq=1.0)
+        _, b0 = rowlane_epoch_model(st, d, hp, TR=1, grid=1, damp=False, ramp_tiles=0)
+        _, b1 = rowlane_epoch_model(st, d, hp, TR=1, grid=1, damp=False, ramp_tiles=0, eps_seq=1.0)
         # the per-factor-sum term of factor 0, entry 0: lr |mult x| L s_abs_0, with L = 3 * lanes + SEQ_EXTRA
         extra[k] = (b1.v[0, 0] - b0.v[0, 0])
     assert extra[32] > 0 and extra[64] > extra[32]
