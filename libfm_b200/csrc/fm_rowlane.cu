@@ -135,8 +135,9 @@ __device__ __forceinline__ void rowlane_tile(const HogwildArgs& a, const uint64_
     x[e] = on ? xs[beg + e] : 0.f;
   }
   // DEALT: the row's last entry is its key entry.  The deal sorts a window's rows by its id, so the lanes of
-  // a warp whose rows share the key form a run; `seg` is the run's first lane.  That lane alone gathers the
-  // key's parameters and hands them to the run, and it issues the run's summed steps after the scores.
+  // a warp whose rows share the key form a run; `seg` is the run's first lane, which issues the run's summed
+  // steps after the scores.  Every lane gathers the key itself, as in file order: the run's lanes load the
+  // same sector, which the warp's load instruction requests from L2 once.
   const int kq = DEALT ? cnt - 1 : -1;  // the key entry (-1: none)
   uint32_t kid = 0xffffffffu;
 #pragma unroll
@@ -152,23 +153,9 @@ __device__ __forceinline__ void rowlane_tile(const HogwildArgs& a, const uint64_
   for (int e = 0; e < Z; ++e) {
     // a missing entry (ragged rows) fetches nothing: an unconditional gather of feature 0's sector would add
     // L2 loads on a line the rows that really contain feature 0 are reducing into
-    const bool fetch = e < cnt && e != kq;
+    const bool fetch = e < cnt;
     vr[e] = gather_row<GP>(V4, fetch ? id[e] : 0xffffffffu, odd);
     wv[e] = (use_w && fetch) ? ld_cg_f(a.w + (size_t)id[e] * a.ws) : 0.f;
-  }
-  if (DEALT) {
-    const bool fetch = lane == seg && kid != 0xffffffffu;
-    FactorRow<GP> kv = gather_row<GP>(V4, fetch ? kid : 0xffffffffu, odd);
-    float kw = (use_w && fetch) ? ld_cg_f(a.w + (size_t)kid * a.ws) : 0.f;
-#pragma unroll
-    for (int f = 0; f < K; ++f) kv.v[f] = __shfl_sync(0xffffffffu, kv.v[f], seg);
-    kw = __shfl_sync(0xffffffffu, kw, seg);
-#pragma unroll
-    for (int e = 0; e < Z; ++e)
-      if (e == kq) {
-        vr[e] = kv;
-        wv[e] = kw;
-      }
   }
 
   // ---- fm_model::predict in registers (fm_model.h:105-127) ----
