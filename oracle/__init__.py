@@ -11,6 +11,8 @@ reference legs may import this package.  Three checkers:
                                       epoch's windows (rowlane_model.py)
   rowgroup_epoch_model                fp64 numpy model of the free-running row-group HOGWILD epoch on
                                       data whose result no schedule can change (rowgroup_model.py)
+  peer_model                          fp64 model of the per-epoch peer exchange: the mean and the
+                                      mean-field combine with a per-element budget (peer_model.py)
 """
 from .binding import Port, Ref, build, have_ref  # noqa: F401
 from .rowgroup_model import concurrency, geometry, row_scores, rowgroup_epoch_model  # noqa: F401
